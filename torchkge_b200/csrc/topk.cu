@@ -10,6 +10,8 @@
 //
 // Order: scores descending, NaN above everything (as torch.topk / sort(descending=True) treat it),
 // exact ties by ascending candidate id (the reference leaves the order among ties unspecified).
+// The order is that of the score's bits (score_key): +0.0 ranks above -0.0 although they compare
+// equal, so that the returned score keeps its sign bit.
 #include "kernels.h"
 
 namespace kge {

@@ -8,7 +8,8 @@ current k-th best, one chunk of candidate rows at a time, and a merge kernel kee
 k (score, id) pairs per query -- no (rows x candidates) score matrix exists.  Known facts are masked
 with -inf exactly as ``filter_scores(..., true_idx=None)`` does (utils/modeling.py:76-102); results
 are sorted descending as the reference's ``sort(descending=True)[:, :k]`` (the ORDER among exactly
-tied scores is unspecified there; here: ascending candidate id).
+tied scores is unspecified there; here: ascending candidate id, except that +0.0 ranks above -0.0
+-- the returned scores keep their sign bit).
 
 Deviation, on purpose: the reference stores the scores with ``self.scores[i * b_size, (i + 1) *
 b_size] = ...`` (inference.py:151, 246) -- an index pair instead of a slice, which raises
