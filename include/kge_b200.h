@@ -39,7 +39,7 @@
 extern "C" {
 #endif
 
-#define KGE_ABI_VERSION 8
+#define KGE_ABI_VERSION 9
 
 /* error codes */
 #define KGE_OK 0
@@ -276,7 +276,10 @@ int kge_score_all(const kge_score_all_args_t* args);
  * sort(descending=True)[:, :k] -- without an (n, n_rows) score matrix: the dense scan runs in a
  * collect mode that writes out only candidates not below the query's current k-th best, a chunk of
  * candidate rows at a time, merged into a per-query sorted list after every chunk.  NaN ranks above
- * everything (as in torch's sort); exact ties are ordered by ascending candidate id. */
+ * everything (as in torch's sort); exact ties are ordered by ascending candidate id.
+ * With a range-partitioned table, `packed` holds the rows [ent_lo, ent_lo + n_rows): pred holds
+ * global ids (ent_lo + row), the mask CSR lists global ids, and kge_topk_merge combines the lists of
+ * the shards into the unsharded result. */
 typedef struct {
   int32_t model, side, dim, k;   /* 1 <= k <= 1024, k <= n_rows */
   int64_t n;                     /* queries */
@@ -294,9 +297,18 @@ typedef struct {
   void* workspace;               /* kge_topk_workspace_bytes() bytes, 256-B aligned */
   size_t workspace_bytes;
   void* stream;
+  int64_t ent_lo;                /* global id of row 0 of `packed` (0: unsharded); ent_lo + n_rows < 2^31 */
 } kge_topk_args_t;
 size_t kge_topk_workspace_bytes(int model, int side, int dim, int64_t n, int64_t n_rows, int k);
 int kge_topk_side(const kge_topk_args_t* args);
+/* pred[i][0..k) / scores[i][0..k): the k best entries of the union of n_lists lists
+ * pred_in / scores_in [n_lists][n][k_in], each sorted best first as kge_topk_side returns them, pred = -1
+ * marking an empty slot (at the end of a list).  Same order as kge_topk_side: score bits (NaN on top,
+ * +0.0 above -0.0), then ascending id; empty slots last, output as (-1, -inf).  Ids must be unique
+ * across the lists (disjoint shards), which makes the result that of one unsharded call.
+ * 1 <= n_lists <= 64, 1 <= k, k_in <= 1024; anything else returns KGE_ERR_ARG. */
+int kge_topk_merge(const int64_t* pred_in, const float* scores_in, int n_lists, int64_t n, int k_in, int k,
+                   int64_t* pred, float* scores, void* stream);
 
 /* ---- dense side paths -----------------------------------------------------------------------
  * RESCAL relation prediction (models/bilinear.py:115-121): the candidates are the relation matrices,

@@ -15,7 +15,7 @@ LIB_PATH = os.path.join(HERE, "lib", "libkge_b200.so")
 TRANSE_L1, TRANSE_L2, DISTMULT, RESCAL, COMPLEX, ROTATE, TORUSE_L1, TORUSE_L2, ANALOGY = range(9)
 SIDE_TAIL, SIDE_HEAD, SIDE_REL = 0, 1, 2
 TILE_C, TILE_Q = 128, 64
-ABI_VERSION = 8
+ABI_VERSION = 9
 FLAG_TENSOR_CORE = 1
 FLAG_APPROX_SCAN = 2
 LOSS_LOGISTIC, LOSS_BCE = 1, 2
@@ -66,6 +66,7 @@ class TopkArgs(ctypes.Structure):
         ("packed", _p), ("rel0", _p), ("rel1", _p), ("hrows", _p), ("trows", _p), ("r_idx", _p),
         ("mask_offs", _p), ("mask_ids", _p), ("pred", _p), ("scores", _p),
         ("workspace", _p), ("workspace_bytes", _c.c_size_t), ("stream", _p),
+        ("ent_lo", _c.c_int64),
     ]
 
 
@@ -119,6 +120,7 @@ SIGNATURES = {
     "kge_score_all": (_c.c_int, [_c.POINTER(ScoreAllArgs)]),
     "kge_topk_workspace_bytes": (_c.c_size_t, [_c.c_int, _c.c_int, _c.c_int, _c.c_int64, _c.c_int64, _c.c_int]),
     "kge_topk_side": (_c.c_int, [_c.POINTER(TopkArgs)]),
+    "kge_topk_merge": (_c.c_int, [_p, _p, _c.c_int, _c.c_int64, _c.c_int, _c.c_int, _p, _p, _p]),
     "kge_rescal_rel_scores": (_c.c_int, [_p, _p, _p, _c.c_int, _c.c_int64, _c.c_int64, _p, _p]),
     "kge_rank_dense": (_c.c_int, [_p, _c.c_int64, _c.c_int64, _p, _p, _p, _p, _p, _p, _p, _p]),
     "kge_topk_dense_workspace_bytes": (_c.c_size_t, [_c.c_int64, _c.c_int64, _c.c_int]),

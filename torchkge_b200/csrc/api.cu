@@ -638,6 +638,9 @@ int kge_topk_side(const kge_topk_args_t* a) {
   if (a->k < 1 || a->k > kge::TOPK_MAX_K) return fail(KGE_ERR_ARG, "kge_topk_side: k must be in [1, 1024]");
   if (a->n < 0 || a->n_rows < 0 || a->dim < 1) return fail(KGE_ERR_ARG, "kge_topk_side: bad sizes");
   if ((int64_t)a->k > a->n_rows) return fail(KGE_ERR_ARG, "kge_topk_side: k exceeds the number of candidates");
+  // candidate ids travel as int32 through the collect lists and the 64-bit keys
+  if (a->ent_lo < 0 || a->ent_lo + a->n_rows > (int64_t)INT32_MAX)
+    return fail(KGE_ERR_ARG, "kge_topk_side: ent_lo + n_rows must lie in [0, 2^31 - 1]");
   if (a->n == 0) return KGE_OK;
   const bool rel_side = a->side == KGE_SIDE_REL;
   if (!a->packed || (!a->rel0 && !rel_side) || !a->hrows || !a->trows || !a->pred || !a->scores || !a->workspace)
@@ -669,7 +672,7 @@ int kge_topk_side(const kge_topk_args_t* a) {
     p.counts = nullptr; p.scores = nullptr;
     p.amb_count = nullptr; p.amb_pairs = nullptr; p.amb_cap = 0; p.rel_eps = 0.f; p.abs_eps = 0.f;
     p.col_buf = t.col_buf; p.col_count = t.col_count; p.col_cap = (unsigned long long)t.chunk_rows;
-    p.col_id_base = c0; p.col_dense = first ? 1 : 0;
+    p.col_id_base = a->ent_lo + c0; p.col_dense = first ? 1 : 0;
     p.dim = a->dim; p.n_q = a->n; p.n_rows = rows;
     p.n_ct = (rows + kge::TILE_C - 1) / kge::TILE_C; p.n_qt = n_qt;
     KGE_CUDA_TRY(timed_scan(el, hs->s.has_cascade, p, st), "topk: collect scan");
@@ -678,6 +681,22 @@ int kge_topk_side(const kge_topk_args_t* a) {
                  "topk: merge");
   }
   KGE_CUDA_TRY(kge::launch_topk_finish(t.best, a->k, a->n, a->pred, a->scores, st), "topk: finish");
+  return KGE_OK;
+}
+
+int kge_topk_merge(const int64_t* pred_in, const float* scores_in, int n_lists, int64_t n, int k_in, int k,
+                   int64_t* pred, float* scores, void* stream) {
+  if (n_lists < 1 || n_lists > kge::TOPK_MAX_LISTS)
+    return fail(KGE_ERR_ARG, "kge_topk_merge: n_lists must be in [1, 64]");
+  if (k < 1 || k > kge::TOPK_MAX_K) return fail(KGE_ERR_ARG, "kge_topk_merge: k must be in [1, 1024]");
+  if (k_in < 1 || k_in > kge::TOPK_MAX_K) return fail(KGE_ERR_ARG, "kge_topk_merge: k_in must be in [1, 1024]");
+  if (n < 0) return fail(KGE_ERR_ARG, "kge_topk_merge: bad sizes");
+  if (n == 0) return KGE_OK;
+  if (!pred_in || !scores_in || !pred || !scores) return fail(KGE_ERR_ARG, "kge_topk_merge: null pointer");
+  DeviceScope device_scope(pred);
+  KGE_CUDA_TRY(kge::launch_topk_lists_merge(pred_in, scores_in, n_lists, n, k_in, k, pred, scores,
+                                            static_cast<cudaStream_t>(stream)),
+               "topk_merge");
   return KGE_OK;
 }
 

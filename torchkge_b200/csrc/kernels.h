@@ -116,6 +116,11 @@ cudaError_t launch_topk_merge(unsigned long long* best, int k, const int2* col_b
 cudaError_t launch_topk_finish(const unsigned long long* best, int k, int64_t n_q, int64_t* pred,
                                float* scores, cudaStream_t stream);
 constexpr int TOPK_MAX_K = 1024;
+constexpr int TOPK_MAX_LISTS = 64;
+// pred[q][0..k) / scores[q][0..k): the k best entries of the union of n_lists sorted lists
+// pred_in / scores_in [n_lists][n][k_in] (same key order as above; pred < 0 marks an empty slot)
+cudaError_t launch_topk_lists_merge(const int64_t* pred_in, const float* scores_in, int n_lists, int64_t n,
+                                    int k_in, int k, int64_t* pred, float* scores, cudaStream_t stream);
 
 // ---- dense side paths (dense.cu) ----
 // scores[i][c] = ((h_i^T M_c) * t_i).sum()   RESCAL relation case, bilinear.py:115-121

@@ -12,6 +12,11 @@
 // exact ties by ascending candidate id (the reference leaves the order among ties unspecified).
 // The order is that of the score's bits (score_key): +0.0 ranks above -0.0 although they compare
 // equal, so that the returned score keeps its sign bit.
+//
+// Ids are global: a scan over a shard of rows [ent_lo, ent_lo + n_rows) collects ent_lo + row, and
+// the mask CSR lists global ids.  The per-shard lists are combined by topk_lists_merge_kernel under
+// the same key order, which gives the unsharded result bit for bit (keys are unique, so the global
+// top k lies in the union of the shards' top min(k, rows)).
 #include "kernels.h"
 
 namespace kge {
@@ -137,7 +142,72 @@ __global__ void topk_finish_kernel(const unsigned long long* __restrict__ best, 
   scores[gid] = key == 0ull ? -INFINITY : key_score((unsigned)(key >> 32));
 }
 
+// ---- merge of per-shard top-k lists (kge_topk_merge) ----
+constexpr int LISTS_WARPS = 4;      // queries per block, one warp each
+
+// key of entry `at` of a (pred, scores) list: the key the scan gave it, 0 for an empty slot (pred < 0)
+__device__ __forceinline__ unsigned long long list_key(const int64_t* __restrict__ pred,
+                                                       const float* __restrict__ scores, size_t at) {
+  const int64_t id = pred[at];
+  return id < 0 ? 0ull : make_key(scores[at], (int)id);
+}
+
+// One warp per query: lane l holds the heads of lists l and l + 32.  Every step takes the largest head
+// (warp max of the 64-bit keys; keys are unique because ids are) and advances the list it came from.
+// Lists are sorted best first, so the output is the k best keys of their union, in key order.
+__global__ void __launch_bounds__(LISTS_WARPS * 32)
+    topk_lists_merge_kernel(const int64_t* __restrict__ pred_in, const float* __restrict__ scores_in,
+                            int n_lists, long long n, int k_in, int k, int64_t* __restrict__ pred,
+                            float* __restrict__ scores) {
+  const long long q = (long long)blockIdx.x * LISTS_WARPS + threadIdx.x / 32;
+  if (q >= n) return;                // whole warps leave together
+  const int lane = threadIdx.x & 31;
+  const size_t list_stride = (size_t)n * k_in, row = (size_t)q * k_in;
+  const size_t base0 = (size_t)lane * list_stride + row, base1 = (size_t)(lane + 32) * list_stride + row;
+  int pos0 = 0, pos1 = 0;
+  unsigned long long h0 = lane < n_lists ? list_key(pred_in, scores_in, base0) : 0ull;
+  unsigned long long h1 = lane + 32 < n_lists ? list_key(pred_in, scores_in, base1) : 0ull;
+  int64_t* out_pred = pred + (size_t)q * k;
+  float* out_scores = scores + (size_t)q * k;
+  for (int j = 0; j < k; ++j) {
+    unsigned long long top = h0 > h1 ? h0 : h1;
+#pragma unroll
+    for (int off = 16; off > 0; off >>= 1) {
+      const unsigned long long o = __shfl_xor_sync(0xffffffffu, top, off);
+      top = o > top ? o : top;
+    }
+    if (top == 0ull) {               // every list is exhausted: the remaining slots stay empty
+      for (int i = j + lane; i < k; i += 32) {
+        out_pred[i] = -1;
+        out_scores[i] = -INFINITY;
+      }
+      return;
+    }
+    if (lane == 0) {
+      out_pred[j] = (int64_t)(0xffffffffu - (unsigned)(top & 0xffffffffull));
+      out_scores[j] = key_score((unsigned)(top >> 32));
+    }
+    if (h0 == top) {
+      ++pos0;
+      h0 = pos0 < k_in ? list_key(pred_in, scores_in, base0 + pos0) : 0ull;
+    } else if (h1 == top) {
+      ++pos1;
+      h1 = pos1 < k_in ? list_key(pred_in, scores_in, base1 + pos1) : 0ull;
+    }
+  }
+}
+
 }  // namespace
+
+cudaError_t launch_topk_lists_merge(const int64_t* pred_in, const float* scores_in, int n_lists, int64_t n,
+                                    int k_in, int k, int64_t* pred, float* scores, cudaStream_t stream) {
+  if (n <= 0) return cudaSuccess;
+  if (n_lists < 1 || n_lists > TOPK_MAX_LISTS || k < 1 || k > TOPK_MAX_K || k_in < 1) return cudaErrorInvalidValue;
+  const long long blocks = (n + LISTS_WARPS - 1) / LISTS_WARPS;
+  topk_lists_merge_kernel<<<(unsigned)blocks, LISTS_WARPS * 32, 0, stream>>>(pred_in, scores_in, n_lists, n, k_in,
+                                                                             k, pred, scores);
+  return cudaGetLastError();
+}
 
 cudaError_t launch_topk_merge(unsigned long long* best, int k, const int2* col_buf,
                               const unsigned* col_count, unsigned long long col_cap, long long dense_count,

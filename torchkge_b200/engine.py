@@ -1,9 +1,10 @@
 """Host-side driver of the CUDA engine: turns torch tensors into C-ABI calls.
 
 Nothing here computes scores: torch is used for device memory, streams and (when the entity
-table is range-partitioned) the two NCCL all-reduces.  The only engine is the CUDA one; tests
-may substitute an object with the same four methods (``pack``, ``gather_rows``,
-``rank_side``, ``score_all``) to exercise the sharding logic on CPU.
+table is range-partitioned) the collectives of the sharded paths.  The only engine is the CUDA one; tests
+may substitute an object with the same methods (``pack``, ``gather_rows``, ``rank_side``,
+``score_all``; ``topk_side`` / ``topk_merge`` for top-k inference) to exercise the sharding logic
+on CPU.
 """
 import ctypes
 import os
@@ -352,8 +353,24 @@ class CudaEngine:
             a.mask_offs, a.mask_ids = _ptr(mask[0]), _ptr(mask[1])
         a.pred, a.scores = _ptr(pred), _ptr(scores)
         a.workspace, a.workspace_bytes, a.stream = _ptr(ws), ws_bytes, _stream(dev)
+        a.ent_lo = spec.ent_lo   # pred holds global ids; mask ids are global too
         _lib.check(self.lib.kge_topk_side(ctypes.byref(a)), "kge_topk_side")
         self.launches += 7   # prep, pack, fill, finish + at least one collect scan / merge pair
+        return pred, scores
+
+    def topk_merge(self, pred_in, scores_in, k):
+        """(pred int64 (n, k), scores float32 (n, k)): the k best entries of the union of the lists
+        pred_in int64 / scores_in float32 (n_lists, n, k_in), each sorted best first as topk_side
+        returns them, pred = -1 marking an empty slot; same order as topk_side (kge_topk_merge)."""
+        _need_cuda(pred_in, scores_in)
+        pred_in, scores_in = pred_in.contiguous(), scores_in.contiguous()
+        n_lists, n, k_in = pred_in.shape
+        dev = pred_in.device
+        pred = torch.empty((n, k), dtype=torch.int64, device=dev)
+        scores = torch.empty((n, k), dtype=torch.float32, device=dev)
+        _lib.check(self.lib.kge_topk_merge(_ptr(pred_in), _ptr(scores_in), n_lists, n, k_in, k, _ptr(pred),
+                                           _ptr(scores), _stream(dev)), "kge_topk_merge")
+        self.launches += 1
         return pred, scores
 
     def rescal_rel_scores(self, spec, hrows, trows):
@@ -438,6 +455,15 @@ class EntityShard:
             dist.all_reduce(t, op=dist.ReduceOp.SUM, group=self.group)
         return t
 
+    def stack_all(self, t):
+        """(world, *t.shape): every rank's ``t`` (same shape on all ranks), in rank order."""
+        if self.world == 1:
+            return t.unsqueeze(0)
+        import torch.distributed as dist
+        everyone = torch.empty((self.world,) + tuple(t.shape), dtype=t.dtype, device=t.device)
+        dist.all_gather(list(everyone.unbind(0)), t.contiguous(), group=self.group)
+        return everyone
+
 
 class QueryShard:
     """Contiguous split of n test triples over the ranks of a process group, for tables that fit
@@ -471,19 +497,21 @@ class QueryShard:
         return t
 
     def all_gather(self, parts):
-        """Per-rank result vectors (one entry per local triple, same dtype) -> full-length vectors on
-        every rank, with ONE collective for all of them."""
+        """Per-rank results (one row per local triple: vectors, or tensors with the same trailing
+        dimensions, all of one dtype) -> full-length results on every rank, with ONE collective for
+        all of them."""
         if self.world == 1:
             return list(parts)
         import torch.distributed as dist
         k = len(parts)
-        mine = torch.zeros((k, self.per), dtype=parts[0].dtype, device=parts[0].device)
+        trail = tuple(parts[0].shape[1:])
+        mine = torch.zeros((k, self.per) + trail, dtype=parts[0].dtype, device=parts[0].device)
         for i, x in enumerate(parts):
-            mine[i, :x.numel()] = x
-        everyone = torch.empty((self.world, k, self.per), dtype=mine.dtype, device=mine.device)
+            mine[i, :x.shape[0]] = x
+        everyone = torch.empty((self.world,) + tuple(mine.shape), dtype=mine.dtype, device=mine.device)
         dist.all_gather([everyone[i] for i in range(self.world)], mine, group=self.group)
         # rank-major slices of length `per` concatenate to the original order of the triples
-        full = everyone.permute(1, 0, 2).reshape(k, self.world * self.per)[:, :self.n]
+        full = everyone.transpose(0, 1).reshape((k, self.world * self.per) + trail)[:, :self.n]
         return [full[i] for i in range(k)]
 
 
@@ -712,3 +740,176 @@ def rank_relation_prediction(spec, h_idx, t_idx, r_idx, filt, directed=True, eng
     ranks, filt_ranks = engine.finalize(counters[0], counters[1])
     del keep
     return ranks, filt_ranks
+
+
+# ------------------------------------------------------------------------------ top-k inference
+#: queries per top-k call (bounds the collect lists of kge_topk_side; results never depend on it)
+TOPK_CHUNK = 16384
+TOPK_MAX_K = 1024          # csrc/kernels.h
+
+
+def _topk_chunks(n, n_cand, k, topk_chunk, mask_csr, device, chunk):
+    """Runs topk_chunk(lo, hi, mask) -> (pred, vals) over chunks of queries; ``mask_csr`` is a host
+    CSR over all n queries, each chunk gets its rows (offsets rebased) on the device."""
+    if k > n_cand:
+        from .exceptions import WrongArgumentsError
+        raise WrongArgumentsError("top_k = %d exceeds the %d candidates" % (k, n_cand))
+    pred = torch.empty((n, k), dtype=torch.int64, device=device)
+    vals = torch.empty((n, k), dtype=torch.float32, device=device)
+    for lo in range(0, n, chunk):
+        hi = min(n, lo + chunk)
+        mask = None
+        if mask_csr is not None:
+            offs, ids = mask_csr
+            a, b = int(offs[lo]), int(offs[hi])
+            mask = ((offs[lo:hi + 1] - a).to(device), ids[a:b].to(device))
+        pred[lo:hi], vals[lo:hi] = topk_chunk(lo, hi, mask)
+    return pred, vals
+
+
+def _pair_pack(pred, vals):
+    """(n, k) int64 ids and (n, k) float32 scores -> one (n, 2, k) int64 tensor holding the score
+    bits, so that one collective carries both."""
+    return torch.stack([pred, vals.view(torch.int32).to(torch.int64)], 1)
+
+
+def _pair_unpack(t):
+    """(..., 2, k) int64 from _pair_pack -> (ids int64 (..., k), scores float32 (..., k)), contiguous."""
+    return t[..., 0, :].contiguous(), t[..., 1, :].to(torch.int32).contiguous().view(torch.float32)
+
+
+def _check_sharded_k(k, n_cand):
+    """Argument errors of a sharded call, raised on every rank before the first collective (a rank
+    with nothing to compute must not wait in a collective that the others never reach)."""
+    if k > n_cand:
+        from .exceptions import WrongArgumentsError
+        raise WrongArgumentsError("top_k = %d exceeds the %d candidates" % (k, n_cand))
+    if not 1 <= k <= TOPK_MAX_K:
+        raise _lib.KgeLibraryError("top-k inference: k must be in [1, %d]" % TOPK_MAX_K)
+
+
+def _by_query_slices(shard, n, mask, run, *idx):
+    """QueryShard: ``run(*local idx, local mask)`` on this rank's slice of the n queries, then one
+    all-gather of the (n_local, k) results."""
+    if shard.n != n:
+        raise ValueError("QueryShard covers %d queries, got %d" % (shard.n, n))
+    pred, vals = run(*shard.slice(*idx), shard.csr(mask))
+    full, = shard.all_gather([_pair_pack(pred, vals)])
+    return _pair_unpack(full)
+
+
+def _exchanged_rows(spec, idx, shard, engine):
+    """(n, planes, dim) rows of the entities ``idx`` on every rank: each rank fills the rows it holds,
+    the others stay zero, one sum-all-reduce."""
+    if spec.n_rows > 0:
+        rows = engine.gather_rows(spec, idx)
+    else:                  # an empty shard (n_ent < world) has no table to read
+        rows = torch.zeros((idx.shape[0], spec.cand_planes, spec.dim), dtype=torch.float32, device=idx.device)
+    return shard.all_reduce_sum(rows)
+
+
+def topk_entity_inference(spec, ents, rels, side, k, mask=None, shard=None, engine=None, chunk=TOPK_CHUNK):
+    """The k best entities completing (ents[i], rels[i], ?) (side SIDE_TAIL) or (?, rels[i], ents[i])
+    (SIDE_HEAD), best first (EntityInference).
+
+    spec       ModelSpec holding the full entity table, or exactly this rank's rows under an
+               EntityShard with local storage (spec.ent_lo / spec.n_ent set from the shard)
+    ents/rels  int64 device tensors (n,)
+    mask       host CSR (offs int64 (n+1,), ids int64) of GLOBAL entity ids to score -inf per query,
+               ascending within a row, or None
+    shard      None; EntityShard: every rank scans its rows for every query (query rows exchanged by
+               one all-reduce per chunk), keeps its top min(k, rows) and the lists of all ranks are
+               all-gathered and merged by kge_topk_merge; QueryShard: every rank answers its slice of
+               the queries against the whole table and the results are all-gathered
+    Returns (pred int64 (n, k), scores float32 (n, k)) on the device, the same on every rank and
+    equal, bit for bit, to the unsharded call.
+    """
+    engine = engine or default_engine()
+    n = ents.shape[0]
+    dev = spec.ent0.device
+    if isinstance(shard, QueryShard) and shard.world > 1:
+        _check_sharded_k(k, spec.n_ent)
+        return _by_query_slices(shard, n, mask, lambda e, r, m: topk_entity_inference(
+            spec, e, r, side, k, m, engine=engine, chunk=chunk), ents, rels)
+    with _device_guard(dev):
+        if shard is None or shard.world == 1:
+            packed = engine.pack(spec)
+
+            def topk_chunk(lo, hi, m):
+                rows = engine.gather_rows(spec, ents[lo:hi])
+                return engine.topk_side(spec, packed, side, rows, rows, rels[lo:hi].contiguous(), k, m)
+
+            return _topk_chunks(n, spec.n_rows, k, topk_chunk, mask, dev, chunk)
+        # EntityShard
+        _check_sharded_k(k, spec.n_ent)
+        if (spec.ent_lo, spec.n_rows) != (shard.lo, shard.hi - shard.lo):
+            spec = spec.narrowed(shard.lo, shard.hi)
+        k_loc = min(k, spec.n_rows)
+        packed = engine.pack(spec) if k_loc > 0 else None
+
+        def topk_chunk(lo, hi, m):
+            rows = _exchanged_rows(spec, ents[lo:hi], shard, engine)
+            pred = torch.full((hi - lo, k), -1, dtype=torch.int64, device=dev)
+            vals = torch.full((hi - lo, k), float("-inf"), dtype=torch.float32, device=dev)
+            if k_loc > 0:     # a shard with fewer rows than k pads its list with empty slots
+                pred[:, :k_loc], vals[:, :k_loc] = engine.topk_side(spec, packed, side, rows, rows,
+                                                                    rels[lo:hi].contiguous(), k_loc, m)
+            pred_in, scores_in = _pair_unpack(shard.stack_all(_pair_pack(pred, vals)))
+            return engine.topk_merge(pred_in, scores_in, k)
+
+        return _topk_chunks(n, spec.n_ent, k, topk_chunk, mask, dev, chunk)
+
+
+def topk_relation_inference(spec, e1, e2, k, mask=None, shard=None, engine=None, chunk=TOPK_CHUNK):
+    """The k best relations completing (e1[i], ?, e2[i]), best first (RelationInference).
+
+    The candidates are the relations, which every rank holds, so both shard types split the queries
+    over the ranks and all-gather the results; under an EntityShard the rows of e1 / e2 are first
+    exchanged (one all-reduce per chunk), the queries of each chunk are split as QueryShard splits
+    them.  Arguments and result as in topk_entity_inference; ``mask`` lists relation ids.
+    """
+    engine = engine or default_engine()
+    n = e1.shape[0]
+    dev = spec.ent0.device
+    if isinstance(shard, QueryShard) and shard.world > 1:
+        _check_sharded_k(k, spec.n_rel)
+        return _by_query_slices(shard, n, mask, lambda a, b, m: topk_relation_inference(
+            spec, a, b, k, m, engine=engine, chunk=chunk), e1, e2)
+    if spec.code == _lib.RESCAL:
+        # candidates are relation matrices: dense (n, n_rel) scores, then the same selection kernels
+        rspec, packed, n_cand = None, None, spec.n_rel
+    else:
+        rspec = relation_spec(spec)
+        packed, n_cand = engine.pack(rspec), rspec.n_rows
+
+    def local_topk(hrows, trows, m):
+        if rspec is None:
+            m_rows = hrows.shape[0]
+            scores = engine.rescal_rel_scores(spec, hrows.view(m_rows, spec.dim), trows.view(m_rows, spec.dim))
+            return engine.topk_dense(scores, k, m)
+        return engine.topk_side(rspec, packed, _lib.SIDE_REL, hrows, trows, None, k, m)
+
+    with _device_guard(dev):
+        if shard is None or shard.world == 1:
+            def topk_chunk(lo, hi, m):
+                return local_topk(engine.gather_rows(spec, e1[lo:hi]), engine.gather_rows(spec, e2[lo:hi]), m)
+
+            return _topk_chunks(n, n_cand, k, topk_chunk, mask, dev, chunk)
+        # EntityShard: the entity table is split, the relations are not
+        _check_sharded_k(k, n_cand)
+        if (spec.ent_lo, spec.n_rows) != (shard.lo, shard.hi - shard.lo):
+            spec = spec.narrowed(shard.lo, shard.hi)
+
+        def topk_chunk(lo, hi, m):
+            rows = _exchanged_rows(spec, torch.cat([e1[lo:hi], e2[lo:hi]]), shard, engine)
+            part = QueryShard(hi - lo, shard.rank, shard.world, shard.group)
+            a, b = part.lo, part.hi
+            if b > a:
+                pred, vals = local_topk(rows[a:b], rows[hi - lo + a:hi - lo + b], part.csr(m))
+            else:
+                pred = torch.empty((0, k), dtype=torch.int64, device=dev)
+                vals = torch.empty((0, k), dtype=torch.float32, device=dev)
+            full, = part.all_gather([_pair_pack(pred, vals)])
+            return _pair_unpack(full)
+
+        return _topk_chunks(n, n_cand, k, topk_chunk, mask, dev, chunk)

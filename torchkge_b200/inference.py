@@ -11,6 +11,10 @@ are sorted descending as the reference's ``sort(descending=True)[:, :k]`` (the O
 tied scores is unspecified there; here: ascending candidate id, except that +0.0 ranks above -0.0
 -- the returned scores keep their sign bit).
 
+Extension: ``shard=EntityShard | QueryShard`` spreads the work over the ranks of a process group
+(host logic in ``engine.topk_entity_inference`` / ``topk_relation_inference``, DESIGN.md section 6);
+every rank ends with the full results, equal to those of one unsharded call.
+
 Deviation, on purpose: the reference stores the scores with ``self.scores[i * b_size, (i + 1) *
 b_size] = ...`` (inference.py:151, 246) -- an index pair instead of a slice, which raises
 IndexError for every usual argument.  Here ``scores[i]`` holds the scores of ``predictions[i]``.
@@ -18,10 +22,12 @@ IndexError for every usual argument.  Here ``scores[i]`` holds the scores of ``p
 import torch
 
 from . import _lib
-from .engine import ModelSpec, default_engine, relation_spec
+from .engine import (TOPK_CHUNK, EntityShard, ModelSpec, default_engine, topk_entity_inference,
+                     topk_relation_inference)
 from .exceptions import WrongArgumentsError
 
-_MAX_QUERIES_PER_CALL = 16384
+#: queries per top-k call
+_MAX_QUERIES_PER_CALL = TOPK_CHUNK
 
 
 def _mask_csr(dictionary, key1, key2):
@@ -37,21 +43,15 @@ def _mask_csr(dictionary, key1, key2):
     return torch.tensor(offs, dtype=torch.int64), torch.tensor(ids, dtype=torch.int64)
 
 
-def _topk_chunks(n, n_cand, top_k, topk_chunk, mask_csr, device):
-    """Runs topk_chunk(lo, hi, mask) -> (pred, vals) over chunks of queries."""
-    if top_k > n_cand:
-        raise WrongArgumentsError("top_k = %d exceeds the %d candidates" % (top_k, n_cand))
-    pred = torch.empty((n, top_k), dtype=torch.int64, device=device)
-    vals = torch.empty((n, top_k), dtype=torch.float32, device=device)
-    for lo in range(0, n, _MAX_QUERIES_PER_CALL):
-        hi = min(n, lo + _MAX_QUERIES_PER_CALL)
-        mask = None
-        if mask_csr is not None:
-            offs, ids = mask_csr
-            a, b = int(offs[lo]), int(offs[hi])
-            mask = ((offs[lo:hi + 1] - a).to(device), ids[a:b].to(device))
-        pred[lo:hi], vals[lo:hi] = topk_chunk(lo, hi, mask)
-    return pred, vals
+def _cuda_spec(model, shard, who):
+    spec = ModelSpec.from_model(model)
+    if isinstance(shard, EntityShard) and shard.local_storage:
+        # the model holds only this rank's rows: its row 0 is entity shard.lo
+        spec.ent_lo, spec.n_ent = shard.lo, shard.n_ent
+    if not spec.ent0.is_cuda:
+        raise _lib.KgeLibraryError("%s.evaluate needs the model on a CUDA device; "
+                                   "this package has no CPU execution path" % who)
+    return spec
 
 
 class EntityInference(object):
@@ -66,12 +66,19 @@ class EntityInference(object):
     dictionary: optional mapping (known entity, relation) -> set of entities known to complete the
         pair (``kg.dict_of_tails`` for missing tails, ``kg.dict_of_heads`` for missing heads);
         those are excluded from the predictions.
+    shard: ``torchkge_b200.engine.EntityShard`` or ``QueryShard``, optional, keyword only
+        (extension).  EntityShard: every rank of the group scans only its range of entity rows
+        (``local_storage=True``: the model holds only those rows) and the per-rank top-k lists are
+        merged on the device.  QueryShard (over ``len(known_entities)`` queries): every rank answers
+        its contiguous slice of the queries against the whole (replicated) table.  Either way every
+        rank ends up with the full results, equal to those of one unsharded call.
 
     Attributes: ``predictions`` LongTensor (n_facts, top_k), ``scores`` FloatTensor (n_facts, top_k),
     both on CPU after ``evaluate``.
     """
 
-    def __init__(self, model, known_entities, known_relations, top_k=1, missing='tails', dictionary=None):
+    def __init__(self, model, known_entities, known_relations, top_k=1, missing='tails', dictionary=None, *,
+                 shard=None):
         if missing not in ('heads', 'tails'):
             raise WrongArgumentsError("missing entity should either be 'heads' or 'tails'")
         self.model = model
@@ -80,30 +87,22 @@ class EntityInference(object):
         self.missing = missing
         self.top_k = top_k
         self.dictionary = dictionary
+        self.shard = shard
         self.predictions = torch.empty(size=(len(known_entities), top_k)).long()
         self.scores = torch.empty(size=(len(known_entities), top_k))
 
     def evaluate(self, b_size, verbose=True):
         """``b_size`` / ``verbose``: accepted for signature compatibility (chunking is by memory)."""
-        spec = ModelSpec.from_model(self.model)
-        if not spec.ent0.is_cuda:
-            raise _lib.KgeLibraryError("EntityInference.evaluate needs the model on a CUDA device; "
-                                       "this package has no CPU execution path")
+        spec = _cuda_spec(self.model, self.shard, "EntityInference")
         dev = spec.ent0.device
-        engine = default_engine()
-        packed = engine.pack(spec)
         ents = self.known_entities.long().to(dev)
         rels = self.known_relations.long().to(dev)
         side = _lib.SIDE_TAIL if self.missing == 'tails' else _lib.SIDE_HEAD
-
-        def topk_chunk(lo, hi, mask):
-            rows = engine.gather_rows(spec, ents[lo:hi])
-            return engine.topk_side(spec, packed, side, rows, rows, rels[lo:hi].contiguous(), self.top_k, mask)
-
         mask = None
         if self.dictionary is not None:
             mask = _mask_csr(self.dictionary, self.known_entities, self.known_relations)
-        pred, vals = _topk_chunks(ents.shape[0], spec.n_rows, self.top_k, topk_chunk, mask, dev)
+        pred, vals = topk_entity_inference(spec, ents, rels, side, self.top_k, mask, shard=self.shard,
+                                           engine=default_engine(), chunk=_MAX_QUERIES_PER_CALL)
         self.predictions, self.scores = pred.cpu(), vals.cpu()
 
 
@@ -113,47 +112,30 @@ class RelationInference(object):
     model: TransE (L1/L2), DistMult or ComplEx model on a CUDA device.  dictionary: optional
     mapping (entity 1, entity 2) -> set of known relations (``kg.dict_of_rels``), excluded from
     the predictions.  Attributes: ``predictions`` (n_facts, top_k) long, ``scores`` float.
+    shard: ``EntityShard`` or ``QueryShard``, optional, keyword only (extension).  The candidates
+    are the relations, which every rank holds: under either type every rank answers a contiguous
+    slice of the queries and the results are all-gathered; under EntityShard the rows of the two
+    entities are first exchanged between the ranks that hold them.  Every rank ends up with the
+    full results.
     """
 
-    def __init__(self, model, entities1, entities2, top_k=1, dictionary=None):
+    def __init__(self, model, entities1, entities2, top_k=1, dictionary=None, *, shard=None):
         self.model = model
         self.entities1 = entities1
         self.entities2 = entities2
         self.topk = top_k
         self.dictionary = dictionary
+        self.shard = shard
         self.predictions = torch.empty(size=(len(entities1), top_k)).long()
         self.scores = torch.empty(size=(len(entities2), top_k))
 
     def evaluate(self, b_size, verbose=True):
-        spec = ModelSpec.from_model(self.model)
-        if not spec.ent0.is_cuda:
-            raise _lib.KgeLibraryError("RelationInference.evaluate needs the model on a CUDA device; "
-                                       "this package has no CPU execution path")
+        spec = _cuda_spec(self.model, self.shard, "RelationInference")
         dev = spec.ent0.device
-        engine = default_engine()
         e1, e2 = self.entities1.long().to(dev), self.entities2.long().to(dev)
-        if spec.code == _lib.RESCAL:
-            # candidates are relation matrices: dense (n, n_rel) scores, then the same selection kernels
-            def topk_chunk(lo, hi, mask):
-                hrows = engine.gather_rows(spec, e1[lo:hi]).view(hi - lo, spec.dim)
-                trows = engine.gather_rows(spec, e2[lo:hi]).view(hi - lo, spec.dim)
-                return engine.topk_dense(engine.rescal_rel_scores(spec, hrows, trows), self.topk, mask)
-
-            mask = None
-            if self.dictionary is not None:
-                mask = _mask_csr(self.dictionary, self.entities1, self.entities2)
-            pred, vals = _topk_chunks(e1.shape[0], spec.n_rel, self.topk, topk_chunk, mask, dev)
-            self.predictions, self.scores = pred.cpu(), vals.cpu()
-            return
-        rspec = relation_spec(spec)
-        packed = engine.pack(rspec)
-
-        def topk_chunk(lo, hi, mask):
-            hrows, trows = engine.gather_rows(spec, e1[lo:hi]), engine.gather_rows(spec, e2[lo:hi])
-            return engine.topk_side(rspec, packed, _lib.SIDE_REL, hrows, trows, None, self.topk, mask)
-
         mask = None
         if self.dictionary is not None:
             mask = _mask_csr(self.dictionary, self.entities1, self.entities2)
-        pred, vals = _topk_chunks(e1.shape[0], rspec.n_rows, self.topk, topk_chunk, mask, dev)
+        pred, vals = topk_relation_inference(spec, e1, e2, self.topk, mask, shard=self.shard,
+                                             engine=default_engine(), chunk=_MAX_QUERIES_PER_CALL)
         self.predictions, self.scores = pred.cpu(), vals.cpu()
