@@ -39,7 +39,7 @@
 extern "C" {
 #endif
 
-#define KGE_ABI_VERSION 9
+#define KGE_ABI_VERSION 10
 
 /* error codes */
 #define KGE_OK 0
@@ -384,7 +384,22 @@ int kge_pair_loss_bwd(int kind, const float* pos, const float* neg, int64_t n, c
  * MarginLoss in one kernel: one warp per positive triple scores it and its n_neg negatives;
  * no (b*n_neg) index or score tensor is materialised unless the optional outputs are given.
  * Negatives: nh/nt if non-NULL (deterministic mode), else drawn in-kernel exactly as
- * kge_corrupt_batch would with the same (seed, offset). */
+ * kge_corrupt_batch would with the same (seed, offset).
+ *
+ * Entity-sharded step (hrows != NULL).  The entity table is range-partitioned: tb.ent0 / ent1 hold
+ * the rows [ent_lo, ent_lo + n_rows) (n_rows = 0 is valid), n_ent is the GLOBAL entity count the draws
+ * use, and hrows / trows are the positives' rows [b][planes][dim] as kge_gather_rows lays them out
+ * (summed over the ranks).  Every rank makes the same draws; a negative is scored only by the rank
+ * that holds its replaced entity, so summing `loss` over the ranks gives the unsharded loss.
+ * Backward: the replaced rows' gradients go into g->ent0 / ent1 (local rows), the gradients of the
+ * positives' h / t rows (also the intact entity of every negative) into grad_hrows / grad_trows
+ * [b][planes][dim] (zeroed by the caller, added into), the relation gradients into g->rel0 / rel1.
+ * Each of these is linear in the set of negatives: summing grad_hrows, grad_trows and the relation
+ * gradients over the ranks, then adding the rows of grad_hrows / grad_trows into the entity gradient
+ * (kge_scatter_rows_add) gives the unsharded gradient.  In this mode nh / nt, pos_out, neg_out,
+ * nh_out, nt_out must be NULL, trows is required and, in backward, grad_hrows / grad_trows;
+ * anything else returns KGE_ERR_ARG.  hrows == NULL: the unsharded step (ent_lo, n_rows, trows,
+ * grad_hrows, grad_trows are ignored). */
 typedef struct {
   kge_tables_t tb;
   int32_t n_neg;
@@ -399,11 +414,21 @@ typedef struct {
   float* pos_out; float* neg_out;       /* optional */
   int64_t* nh_out; int64_t* nt_out;     /* optional */
   void* stream;
+  int64_t ent_lo;                       /* sharded: global id of row 0 of tb.ent0 / ent1 */
+  int64_t n_rows;                       /* sharded: rows held */
+  const float* hrows; const float* trows;   /* sharded: [b][planes][dim] positive rows, or NULL */
+  float* grad_hrows; float* grad_trows;     /* sharded backward: [b][planes][dim], += */
 } kge_margin_step_args_t;
 int kge_margin_step_fwd(const kge_margin_step_args_t* a);
 /* grad_loss: device pointer to the upstream gradient of the scalar loss */
 int kge_margin_step_bwd(const kge_margin_step_args_t* a, const kge_grads_t* g,
                         const float* grad_loss);
+/* The inverse of kge_gather_rows for gradients: grad_plane[idx[i] - ent_lo] += rows[i][plane] for
+ * every i < n with ent_lo <= idx[i] < ent_lo + n_rows (atomics: ids may repeat); other ids are
+ * ignored.  rows: [n][planes][dim]; grad1 for two- and three-plane models (plane 2 at
+ * grad1 + (grad1 - grad0)). */
+int kge_scatter_rows_add(int model, float* grad0, float* grad1, int64_t ent_lo, int64_t n_rows, int dim,
+                         const int64_t* idx, int64_t n, const float* rows, void* stream);
 
 /* ---- measurement hook ------------------------------------------------------------------
  * When enabled, the dominant kernels of kge_rank_side / kge_score_all are bracketed by CUDA

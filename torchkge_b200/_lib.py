@@ -15,7 +15,7 @@ LIB_PATH = os.path.join(HERE, "lib", "libkge_b200.so")
 TRANSE_L1, TRANSE_L2, DISTMULT, RESCAL, COMPLEX, ROTATE, TORUSE_L1, TORUSE_L2, ANALOGY = range(9)
 SIDE_TAIL, SIDE_HEAD, SIDE_REL = 0, 1, 2
 TILE_C, TILE_Q = 128, 64
-ABI_VERSION = 9
+ABI_VERSION = 10
 FLAG_TENSOR_CORE = 1
 FLAG_APPROX_SCAN = 2
 LOSS_LOGISTIC, LOSS_BCE = 1, 2
@@ -90,6 +90,8 @@ class MarginStepArgs(ctypes.Structure):
         ("seed", _c.c_uint64), ("offset", _c.c_uint64),
         ("loss", _p), ("pos_out", _p), ("neg_out", _p), ("nh_out", _p), ("nt_out", _p),
         ("stream", _p),
+        ("ent_lo", _c.c_int64), ("n_rows", _c.c_int64),
+        ("hrows", _p), ("trows", _p), ("grad_hrows", _p), ("grad_trows", _p),
     ]
 
 
@@ -136,6 +138,8 @@ SIGNATURES = {
     "kge_pair_loss_bwd": (_c.c_int, [_c.c_int, _p, _p, _c.c_int64, _p, _p, _p, _p]),
     "kge_margin_step_fwd": (_c.c_int, [_c.POINTER(MarginStepArgs)]),
     "kge_margin_step_bwd": (_c.c_int, [_c.POINTER(MarginStepArgs), _c.POINTER(Grads), _p]),
+    "kge_scatter_rows_add": (_c.c_int, [_c.c_int, _p, _p, _c.c_int64, _c.c_int64, _c.c_int, _p, _c.c_int64,
+                                        _p, _p]),
     "kge_scan_timing_enable": (_c.c_int, [_c.c_int]),
     "kge_scan_timing_read": (_c.c_int, [_c.c_int, _c.POINTER(_c.c_int64), _c.POINTER(_c.c_double)]),
 }

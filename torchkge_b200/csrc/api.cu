@@ -780,15 +780,40 @@ kge::MarginStepParams to_step(const kge_margin_step_args_t* a) {
   p.h = a->h; p.t = a->t; p.r = a->r; p.nh = a->nh; p.nt = a->nt; p.probs = a->bern_probs;
   p.seed = a->seed; p.offset = a->offset; p.loss = a->loss; p.pos_out = a->pos_out;
   p.neg_out = a->neg_out; p.nh_out = a->nh_out; p.nt_out = a->nt_out;
+  p.ent_lo = a->ent_lo; p.n_rows = a->n_rows; p.hrows = a->hrows; p.trows = a->trows;
+  p.grad_hrows = a->grad_hrows; p.grad_trows = a->grad_trows;
   return p;
 }
+// A shard that holds no rows (n_rows = 0) may pass no entity planes.
+bool step_tables_ok(const kge_margin_step_args_t* a) {
+  if (tables_ok(&a->tb)) return true;
+  if (!a->hrows || a->n_rows != 0) return false;
+  kge_tables_t tb = a->tb;
+  tb.ent0 = a->hrows;
+  tb.ent1 = a->hrows;
+  return tables_ok(&tb);
+}
+bool step_grads_ok(const kge_margin_step_args_t* a, const kge_grads_t* g) {
+  if (grads_ok(&a->tb, g)) return true;
+  if (!g || !a->hrows || a->n_rows != 0) return false;
+  kge_grads_t gg = *g;
+  gg.ent0 = gg.ent1 = a->grad_hrows;
+  return grads_ok(&a->tb, &gg);
+}
 bool step_ok(const kge_margin_step_args_t* a) {
-  if (!a || !tables_ok(&a->tb) || a->b < 0 || a->n_neg < 1 || !a->loss) return false;
+  if (!a || !step_tables_ok(a) || a->b < 0 || a->n_neg < 1 || !a->loss) return false;
   if (a->b > 0 && (!a->h || !a->t || !a->r)) return false;
   if ((a->nh == nullptr) != (a->nt == nullptr)) return false;
   if (!a->nh && !a->bern_probs) return false;
   if ((a->nh_out == nullptr) != (a->nt_out == nullptr)) return false;
+  if (a->hrows) {   // entity-sharded: Philox draws only, no per-negative outputs
+    if (!a->trows || a->nh || a->pos_out || a->neg_out || a->nh_out) return false;
+    if (a->ent_lo < 0 || a->n_rows < 0 || a->ent_lo + a->n_rows > a->n_ent) return false;
+  }
   return true;
+}
+bool shard_grads_ok(const kge_margin_step_args_t* a) {
+  return !a->hrows || (a->grad_hrows && a->grad_trows);
 }
 }  // namespace
 
@@ -886,12 +911,27 @@ int kge_margin_step_fwd(const kge_margin_step_args_t* a) {
 
 int kge_margin_step_bwd(const kge_margin_step_args_t* a, const kge_grads_t* g,
                         const float* grad_loss) {
-  if (!step_ok(a) || !grads_ok(&a->tb, g) || !grad_loss)
+  if (!step_ok(a) || !step_grads_ok(a, g) || !grad_loss || !shard_grads_ok(a))
     return fail(KGE_ERR_ARG, "kge_margin_step_bwd: bad argument");
   DeviceScope device_scope(a->tb.ent0);
   KGE_CUDA_TRY(kge::launch_margin_step_bwd(to_step(a), to_grads(g), grad_loss,
                                            static_cast<cudaStream_t>(a->stream)),
                "margin_step_bwd");
+  return KGE_OK;
+}
+
+int kge_scatter_rows_add(int model, float* grad0, float* grad1, int64_t ent_lo, int64_t n_rows, int dim,
+                         const int64_t* idx, int64_t n, const float* rows, void* stream) {
+  const int planes = kge_cand_planes(model);
+  if (planes == 0) return fail(KGE_ERR_ARG, "kge_scatter_rows_add: unknown model");
+  if (n < 0 || n_rows < 0 || dim < 1) return fail(KGE_ERR_ARG, "kge_scatter_rows_add: bad sizes");
+  if (n == 0 || n_rows == 0) return KGE_OK;
+  if (!grad0 || !idx || !rows || (planes >= 2 && !grad1))
+    return fail(KGE_ERR_ARG, "kge_scatter_rows_add: null pointer");
+  DeviceScope device_scope(grad0);
+  KGE_CUDA_TRY(kge::launch_scatter_rows_add(grad0, grad1, planes, ent_lo, n_rows, dim, idx, n, rows,
+                                            static_cast<cudaStream_t>(stream)),
+               "scatter_rows_add");
   return KGE_OK;
 }
 

@@ -55,18 +55,27 @@ __device__ __forceinline__ uint4 philox4x32(uint64_t seed, uint64_t offset, uint
   return make_uint4(c0, c1, c2, c3);
 }
 
-// One corrupted triple: Bernoulli(p_r) decides head vs tail, the replacement is uniform on
-// [1, n_ent) -- entity 0 is never drawn and true triples are not rejected, as in
-// sampling.py:318-325.
-__device__ __forceinline__ void corrupt_one(uint64_t seed, uint64_t offset, uint64_t idx, float p,
-                                            long long n_ent, long long h, long long t,
-                                            long long* nh, long long* nt) {
+// The draw of one negative: Bernoulli(p_r) decides head vs tail (returned), the replacement *e is
+// uniform on [1, n_ent) -- entity 0 is never drawn and true triples are not rejected, as in
+// sampling.py:318-325.  Both depend on (seed, offset, idx, p, n_ent) only, so every rank of a sharded
+// step makes the same draw and the same head / tail decision.
+__device__ __forceinline__ bool draw_one(uint64_t seed, uint64_t offset, uint64_t idx, float p,
+                                         long long n_ent, long long* e_out) {
   const uint4 rnd = philox4x32(seed, offset, idx);
   const float u = (rnd.x >> 8) * (1.0f / 16777216.0f);  // [0, 1)
   const long long span = n_ent - 1;
   long long e = 1;
   if (span > 0) e = 1 + (long long)(((unsigned long long)rnd.y * (unsigned long long)span) >> 32);
-  const bool head = u < p;
+  *e_out = e;
+  return u < p;
+}
+
+// One corrupted triple (nh, nt) of the positive (h, t).
+__device__ __forceinline__ void corrupt_one(uint64_t seed, uint64_t offset, uint64_t idx, float p,
+                                            long long n_ent, long long h, long long t,
+                                            long long* nh, long long* nt) {
+  long long e;
+  const bool head = draw_one(seed, offset, idx, p, n_ent, &e);
   *nh = head ? e : h;
   *nt = head ? t : e;
 }
@@ -174,19 +183,99 @@ __device__ __forceinline__ RowPtrs make_rows(int model, int dim, const TrainTabl
   return p;
 }
 
-// Gradient of one triple's score, scaled by g, scattered into the dense gradient tables.
-// Through F.normalize:  d/dh = (G - h~ (h~ . G)) / max(|h|, eps)  with G = dscore/dh~.
-__device__ void triple_backward(int model, int dim, const RowPtrs& p, const TrainGrads& gr,
-                                long long h, long long t, long long r, float g, int lane) {
-  if (g == 0.f) return;
-  float* gh0 = gr.ent0 + (size_t)h * dim;
-  float* gt0 = gr.ent0 + (size_t)t * dim;
+// Destination rows of one triple's gradient, plane by plane (same layout as RowPtrs).
+struct GradRows {
+  float* h0; float* h1;
+  float* t0; float* t1;
+  float* r0; float* r1;
+  float* h2; float* t2; float* r2;
+};
+
+// The rows of triple (h, t, r) in the dense gradient tables.
+__device__ __forceinline__ GradRows grad_rows(int model, int dim, const TrainGrads& gr, long long h,
+                                              long long t, long long r) {
+  GradRows d;
   const size_t rstride = model == KGE_RESCAL ? (size_t)dim * dim : (size_t)dim;
-  float* gr0 = gr.rel0 + (size_t)r * rstride;
+  d.h0 = gr.ent0 + (size_t)h * dim;
+  d.t0 = gr.ent0 + (size_t)t * dim;
+  d.r0 = gr.rel0 + (size_t)r * rstride;
+  d.h1 = d.t1 = d.r1 = d.h2 = d.t2 = d.r2 = nullptr;
+  if (model == KGE_COMPLEX || model == KGE_ROTATE || model == KGE_ANALOGY) {
+    d.h1 = gr.ent1 + (size_t)h * dim;
+    d.t1 = gr.ent1 + (size_t)t * dim;
+    d.r1 = gr.rel1 + (size_t)r * dim;
+  }
+  if (model == KGE_ANALOGY) {
+    float* ge2 = gr.ent1 + (gr.ent1 - gr.ent0);
+    d.h2 = ge2 + (size_t)h * dim;
+    d.t2 = ge2 + (size_t)t * dim;
+    d.r2 = gr.rel1 + (gr.rel1 - gr.rel0) + (size_t)r * dim;
+  }
+  return d;
+}
+
+// ---- entity-sharded rows: the replaced entity from the local table, the rest from [b][planes][dim]
+__device__ __forceinline__ int ent_planes(int model) {
+  return model == KGE_ANALOGY ? 3 : (model == KGE_COMPLEX || model == KGE_ROTATE ? 2 : 1);
+}
+
+template <class T>
+struct Planes { T* p0; T* p1; T* p2; };
+
+// plane pointers of the row at element offset `off` of a table with planes p0, p1 (a third plane at
+// p1 + (p1 - p0), include/kge_b200.h)
+template <class T>
+__device__ __forceinline__ Planes<T> table_planes(T* p0, T* p1, int np, size_t off) {
+  Planes<T> o;
+  o.p0 = p0 + off;
+  o.p1 = np > 1 ? p1 + off : nullptr;
+  o.p2 = np > 2 ? p1 + (p1 - p0) + off : nullptr;
+  return o;
+}
+
+// row w of a [b][np][dim] buffer (hrows / trows / grad_hrows / grad_trows)
+template <class T>
+__device__ __forceinline__ Planes<T> buf_planes(T* buf, int np, int dim, long long w) {
+  T* base = buf + (size_t)w * np * dim;
+  return table_planes(base, base + dim, np, 0);
+}
+
+// relation row r of the (replicated) relation tables
+template <class T>
+__device__ __forceinline__ Planes<T> rel_planes(int model, int dim, T* r0, T* r1, long long r) {
+  const size_t rstride = model == KGE_RESCAL ? (size_t)dim * dim : (size_t)dim;
+  return table_planes(r0, r1, ent_planes(model), (size_t)r * rstride);
+}
+
+__device__ __forceinline__ RowPtrs rows_of(const Planes<const float>& h, const Planes<const float>& t,
+                                           const Planes<const float>& r) {
+  RowPtrs p;
+  p.h0 = h.p0; p.h1 = h.p1; p.h2 = h.p2;
+  p.t0 = t.p0; p.t1 = t.p1; p.t2 = t.p2;
+  p.r0 = r.p0; p.r1 = r.p1; p.r2 = r.p2;
+  return p;
+}
+
+__device__ __forceinline__ GradRows grads_of(const Planes<float>& h, const Planes<float>& t,
+                                             const Planes<float>& r) {
+  GradRows d;
+  d.h0 = h.p0; d.h1 = h.p1; d.h2 = h.p2;
+  d.t0 = t.p0; d.t1 = t.p1; d.t2 = t.p2;
+  d.r0 = r.p0; d.r1 = r.p1; d.r2 = r.p2;
+  return d;
+}
+
+// Gradient of one triple's score, scaled by g, added into the rows `d` (atomics: rows repeat).
+// Through F.normalize:  d/dh = (G - h~ (h~ . G)) / max(|h|, eps)  with G = dscore/dh~.
+__device__ void triple_backward(int model, int dim, const RowPtrs& p, const GradRows& d, float g, int lane) {
+  if (g == 0.f) return;
+  float* gh0 = d.h0;
+  float* gt0 = d.t0;
+  float* gr0 = d.r0;
   if (model == KGE_COMPLEX || model == KGE_ROTATE) {
-    float* gh1 = gr.ent1 + (size_t)h * dim;
-    float* gt1 = gr.ent1 + (size_t)t * dim;
-    float* gr1 = gr.rel1 + (size_t)r * dim;
+    float* gh1 = d.h1;
+    float* gt1 = d.t1;
+    float* gr1 = d.r1;
     for (int k = lane; k < dim; k += 32) {
       const float rh = p.h0[k], ih = p.h1[k], rt = p.t0[k], it = p.t1[k], rr = p.r0[k], ir = p.r1[k];
       float d_rh, d_ih, d_rt, d_it, d_rr, d_ir;
@@ -209,13 +298,12 @@ __device__ void triple_backward(int model, int dim, const RowPtrs& p, const Trai
     return;
   }
   if (model == KGE_ANALOGY) {
-    float* gh1 = gr.ent1 + (size_t)h * dim;
-    float* gt1 = gr.ent1 + (size_t)t * dim;
-    float* gr1 = gr.rel1 + (size_t)r * dim;
-    float* ge2 = gr.ent1 + (gr.ent1 - gr.ent0);
-    float* gh2 = ge2 + (size_t)h * dim;
-    float* gt2 = ge2 + (size_t)t * dim;
-    float* gr2 = gr.rel1 + (gr.rel1 - gr.rel0) + (size_t)r * dim;
+    float* gh1 = d.h1;
+    float* gt1 = d.t1;
+    float* gr1 = d.r1;
+    float* gh2 = d.h2;
+    float* gt2 = d.t2;
+    float* gr2 = d.r2;
     for (int k = lane; k < dim; k += 32) {
       const float sh = p.h0[k], st = p.t0[k], sr = p.r0[k];
       atomicAdd(gh0 + k, g * (sr * st)); atomicAdd(gt0 + k, g * (sh * sr)); atomicAdd(gr0 + k, g * (sh * st));
@@ -317,7 +405,7 @@ __global__ void score_triples_bwd_kernel(int model, int dim, TrainTables tb, Tra
   if (w >= n) return;
   const long long hi = h[w], ti = t[w], ri = r[w];
   const RowPtrs p = make_rows(model, dim, tb, hi, ti, ri);
-  triple_backward(model, dim, p, gr, hi, ti, ri, gout[w], lane);
+  triple_backward(model, dim, p, grad_rows(model, dim, gr, hi, ti, ri), gout[w], lane);
 }
 
 __global__ void corrupt_batch_kernel(const int64_t* __restrict__ h, const int64_t* __restrict__ t,
@@ -383,10 +471,87 @@ __global__ void margin_step_bwd_kernel(MarginStepParams a, TrainGrads gr, const 
     const float neg = triple_score(a.model, a.dim, pn, lane, nullptr, nullptr);
     if (a.margin - pos + neg > 0.f) {  // same sub-gradient as torch: zero at the kink
       ++active;
-      triple_backward(a.model, a.dim, pn, gr, nh, nt, ri, g, lane);
+      triple_backward(a.model, a.dim, pn, grad_rows(a.model, a.dim, gr, nh, nt, ri), g, lane);
     }
   }
-  if (active) triple_backward(a.model, a.dim, pp, gr, hi, ti, ri, -g * (float)active, lane);
+  if (active) triple_backward(a.model, a.dim, pp, grad_rows(a.model, a.dim, gr, hi, ti, ri), -g * (float)active, lane);
+}
+
+// Entity-sharded fused step (a.hrows set), one warp per positive.  Every rank runs the same draws;
+// a negative is scored here only if its replaced entity e lies in [ent_lo, ent_lo + n_rows).  Its
+// rows: e from the local table (row e - ent_lo), the intact entity from hrows / trows, the relation
+// from the replicated table.  The positive is scored on every rank from hrows / trows.
+__device__ __forceinline__ RowPtrs shard_neg_rows(const MarginStepParams& a, long long w, long long ri,
+                                                  bool head, long long loc) {
+  const int np = ent_planes(a.model);
+  const Planes<const float> e = table_planes(a.tb.ent0, a.tb.ent1, np, (size_t)loc * a.dim);
+  const Planes<const float> h = head ? e : buf_planes(a.hrows, np, a.dim, w);
+  const Planes<const float> t = head ? buf_planes(a.trows, np, a.dim, w) : e;
+  return rows_of(h, t, rel_planes(a.model, a.dim, a.tb.rel0, a.tb.rel1, ri));
+}
+
+__device__ __forceinline__ RowPtrs shard_pos_rows(const MarginStepParams& a, long long w, long long ri) {
+  const int np = ent_planes(a.model);
+  return rows_of(buf_planes(a.hrows, np, a.dim, w), buf_planes(a.trows, np, a.dim, w),
+                 rel_planes(a.model, a.dim, a.tb.rel0, a.tb.rel1, ri));
+}
+
+__device__ __forceinline__ bool owned_draw(const MarginStepParams& a, long long idx, float p_head,
+                                           bool* head, long long* loc) {
+  long long e;
+  *head = draw_one(a.seed, a.offset, (uint64_t)idx, p_head, a.n_ent, &e);
+  *loc = e - a.ent_lo;
+  return (unsigned long long)*loc < (unsigned long long)a.n_rows;
+}
+
+__global__ void margin_step_shard_fwd_kernel(MarginStepParams a) {
+  const long long w = ((long long)blockIdx.x * blockDim.x + threadIdx.x) >> 5;
+  const int lane = threadIdx.x & 31;
+  if (w >= a.b) return;
+  const long long ri = a.r[w];
+  const float pos = triple_score(a.model, a.dim, shard_pos_rows(a, w, ri), lane, nullptr, nullptr);
+  const float p_head = a.probs[ri];
+  float loss = 0.f;
+  for (int j = 0; j < a.n_neg; ++j) {
+    bool head;
+    long long loc;
+    if (!owned_draw(a, (long long)j * a.b + w, p_head, &head, &loc)) continue;
+    const float neg = triple_score(a.model, a.dim, shard_neg_rows(a, w, ri, head, loc), lane, nullptr, nullptr);
+    if (lane == 0) loss += fmaxf(0.f, a.margin - pos + neg);
+  }
+  if (lane == 0) atomicAdd(a.loss, loss);
+}
+
+// Backward of the sharded step: the replaced row's gradient goes to the local table (this rank owns
+// it), the intact entity's and the positive's to grad_hrows / grad_trows[w], the relation's to the
+// local copy of the relation gradient; the caller sums the last three over the ranks.
+__global__ void margin_step_shard_bwd_kernel(MarginStepParams a, TrainGrads gr, const float* gloss) {
+  const long long w = ((long long)blockIdx.x * blockDim.x + threadIdx.x) >> 5;
+  const int lane = threadIdx.x & 31;
+  if (w >= a.b) return;
+  const float g = *gloss;
+  const long long ri = a.r[w];
+  const RowPtrs pp = shard_pos_rows(a, w, ri);
+  const float pos = triple_score(a.model, a.dim, pp, lane, nullptr, nullptr);
+  const float p_head = a.probs[ri];
+  const int np = ent_planes(a.model);
+  const Planes<float> gh = buf_planes(a.grad_hrows, np, a.dim, w);
+  const Planes<float> gt = buf_planes(a.grad_trows, np, a.dim, w);
+  const Planes<float> grel = rel_planes(a.model, a.dim, gr.rel0, gr.rel1, ri);
+  int active = 0;
+  for (int j = 0; j < a.n_neg; ++j) {
+    bool head;
+    long long loc;
+    if (!owned_draw(a, (long long)j * a.b + w, p_head, &head, &loc)) continue;
+    const RowPtrs pn = shard_neg_rows(a, w, ri, head, loc);
+    const float neg = triple_score(a.model, a.dim, pn, lane, nullptr, nullptr);
+    if (a.margin - pos + neg > 0.f) {
+      ++active;
+      const Planes<float> ge = table_planes(gr.ent0, gr.ent1, np, (size_t)loc * a.dim);
+      triple_backward(a.model, a.dim, pn, grads_of(head ? ge : gh, head ? gt : ge, grel), g, lane);
+    }
+  }
+  if (active) triple_backward(a.model, a.dim, pp, grads_of(gh, gt, grel), -g * (float)active, lane);
 }
 
 // ------------------------------------------------------------------------------------------
@@ -561,9 +726,9 @@ margin_step_fast_kernel(MarginStepParams a, TrainGrads gr, const float* __restri
           loss += fmaxf(0.f, v);
         }
         if (BWD && v > 0.f) {
-          triple_backward(MODEL, dim, pn, gr, nh, nt, ri, g, lane);
+          triple_backward(MODEL, dim, pn, grad_rows(MODEL, dim, gr, nh, nt, ri), g, lane);
           const RowPtrs pp = make_rows(MODEL, dim, a.tb, hi, ti, ri);
-          triple_backward(MODEL, dim, pp, gr, hi, ti, ri, -g, lane);
+          triple_backward(MODEL, dim, pp, grad_rows(MODEL, dim, gr, hi, ti, ri), -g, lane);
         }
         continue;
       }
@@ -687,7 +852,11 @@ __device__ __forceinline__ Vec vec_load_smem(const float* row, int dim, int lane
 
 // MINB: minimum resident CTAs per SM the register allocation is held to (0: the compiler's choice --
 // 72 registers forward, 128 backward; 5 holds the backward form to 96 registers, 20 warps per SM)
-template <int MODEL, bool BWD, int MINB = 0>
+// SHARD: the entity-sharded step (MarginStepParams::hrows).  The positive's h / t come from hrows /
+// trows, the draw loop keeps only the negatives whose replaced entity this rank holds (ballot +
+// prefix, local row numbers in `codes`), so the ring streams owned rows only, and the positive's
+// gradients go to grad_hrows / grad_trows[w].
+template <int MODEL, bool BWD, int MINB = 0, bool SHARD = false>
 __global__ void __launch_bounds__(WARPS_PER_BLOCK * 32, MINB == 0 ? 1 : MINB)
 margin_step_ring_kernel(MarginStepParams a, TrainGrads gr, const float* __restrict__ gloss) {
   extern __shared__ __align__(128) unsigned char ring_smem[];
@@ -711,33 +880,53 @@ margin_step_ring_kernel(MarginStepParams a, TrainGrads gr, const float* __restri
   const long long hi = a.h[w], ti = a.t[w], ri = a.r[w];
   const float p_head = a.nh ? 0.f : a.probs[ri];
   // ---- all corruptions of this positive, up front: code = entity | head flag ----
-  for (int j0 = 0; j0 < a.n_neg; j0 += 32) {
-    const int j = j0 + lane;
-    if (j < a.n_neg) {
-      const long long idx = (long long)j * a.b + w;
-      long long nh = hi, nt = ti;
-      if (a.nh) { nh = a.nh[idx]; nt = a.nt[idx]; }
-      else corrupt_one(a.seed, a.offset, (uint64_t)idx, p_head, a.n_ent, hi, ti, &nh, &nt);
-      if (!BWD && a.nh_out) { a.nh_out[idx] = nh; a.nt_out[idx] = nt; }
-      const bool head = nh != hi;
-      codes[j] = (nh != hi && nt != ti) ? CODE_BOTH : ((unsigned)(head ? nh : nt) | (head ? 0x80000000u : 0u));
+  int n_loop = a.n_neg;            // SHARD: the owned negatives, compacted to the front of `codes`
+  if constexpr (SHARD) {
+    n_loop = 0;
+    for (int j0 = 0; j0 < a.n_neg; j0 += 32) {
+      const int j = j0 + lane;
+      bool own = false;
+      unsigned code = 0u;
+      if (j < a.n_neg) {
+        long long e;
+        const bool head = draw_one(a.seed, a.offset, (uint64_t)((long long)j * a.b + w), p_head, a.n_ent, &e);
+        const unsigned long long loc = (unsigned long long)(e - a.ent_lo);
+        own = loc < (unsigned long long)a.n_rows;      // n_rows < 2^31 (ring_step_ok)
+        code = (unsigned)loc | (head ? 0x80000000u : 0u);
+      }
+      const unsigned ball = __ballot_sync(0xffffffffu, own);
+      if (own) codes[n_loop + __popc(ball & ((1u << lane) - 1u))] = code;
+      n_loop += __popc(ball);
+    }
+  } else {
+    for (int j0 = 0; j0 < a.n_neg; j0 += 32) {
+      const int j = j0 + lane;
+      if (j < a.n_neg) {
+        const long long idx = (long long)j * a.b + w;
+        long long nh = hi, nt = ti;
+        if (a.nh) { nh = a.nh[idx]; nt = a.nt[idx]; }
+        else corrupt_one(a.seed, a.offset, (uint64_t)idx, p_head, a.n_ent, hi, ti, &nh, &nt);
+        if (!BWD && a.nh_out) { a.nh_out[idx] = nh; a.nt_out[idx] = nt; }
+        const bool head = nh != hi;
+        codes[j] = (nh != hi && nt != ti) ? CODE_BOTH : ((unsigned)(head ? nh : nt) | (head ? 0x80000000u : 0u));
+      }
     }
   }
   __syncwarp();
   auto request = [&](int j) {      // lane 0: start the copy of negative j's row into its slot
     const unsigned code = codes[j];
-    if (code == CODE_BOTH) return;
+    if (!SHARD && code == CODE_BOTH) return;
     const int slot = j % RING;
     ptx::mbar_arrive_expect_tx(&bars[slot], row_bytes);
     ptx::bulk_g2s(ring + (size_t)slot * dim, ent + (size_t)(code & 0x7FFFFFFFu) * dim, row_bytes, &bars[slot]);
   };
   if (lane == 0) {
-    const int first = a.n_neg < RING ? a.n_neg : RING;
+    const int first = n_loop < RING ? n_loop : RING;
     for (int j = 0; j < first; ++j) request(j);
   }
   // ---- the positive (its three rows come straight from global memory, once) ----
-  const Vec h = vec_load(ent + (size_t)hi * dim, dim, lane);
-  const Vec t = vec_load(ent + (size_t)ti * dim, dim, lane);
+  const Vec h = vec_load(SHARD ? a.hrows + (size_t)w * dim : ent + (size_t)hi * dim, dim, lane);
+  const Vec t = vec_load(SHARD ? a.trows + (size_t)w * dim : ent + (size_t)ti * dim, dim, lane);
   const Vec r = vec_load(a.tb.rel0 + (size_t)ri * dim, dim, lane);
   float sh = vec_dot(h, h), stt = vec_dot(t, t);
   warp_sum2(sh, stt);
@@ -770,10 +959,10 @@ margin_step_ring_kernel(MarginStepParams a, TrainGrads gr, const float* __restri
   for (int i = 0; i < FAST_NCH; ++i) Vt.c[i] = Vh.c[i] = make_float4(0.f, 0.f, 0.f, 0.f);
   int n_t = 0, n_h = 0;
   unsigned phases = 0u;   // bit s = parity of the next completion of slot s (a skipped use does not advance it)
-  for (int j = 0; j < a.n_neg; ++j) {
+  for (int j = 0; j < n_loop; ++j) {
     const unsigned code = codes[j];
-    const long long idx = (long long)j * a.b + w;
-    if (code == CODE_BOTH) {
+    const long long idx = (long long)j * a.b + w;   // (unsharded: the negative's index in nh / nt / neg_out)
+    if (!SHARD && code == CODE_BOTH) {
       // both ends replaced (possible with caller-supplied negatives only): generic path, no ring slot
       const long long nh = a.nh[idx], nt = a.nt[idx];
       const RowPtrs pn = make_rows(MODEL, dim, a.tb, nh, nt, ri);
@@ -784,11 +973,11 @@ margin_step_ring_kernel(MarginStepParams a, TrainGrads gr, const float* __restri
         loss += fmaxf(0.f, v);
       }
       if (BWD && v > 0.f) {
-        triple_backward(MODEL, dim, pn, gr, nh, nt, ri, g, lane);
+        triple_backward(MODEL, dim, pn, grad_rows(MODEL, dim, gr, nh, nt, ri), g, lane);
         const RowPtrs pp = make_rows(MODEL, dim, a.tb, hi, ti, ri);
-        triple_backward(MODEL, dim, pp, gr, hi, ti, ri, -g, lane);
+        triple_backward(MODEL, dim, pp, grad_rows(MODEL, dim, gr, hi, ti, ri), -g, lane);
       }
-      if (lane == 0 && j + RING < a.n_neg) request(j + RING);
+      if (lane == 0 && j + RING < n_loop) request(j + RING);
       continue;
     }
     const int slot = j % RING;
@@ -796,7 +985,7 @@ margin_step_ring_kernel(MarginStepParams a, TrainGrads gr, const float* __restri
     phases ^= 1u << slot;
     const Vec ev = vec_load_smem(ring + (size_t)slot * dim, dim, lane);
     __syncwarp();                        // every lane has its copy: the slot may be refilled
-    if (lane == 0 && j + RING < a.n_neg) {
+    if (lane == 0 && j + RING < n_loop) {
       ptx::fence_proxy_async();          // generic-proxy reads above, async-proxy write below
       request(j + RING);
     }
@@ -880,8 +1069,8 @@ margin_step_ring_kernel(MarginStepParams a, TrainGrads gr, const float* __restri
   warp_sum2(ph, pt);
   const Vec gh = vec_map(Gh, hn, [=](float gg, float q) { return (gg - q * ph) * inv_h; });
   const Vec gt = vec_map(Gt, tn, [=](float gg, float q) { return (gg - q * pt) * inv_t; });
-  vec_atomic_add(gr.ent0 + (size_t)hi * dim, dim, lane, gh);
-  vec_atomic_add(gr.ent0 + (size_t)ti * dim, dim, lane, gt);
+  vec_atomic_add(SHARD ? a.grad_hrows + (size_t)w * dim : gr.ent0 + (size_t)hi * dim, dim, lane, gh);
+  vec_atomic_add(SHARD ? a.grad_trows + (size_t)w * dim : gr.ent0 + (size_t)ti * dim, dim, lane, gt);
   vec_atomic_add(gr.rel0 + (size_t)ri * dim, dim, lane, Gr);
 }
 
@@ -889,13 +1078,15 @@ __host__ inline size_t ring_smem_bytes(const MarginStepParams& a) {
   const size_t per_warp = (size_t)RING * a.dim * 4 + (size_t)((a.n_neg + 3) & ~3) * 4 + RING * sizeof(uint64_t);
   return WARPS_PER_BLOCK * ((per_warp + 127) & ~(size_t)127);
 }
-// KGE_TRAIN_RING=0 selects the register-resident form (margin_step_fast_kernel)
+// KGE_TRAIN_RING=0 selects the register-resident form (margin_step_fast_kernel; the sharded step then
+// takes the generic kernels).  Codes hold 31-bit row numbers: of the table, or of the shard.
 __host__ inline bool ring_step_ok(const MarginStepParams& a) {
   static const bool enabled = [] { const char* v = getenv("KGE_TRAIN_RING"); return !(v && v[0] == '0'); }();
-  return enabled && a.n_neg <= 8192 && a.n_ent < 0x7FFFFFFFll && ring_smem_bytes(a) <= 96 * 1024;
+  const long long rows = a.hrows ? a.n_rows : a.n_ent;
+  return enabled && a.n_neg <= 8192 && rows < 0x7FFFFFFFll && ring_smem_bytes(a) <= 96 * 1024;
 }
 
-template <int MODEL, bool BWD, int MINB>
+template <int MODEL, bool BWD, int MINB, bool SHARD = false>
 cudaError_t launch_ring_variant(const MarginStepParams& a, const TrainGrads& gr, const float* gloss, cudaStream_t st) {
   const size_t smem = ring_smem_bytes(a);
   static bool configured[64] = {};
@@ -903,19 +1094,21 @@ cudaError_t launch_ring_variant(const MarginStepParams& a, const TrainGrads& gr,
   cudaError_t e = cudaGetDevice(&dev);
   if (e != cudaSuccess) return e;
   if (smem > 48 * 1024 && (dev < 0 || dev >= 64 || !configured[dev])) {
-    e = cudaFuncSetAttribute(margin_step_ring_kernel<MODEL, BWD, MINB>, cudaFuncAttributeMaxDynamicSharedMemorySize,
-                             96 * 1024);
+    e = cudaFuncSetAttribute(margin_step_ring_kernel<MODEL, BWD, MINB, SHARD>,
+                             cudaFuncAttributeMaxDynamicSharedMemorySize, 96 * 1024);
     if (e != cudaSuccess) return e;
     if (dev >= 0 && dev < 64) configured[dev] = true;
   }
   const unsigned blocks = (unsigned)((a.b + WARPS_PER_BLOCK - 1) / WARPS_PER_BLOCK);
-  margin_step_ring_kernel<MODEL, BWD, MINB><<<blocks, WARPS_PER_BLOCK * 32, smem, st>>>(a, gr, gloss);
+  margin_step_ring_kernel<MODEL, BWD, MINB, SHARD><<<blocks, WARPS_PER_BLOCK * 32, smem, st>>>(a, gr, gloss);
   return cudaGetLastError();
 }
 
-// KGE_TRAIN_BWD_BLOCKS=5 holds the backward kernel to 96 registers (5 CTAs = 20 warps per SM)
+// KGE_TRAIN_BWD_BLOCKS=5 holds the backward kernel to 96 registers (5 CTAs = 20 warps per SM; the
+// unsharded step only)
 template <int MODEL, bool BWD>
 cudaError_t launch_ring(const MarginStepParams& a, const TrainGrads& gr, const float* gloss, cudaStream_t st) {
+  if (a.hrows) return launch_ring_variant<MODEL, BWD, 0, true>(a, gr, gloss, st);
   if constexpr (BWD) {
     static const bool tight = [] { const char* v = getenv("KGE_TRAIN_BWD_BLOCKS"); return v && v[0] == '5'; }();
     if (tight) return launch_ring_variant<MODEL, true, 5>(a, gr, gloss, st);
@@ -991,7 +1184,34 @@ inline unsigned blocks_for_warps(long long warps) {
   return (unsigned)((warps + WARPS_PER_BLOCK - 1) / WARPS_PER_BLOCK);
 }
 
+// grad_plane[idx[i] - ent_lo] += rows[i][plane] for the ids this shard holds (the inverse of
+// gather_rows_kernel); one warp per (i, plane) row, atomics because ids repeat.
+__global__ void scatter_rows_add_kernel(float* __restrict__ grad0, float* __restrict__ grad1, int planes,
+                                        long long ent_lo, long long n_rows, int dim,
+                                        const int64_t* __restrict__ idx, long long n,
+                                        const float* __restrict__ rows) {
+  const long long w = ((long long)blockIdx.x * blockDim.x + threadIdx.x) >> 5;
+  const int lane = threadIdx.x & 31;
+  if (w >= n * planes) return;
+  const long long i = w / planes;
+  const int pl = (int)(w - i * planes);
+  const long long row = idx[i] - ent_lo;
+  if (row < 0 || row >= n_rows) return;
+  float* dst = (pl == 0 ? grad0 : (pl == 1 ? grad1 : grad1 + (grad1 - grad0))) + (size_t)row * dim;
+  const float* src = rows + (size_t)w * dim;
+  for (int k = lane; k < dim; k += 32) atomicAdd(dst + k, src[k]);
+}
+
 }  // namespace
+
+cudaError_t launch_scatter_rows_add(float* grad0, float* grad1, int planes, int64_t ent_lo, int64_t n_rows,
+                                    int dim, const int64_t* idx, int64_t n, const float* rows, cudaStream_t st) {
+  const long long warps = (long long)n * planes;
+  if (warps <= 0) return cudaSuccess;
+  scatter_rows_add_kernel<<<blocks_for_warps(warps), WARPS_PER_BLOCK * 32, 0, st>>>(grad0, grad1, planes, ent_lo,
+                                                                                    n_rows, dim, idx, n, rows);
+  return cudaGetLastError();
+}
 
 cudaError_t launch_score_triples_fwd(int model, int dim, const TrainTables& tb, const int64_t* h,
                                      const int64_t* t, const int64_t* r, int64_t n, float* out,
@@ -1021,7 +1241,12 @@ cudaError_t launch_corrupt_batch(const int64_t* h, const int64_t* t, const int64
   return cudaGetLastError();
 }
 
+cudaError_t launch_margin_step_shard_fwd(const MarginStepParams& a, cudaStream_t st);
+cudaError_t launch_margin_step_shard_bwd(const MarginStepParams& a, const TrainGrads& gr, const float* gloss,
+                                         cudaStream_t st);
+
 cudaError_t launch_margin_step_fwd(const MarginStepParams& a, cudaStream_t st) {
+  if (a.hrows) return launch_margin_step_shard_fwd(a, st);
   if (a.b <= 0) return cudaSuccess;
   if (fast_step_ok(a) && ring_step_ok(a)) {
     const TrainGrads none{nullptr, nullptr, nullptr, nullptr};
@@ -1045,8 +1270,39 @@ cudaError_t launch_margin_step_fwd(const MarginStepParams& a, cudaStream_t st) {
   return cudaGetLastError();
 }
 
+// Entity-sharded step: the ring kernel's SHARD form where it applies, else the generic sharded kernels
+// (the register-resident form has no sharded variant).
+cudaError_t launch_margin_step_shard_fwd(const MarginStepParams& a, cudaStream_t st) {
+  if (a.b <= 0 || a.n_rows <= 0) return cudaSuccess;   // nothing held: no negative is scored here
+  if (fast_step_ok(a) && ring_step_ok(a)) {
+    const TrainGrads none{nullptr, nullptr, nullptr, nullptr};
+    switch (a.model) {
+      case KGE_TRANSE_L1: return launch_ring<KGE_TRANSE_L1, false>(a, none, nullptr, st);
+      case KGE_TRANSE_L2: return launch_ring<KGE_TRANSE_L2, false>(a, none, nullptr, st);
+      default: return launch_ring<KGE_DISTMULT, false>(a, none, nullptr, st);
+    }
+  }
+  margin_step_shard_fwd_kernel<<<blocks_for_warps(a.b), WARPS_PER_BLOCK * 32, 0, st>>>(a);
+  return cudaGetLastError();
+}
+
+cudaError_t launch_margin_step_shard_bwd(const MarginStepParams& a, const TrainGrads& gr, const float* gloss,
+                                         cudaStream_t st) {
+  if (a.b <= 0 || a.n_rows <= 0) return cudaSuccess;
+  if (fast_step_ok(a) && ring_step_ok(a)) {
+    switch (a.model) {
+      case KGE_TRANSE_L1: return launch_ring<KGE_TRANSE_L1, true>(a, gr, gloss, st);
+      case KGE_TRANSE_L2: return launch_ring<KGE_TRANSE_L2, true>(a, gr, gloss, st);
+      default: return launch_ring<KGE_DISTMULT, true>(a, gr, gloss, st);
+    }
+  }
+  margin_step_shard_bwd_kernel<<<blocks_for_warps(a.b), WARPS_PER_BLOCK * 32, 0, st>>>(a, gr, gloss);
+  return cudaGetLastError();
+}
+
 cudaError_t launch_margin_step_bwd(const MarginStepParams& a, const TrainGrads& gr, const float* gloss,
                                    cudaStream_t st) {
+  if (a.hrows) return launch_margin_step_shard_bwd(a, gr, gloss, st);
   if (a.b <= 0) return cudaSuccess;
   if (fast_step_ok(a) && ring_step_ok(a)) {
     switch (a.model) {

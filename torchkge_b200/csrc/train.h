@@ -40,6 +40,15 @@ struct MarginStepParams {
   float* neg_out;  // optional (b * n_neg)
   int64_t* nh_out;  // optional
   int64_t* nt_out;
+  // Entity-sharded step (hrows != nullptr): tb.ent0 / ent1 hold rows [ent_lo, ent_lo + n_rows) of a
+  // range-partitioned table, n_ent is the global count the draws use, the positive rows come from
+  // hrows / trows and only the negatives whose replaced entity is held here are scored.
+  long long ent_lo;
+  long long n_rows;
+  const float* hrows;  // [b][planes][dim]
+  const float* trows;
+  float* grad_hrows;   // [b][planes][dim], +=
+  float* grad_trows;
 };
 
 cudaError_t launch_score_triples_fwd(int model, int dim, const TrainTables& tb, const int64_t* h,
@@ -54,6 +63,8 @@ cudaError_t launch_corrupt_batch(const int64_t* h, const int64_t* t, const int64
 cudaError_t launch_margin_step_fwd(const MarginStepParams& a, cudaStream_t st);
 cudaError_t launch_margin_step_bwd(const MarginStepParams& a, const TrainGrads& gr, const float* gloss,
                                    cudaStream_t st);
+cudaError_t launch_scatter_rows_add(float* grad0, float* grad1, int planes, int64_t ent_lo, int64_t n_rows,
+                                    int dim, const int64_t* idx, int64_t n, const float* rows, cudaStream_t st);
 cudaError_t launch_margin_loss_fwd(const float* pos, const float* neg, int64_t n, float margin,
                                    float* loss, cudaStream_t st);
 cudaError_t launch_pair_loss_fwd(int kind, const float* pos, const float* neg, int64_t n, float* loss,

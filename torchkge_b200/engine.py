@@ -3,8 +3,9 @@
 Nothing here computes scores: torch is used for device memory, streams and (when the entity
 table is range-partitioned) the collectives of the sharded paths.  The only engine is the CUDA one; tests
 may substitute an object with the same methods (``pack``, ``gather_rows``, ``rank_side``,
-``score_all``; ``topk_side`` / ``topk_merge`` for top-k inference) to exercise the sharding logic
-on CPU.
+``score_all``; ``topk_side`` / ``topk_merge`` for top-k inference; ``margin_step_fwd`` /
+``margin_step_bwd`` / ``scatter_rows_add`` for the sharded training step) to exercise the sharding
+logic on CPU.
 """
 import ctypes
 import os
@@ -131,6 +132,14 @@ class ModelSpec:
 
 def _ptr(t):
     return None if t is None else ctypes.c_void_p(t.data_ptr())
+
+
+def _plane_ptrs(x0, x1):
+    """(plane 0, plane 1) pointers of a table: a stacked (3, n, dim) tensor stands for three equally
+    spaced planes, of which the C ABI takes the first two (include/kge_b200.h, "three-plane tables")."""
+    if x0 is not None and x0.dim() == 3:
+        return _ptr(x0[0]), _ptr(x0[1])
+    return _ptr(x0), _ptr(x1)
 
 
 def _equally_spaced(p0, p1, p2):
@@ -419,6 +428,58 @@ class CudaEngine:
                    "kge_finalize_ranks")
         self.launches += 1
         return ranks, filt
+
+    # ---- entity-sharded fused training step (torchkge_b200.training.sharded_margin_step) ----
+    @staticmethod
+    def _shard_step_args(step, tables, h, t, r, probs, loss, hrows, trows):
+        _need_cuda(tables[0], h, hrows, trows)
+        a = _lib.MarginStepArgs()
+        a.tb = _lib.Tables()
+        a.tb.model, a.tb.dim = step.code, step.dim
+        a.tb.ent0, a.tb.ent1 = _plane_ptrs(tables[0], tables[1])
+        a.tb.rel0, a.tb.rel1 = _plane_ptrs(tables[2], tables[3])
+        a.n_neg, a.margin, a.b, a.n_ent = step.n_neg, step.margin, h.shape[0], step.n_ent
+        a.h, a.t, a.r, a.bern_probs = _ptr(h), _ptr(t), _ptr(r), _ptr(probs)
+        a.seed, a.offset = step.seed, step.offset
+        a.loss, a.stream = _ptr(loss), _stream(h.device)
+        a.ent_lo, a.n_rows = step.ent_lo, step.n_rows
+        a.hrows, a.trows = _ptr(hrows), _ptr(trows)
+        return a
+
+    def margin_step_fwd(self, step, tables, h, t, r, probs, hrows, trows):
+        """Sum of the hinge terms of the negatives this shard scores (float32 scalar tensor): the
+        negatives whose replaced entity lies in [step.ent_lo, step.ent_lo + step.n_rows).  ``tables``:
+        (ent0, ent1, rel0, rel1) with this shard's entity rows (a three-plane table as one stacked
+        (3, n, dim) tensor in ent0 / rel0); hrows / trows: (b, planes, dim) rows of every positive."""
+        loss = torch.zeros((), dtype=torch.float32, device=h.device)
+        a = self._shard_step_args(step, tables, h, t, r, probs, loss, hrows, trows)
+        _lib.check(self.lib.kge_margin_step_fwd(ctypes.byref(a)), "kge_margin_step_fwd")
+        self.launches += 1
+        return loss
+
+    def margin_step_bwd(self, step, tables, grads, h, t, r, probs, gloss, hrows, trows, grad_hrows, grad_trows):
+        """Backward of margin_step_fwd, added into ``grads`` (gradient tensors shaped like ``tables``)
+        and grad_hrows / grad_trows (b, planes, dim)."""
+        dummy = torch.zeros((), dtype=torch.float32, device=h.device)   # the loss is not recomputed
+        a = self._shard_step_args(step, tables, h, t, r, probs, dummy, hrows, trows)
+        a.grad_hrows, a.grad_trows = _ptr(grad_hrows), _ptr(grad_trows)
+        g = _lib.Grads()
+        g.ent0, g.ent1 = _plane_ptrs(grads[0], grads[1])
+        g.rel0, g.rel1 = _plane_ptrs(grads[2], grads[3])
+        _lib.check(self.lib.kge_margin_step_bwd(ctypes.byref(a), ctypes.byref(g), _ptr(gloss)),
+                   "kge_margin_step_bwd")
+        self.launches += 1
+
+    def scatter_rows_add(self, code, dim, grad0, grad1, ent_lo, idx, rows):
+        """grad[idx[i] - ent_lo] += rows[i] plane by plane for the ids this shard holds, others ignored
+        (kge_scatter_rows_add); grad0 / grad1 as in _plane_ptrs, rows (n, planes, dim)."""
+        _need_cuda(grad0, idx, rows)
+        g0, g1 = _plane_ptrs(grad0, grad1)
+        rows = rows.contiguous()
+        _lib.check(self.lib.kge_scatter_rows_add(code, g0, g1, ent_lo, grad0.shape[-2], dim, _ptr(idx),
+                                                 idx.shape[0], _ptr(rows), _stream(rows.device)),
+                   "kge_scatter_rows_add")
+        self.launches += 1
 
 
 _default_engine = None

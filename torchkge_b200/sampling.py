@@ -135,16 +135,23 @@ class BernoulliNegativeSampler(NegativeSampler):
                    "kge_corrupt_batch")
         return nh, nt
 
-    def fused_step(self, model, heads, tails, relations, margin, n_neg=None):
+    def fused_step(self, model, heads, tails, relations, margin, n_neg=None, *, shard=None):
         """Extension: corruption + ``model(...)`` + ``MarginLoss(margin)`` in ONE kernel; returns
         the differentiable scalar loss.  Draws the negatives ``corrupt_batch`` would draw at the
-        same call count."""
+        same call count.
+
+        shard: ``EntityShard(local_storage=True)`` for a model holding only its entity rows (see
+        ``training.fused_margin_step``); every rank uses a sampler with the same seed and call count,
+        built on the whole graph, and passes the same batch."""
         if n_neg is None:
             n_neg = self.n_neg
+        if shard is not None and getattr(shard, "n_ent", self.n_ent) != self.n_ent:
+            raise ValueError("the sampler draws on %d entities, the shard partitions %d"
+                             % (self.n_ent, shard.n_ent))
         self.bern_probs = self.bern_probs.to(heads.device)
         return fused_margin_step(model, heads, tails, relations, margin, n_neg=n_neg,
                                  bern_probs=self.bern_probs, seed=self.seed,
-                                 offset=self._next_offset())
+                                 offset=self._next_offset(), shard=shard)
 
 
 class PositionalNegativeSampler(BernoulliNegativeSampler):

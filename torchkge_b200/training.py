@@ -3,12 +3,15 @@
 kernels of csrc/train.cu.  Gradients are dense tables (what ``nn.Embedding`` yields in the
 reference), accumulated with atomics.
 """
+import collections
 import ctypes
+import struct
 
 import torch
 
 from . import _lib
-from .engine import ModelSpec, _ptr, _stream
+from .engine import (EntityShard, ModelSpec, QueryShard, _device_guard, _exchanged_rows, _plane_ptrs, _ptr,
+                     _stream, default_engine)
 
 
 def _param_tensors(model, code):
@@ -35,14 +38,6 @@ def _param_tensors(model, code):
 def _kernel_dim(model, code):
     """Width of one plane: emb_dim, or Analogy's scalar_dim (= complex_dim on this path)."""
     return model.scalar_dim if code == _lib.ANALOGY else model.emb_dim
-
-
-def _plane_ptrs(x0, x1):
-    """(plane 0, plane 1) pointers of a table: a stacked (3, n, dim) tensor stands for three equally
-    spaced planes, of which the C ABI takes the first two (include/kge_b200.h, "three-plane tables")."""
-    if x0 is not None and x0.dim() == 3:
-        return _ptr(x0[0]), _ptr(x0[1])
-    return _ptr(x0), _ptr(x1)
 
 
 def _tables(code, dim, tensors):
@@ -249,8 +244,129 @@ class _MarginStep(torch.autograd.Function):
         return (None,) * 13 + tuple(gs)
 
 
+#: what every rank's kernels of one sharded step are told (engine.margin_step_fwd / _bwd)
+ShardedStep = collections.namedtuple("ShardedStep", "code dim n_ent ent_lo n_rows n_neg margin seed offset")
+
+
+class _ShardedMarginStep(torch.autograd.Function):
+    """The fused margin step on a range-partitioned entity table (EntityShard, local storage):
+      1. the positives' h / t rows: each rank gathers the rows it holds, one sum-all-reduce;
+      2. every rank draws all negatives with the global n_ent and scores those whose replaced entity
+         it holds (the intact entity's row comes from step 1, the relation table is replicated);
+      3. one all-reduce of the scalar loss.
+    Backward: replaced rows go straight into the local gradient; the gradients of the positives' rows
+    (grad_hrows / grad_trows) and of the relations are summed over the ranks by ONE all-reduce, after
+    which every rank adds the rows it holds into its entity gradient.  Communication per step:
+    2 b planes dim floats forward, the same plus the relation table backward -- independent of n_neg."""
+
+    @staticmethod
+    def forward(ctx, step, shard, engine, h, t, r, probs, ent0, ent1, rel0, rel1):
+        tensors = [None if x is None else x.detach().contiguous() for x in (ent0, ent1, rel0, rel1)]
+        dev = tensors[2].device
+        h, t, r = _idx(h, dev), _idx(t, dev), _idx(r, dev)
+        probs = probs.to(device=dev, dtype=torch.float32).contiguous()
+        b = h.shape[0]
+        with _device_guard(dev):
+            spec = _row_spec(step, tensors)
+            rows = _exchanged_rows(spec, torch.cat([h, t]), shard, engine)   # (2b, planes, dim)
+            hrows, trows = rows[:b], rows[b:]
+            if step.n_rows > 0:
+                loss = engine.margin_step_fwd(step, tensors, h, t, r, probs, hrows, trows)
+            else:             # holds no entity: scores no negative, still joins every collective
+                loss = torch.zeros((), dtype=torch.float32, device=dev)
+            shard.all_reduce_sum(loss)
+        ctx.step, ctx.shard, ctx.engine = step, shard, engine
+        ctx.present = [x is not None for x in tensors]
+        ctx.save_for_backward(h, t, r, probs, rows, *[x for x in tensors if x is not None])
+        return loss
+
+    @staticmethod
+    def backward(ctx, gl):
+        step, shard, engine = ctx.step, ctx.shard, ctx.engine
+        saved = list(ctx.saved_tensors)
+        h, t, r, probs, rows = saved[:5]
+        it = iter(saved[5:])
+        tensors = [next(it) if p else None for p in ctx.present]
+        dev = h.device
+        b = h.shape[0]
+        gl = gl.detach().to(device=dev, dtype=torch.float32).contiguous()
+        # grad_hrows, grad_trows and the relation gradients are views of ONE buffer: one all-reduce
+        sizes = [rows.numel()] + [0 if x is None else x.numel() for x in tensors[2:]]
+        flat = torch.zeros(sum(sizes), dtype=torch.float32, device=dev)
+        grad_rows = flat[:sizes[0]].view(rows.shape)
+        grel = [None if x is None else part.view(x.shape)
+                for x, part in zip(tensors[2:], flat[sizes[0]:].split(sizes[1:]))]
+        gent = [None if x is None else torch.zeros_like(x, dtype=torch.float32) for x in tensors[:2]]
+        grads = gent + grel
+        with _device_guard(dev):
+            if step.n_rows > 0:
+                engine.margin_step_bwd(step, tensors, grads, h, t, r, probs, gl, rows[:b], rows[b:],
+                                       grad_rows[:b], grad_rows[b:])
+            shard.all_reduce_sum(flat)
+            if step.n_rows > 0:
+                engine.scatter_rows_add(step.code, step.dim, gent[0], gent[1], step.ent_lo, torch.cat([h, t]),
+                                        grad_rows)
+        return (None,) * 7 + tuple(grads)
+
+
+def _row_spec(step, tensors):
+    """ModelSpec over this shard's entity rows, for the positive-row gather (engine.gather_rows)."""
+    e0, e1, r0, r1 = tensors
+    e2 = r2 = None
+    if e0.dim() == 3:            # Analogy: stacked (3, n, dim) planes
+        e0, e1, e2 = e0[0], e0[1], e0[2]
+        r0, r1, r2 = r0[0], r0[1], r0[2]
+    return ModelSpec(step.code, step.dim, step.n_ent, r0.shape[0], e0, e1, r0, r1, ent_lo=step.ent_lo,
+                     ent2=e2, rel2=r2)
+
+
+def _signed64(x):
+    x = int(x) & 0xFFFFFFFFFFFFFFFF
+    return x - (1 << 64) if x >= (1 << 63) else x
+
+
+def sharded_margin_step(model, heads, tails, relations, margin, n_neg, bern_probs, seed, offset, shard,
+                        engine=None):
+    """``fused_margin_step(..., shard=shard)`` for a model that holds only the entity rows
+    [shard.lo, shard.hi) of an EntityShard with local storage; the same (heads, tails, relations),
+    seed, offset, n_neg and margin on every rank.  Returns the full loss on every rank; its backward
+    leaves every rank with the gradient of its own rows and the (identical) relation gradient.
+    ``engine``: CudaEngine or a stand-in with margin_step_fwd / margin_step_bwd / scatter_rows_add /
+    gather_rows."""
+    # argument errors first, on every rank: none of them may leave the others waiting in a collective
+    if isinstance(shard, QueryShard):
+        raise ValueError("the fused training step takes an EntityShard; QueryShard (data-parallel "
+                         "replicas) is not supported")
+    if not isinstance(shard, EntityShard):
+        raise ValueError("shard must be an EntityShard, got %s" % type(shard).__name__)
+    if not shard.local_storage:
+        raise ValueError("the sharded training step needs EntityShard(local_storage=True): the model "
+                         "holds only rows [lo, hi)")
+    if bern_probs is None:
+        raise ValueError("bern_probs must be given (a sharded step draws its own negatives)")
+    code = _training_code(model)
+    ent0, ent1, rel0, rel1 = _param_tensors(model, code)
+    held = int(ent0.shape[-2])
+    if held != shard.hi - shard.lo or int(model.n_ent) != held:
+        raise ValueError("the model holds %d entity rows, the shard's range [%d, %d) has %d"
+                         % (held, shard.lo, shard.hi, shard.hi - shard.lo))
+    b = int(heads.shape[0])
+    step = ShardedStep(code, _kernel_dim(model, code), shard.n_ent, shard.lo, held, int(n_neg), float(margin),
+                       int(seed) & 0xFFFFFFFFFFFFFFFF, int(offset) & 0xFFFFFFFFFFFFFFFF)
+    # one small collective: every rank must draw the same negatives for the same batch
+    mine = torch.tensor([_signed64(step.seed), _signed64(step.offset), b, step.n_neg,
+                         struct.unpack("<q", struct.pack("<d", step.margin))[0]],
+                        dtype=torch.int64, device=rel0.device)
+    everyone = shard.stack_all(mine)
+    if not bool((everyone == mine).all()):
+        raise ValueError("the ranks of a sharded step disagree on (seed, offset, batch size, n_neg, margin): "
+                         "%s" % everyone.tolist())
+    return _ShardedMarginStep.apply(step, shard, engine or default_engine(), heads, tails, relations,
+                                    bern_probs, ent0, ent1, rel0, rel1)
+
+
 def fused_margin_step(model, heads, tails, relations, margin, n_neg=1, negatives=None,
-                      bern_probs=None, seed=0, offset=0):
+                      bern_probs=None, seed=0, offset=0, *, shard=None):
     """Loss of one training step, fused: Bernoulli corruption (or the given ``negatives =
     (neg_heads, neg_tails)``), ``model(h, t, r, nh, nt)`` and ``MarginLoss(margin)`` in a
     single kernel, differentiable with respect to the embedding tables.
@@ -259,7 +375,18 @@ def fused_margin_step(model, heads, tails, relations, margin, n_neg=1, negatives
         nh, nt = sampler.corrupt_batch(h, t, r); pos, neg = model(h, t, r, nh, nt)
         loss = criterion(pos, neg)
     without materialising nh, nt, pos, neg.
+
+    shard: ``EntityShard(local_storage=True)`` when the model holds only the entity rows [lo, hi) of
+        a table range-partitioned over a process group (sharded_margin_step).  Every rank passes the
+        same batch, seed, offset, n_neg and margin -- the batch contents are not checked -- and gets
+        the full loss; the negatives are drawn on [1, shard.n_ent).  External negatives are not
+        supported in this mode.
     """
+    if shard is not None:
+        if negatives is not None:
+            raise ValueError("external negatives are not supported by the sharded training step")
+        return sharded_margin_step(model, heads, tails, relations, margin, n_neg, bern_probs, seed, offset,
+                                   shard)
     spec_code = _training_code(model)
     ent0, ent1, rel0, rel1 = _param_tensors(model, spec_code)
     nh = nt = None
