@@ -39,7 +39,7 @@
 extern "C" {
 #endif
 
-#define KGE_ABI_VERSION 10
+#define KGE_ABI_VERSION 11
 
 /* error codes */
 #define KGE_OK 0
@@ -373,7 +373,9 @@ int kge_margin_loss_bwd(const float* pos, const float* neg, int64_t n, float mar
  * and BinaryCrossEntropyLoss (utils/losses.py:81-112: BCELoss(sum) of sigmoid(pos) vs 1 and
  * sigmoid(neg) vs 0, log clamped at -100 as torch does):
  *   kind 1: loss += sum_i log(1 + exp(-pos[i])) + log(1 + exp(neg[i]))
- *   kind 2: loss += sum_i -max(log(sig(pos[i])), -100) - max(log(1 - sig(neg[i])), -100) */
+ *   kind 2: loss += sum_i -max(log(sig(pos[i])), -100) - max(log(1 - sig(neg[i])), -100)
+ * Kind 0 (MarginLoss) is a loss kind of the fused step only (kge_margin_step_args_t.loss_kind). */
+#define KGE_LOSS_MARGIN 0
 #define KGE_LOSS_LOGISTIC 1
 #define KGE_LOSS_BCE 2
 int kge_pair_loss_fwd(int kind, const float* pos, const float* neg, int64_t n, float* loss, void* stream);
@@ -381,10 +383,15 @@ int kge_pair_loss_bwd(int kind, const float* pos, const float* neg, int64_t n, c
                       float* grad_pos, float* grad_neg, void* stream);
 
 /* Fused training step = corrupt_batch + Model.forward (models/interfaces.py:39-82) +
- * MarginLoss in one kernel: one warp per positive triple scores it and its n_neg negatives;
+ * the loss in one kernel: one warp per positive triple scores it and its n_neg negatives;
  * no (b*n_neg) index or score tensor is materialised unless the optional outputs are given.
  * Negatives: nh/nt if non-NULL (deterministic mode), else drawn in-kernel exactly as
  * kge_corrupt_batch would with the same (seed, offset).
+ *
+ * Loss (loss_kind): KGE_LOSS_MARGIN (MarginLoss(margin)), KGE_LOSS_LOGISTIC (LogisticLoss) or
+ * KGE_LOSS_BCE (BinaryCrossEntropyLoss), summed over every (positive i, negative j) pair with the
+ * per-pair terms of kge_pair_loss_fwd; margin is ignored unless loss_kind == KGE_LOSS_MARGIN.  Any
+ * other kind returns KGE_ERR_ARG.  A zero-initialised loss_kind is the margin step of ABI 10.
  *
  * Entity-sharded step (hrows != NULL).  The entity table is range-partitioned: tb.ent0 / ent1 hold
  * the rows [ent_lo, ent_lo + n_rows) (n_rows = 0 is valid), n_ent is the GLOBAL entity count the draws
@@ -418,6 +425,7 @@ typedef struct {
   int64_t n_rows;                       /* sharded: rows held */
   const float* hrows; const float* trows;   /* sharded: [b][planes][dim] positive rows, or NULL */
   float* grad_hrows; float* grad_trows;     /* sharded backward: [b][planes][dim], += */
+  int32_t loss_kind;                    /* KGE_LOSS_MARGIN (0), KGE_LOSS_LOGISTIC or KGE_LOSS_BCE */
 } kge_margin_step_args_t;
 int kge_margin_step_fwd(const kge_margin_step_args_t* a);
 /* grad_loss: device pointer to the upstream gradient of the scalar loss */

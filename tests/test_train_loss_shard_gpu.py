@@ -1,0 +1,236 @@
+"""The entity-sharded fused step with LogisticLoss and BinaryCrossEntropyLoss: per-rank kernel calls on
+row ranges of one table, summed over the ranks and scattered as the host logic does, must reproduce the
+unsharded fused step of the same loss -- loss within 1e-5 relative, gradients under the atomics-order
+rule of tests/test_train_gpu.py.  Every rank counts the positive's term only for the negatives it owns.
+Then the public API trains in two processes over gloo on one GPU; the NCCL form needs two GPUs and is
+skipped on a machine with one."""
+import os
+import socket
+
+import pytest
+import torch
+
+import torchkge_b200 as tk
+from tests import helpers
+from torchkge_b200 import _lib
+from torchkge_b200.engine import CudaEngine, EntityShard, _exchanged_rows
+from torchkge_b200.training import ShardedStep, _kernel_dim, _MarginStep, _param_tensors, _row_spec, _training_code
+
+pytestmark = pytest.mark.gpu
+DEV = "cuda:0"
+ALL_KINDS = ["transe_l1", "transe_l2", "distmult", "rescal", "complex", "rotate", "analogy", "toruse_l1",
+             "toruse_l2"]
+KINDS = {"logistic": _lib.LOSS_LOGISTIC, "bce": _lib.LOSS_BCE}
+
+
+def _close_grad(a, b, rtol=1e-4):
+    """as tests/test_train_gpu.py: rtol plus an absolute floor of 1e-5 of the largest entry"""
+    b = b.detach().cpu().float()
+    torch.testing.assert_close(a.detach().cpu().float(), b, rtol=rtol, atol=1e-5 * float(b.abs().max()) + 1e-9)
+
+
+def _leaves(model):
+    code = _training_code(model)
+    ts = [None if x is None else x.detach().clone().contiguous().requires_grad_(True)
+          for x in _param_tensors(model, code)]
+    return code, _kernel_dim(model, code), ts
+
+
+def unsharded(model, h, t, r, probs, loss_kind, n_neg, seed, offset):
+    code, dim, ts = _leaves(model)
+    loss = _MarginStep.apply(code, dim, model.n_ent, 0.0, n_neg, h, t, r, None, None, probs, seed, offset, *ts,
+                             loss_kind)
+    loss.backward()
+    return loss.item(), [None if x is None else x.grad for x in ts]
+
+
+def emulated(model, h, t, r, probs, loss_kind, n_neg, seed, offset, world, eng):
+    """What `world` ranks compute, one rank range after the other on one device (the all-reduces are
+    sums here), then every rank's scatter into its own rows."""
+    code, dim, ts = _leaves(model)
+    tabs = [None if x is None else x.detach() for x in ts]
+    n_ent, b = model.n_ent, h.shape[0]
+    full = ShardedStep(code, dim, n_ent, 0, n_ent, n_neg, 0.0, seed, offset, loss_kind)
+    rows = _exchanged_rows(_row_spec(full, tabs), torch.cat([h, t]), EntityShard(n_ent), eng)
+    hrows, trows = rows[:b], rows[b:]
+    loss = torch.zeros((), dtype=torch.float32, device=DEV)
+    grad_rows = torch.zeros_like(rows)
+    grel = [None if x is None else torch.zeros_like(x) for x in tabs[2:]]
+    gent = [None if x is None else torch.zeros_like(x) for x in tabs[:2]]
+    parts = []
+    for rank in range(world):
+        sh = EntityShard(n_ent, rank, world, local_storage=True)
+        n = sh.hi - sh.lo
+        local = [None if x is None else x.narrow(-2, sh.lo, n) for x in tabs[:2]] + tabs[2:]
+        lg = [None if x is None else x.narrow(-2, sh.lo, n) for x in gent]
+        parts.append((sh, lg))
+        if n == 0:
+            continue
+        step = ShardedStep(code, dim, n_ent, sh.lo, n, n_neg, 0.0, seed, offset, loss_kind)
+        loss += eng.margin_step_fwd(step, local, h, t, r, probs, hrows, trows)
+        g_rows = torch.zeros_like(rows)
+        g_rel = [None if x is None else torch.zeros_like(x) for x in tabs[2:]]
+        gl = torch.ones((), dtype=torch.float32, device=DEV)
+        eng.margin_step_bwd(step, local, lg + g_rel, h, t, r, probs, gl, hrows, trows, g_rows[:b], g_rows[b:])
+        grad_rows += g_rows
+        for a, c in zip(grel, g_rel):
+            if a is not None:
+                a += c
+    for sh, lg in parts:
+        if sh.hi > sh.lo:
+            eng.scatter_rows_add(code, dim, lg[0], lg[1], sh.lo, torch.cat([h, t]), grad_rows)
+    return loss.item(), gent + grel
+
+
+def _batch(n_ent, n_rel, b, seed):
+    g = torch.Generator().manual_seed(seed)
+    h = torch.randint(0, n_ent, (b,), generator=g)
+    t = torch.randint(0, n_ent, (b,), generator=g)
+    r = torch.randint(0, n_rel, (b,), generator=g)
+    probs = torch.rand(n_rel, generator=g)
+    return h.to(DEV), t.to(DEV), r.to(DEV), probs.to(DEV)
+
+
+def _model(kind, d, n_ent, n_rel, seed):
+    model = helpers.make_model(kind, d, n_ent, n_rel, seed=seed)
+    if kind in ("transe_l1", "transe_l2", "distmult", "rescal"):
+        with torch.no_grad():
+            model.ent_emb.weight.mul_(1.0 + torch.rand(n_ent, 1))   # un-normalised rows
+    if kind.startswith("toruse"):
+        model.normalize_parameters()
+    return model.to(DEV)
+
+
+def _compare(got, want, rtol=1e-4):
+    (gl, gg), (wl, wg) = got, want
+    assert gl == pytest.approx(wl, rel=1e-5, abs=1e-6)
+    for a, b in zip(gg, wg):
+        if b is not None:
+            _close_grad(a, b, rtol)
+
+
+# ---------------------------------------------------------------- 1. emulated shards vs unsharded
+RING = [(k, d) for k in ("transe_l1", "transe_l2", "distmult") for d in (36, 200, 256)]
+GENERIC = [(k, 50 if k != "rescal" else 12) for k in ALL_KINDS]
+CASES = [(k, d, (1, 33, 256)[i % 3]) for i, (k, d) in enumerate(RING + GENERIC)]
+
+
+@pytest.mark.parametrize("loss", sorted(KINDS))
+@pytest.mark.parametrize("kind,d,n_neg", CASES, ids=["%s-d%d-neg%d" % c for c in CASES])
+def test_emulated_shards_equal_unsharded(kind, d, n_neg, loss):
+    n_ent, n_rel, b = 700, 40, 160
+    model = _model(kind, d, n_ent, n_rel, seed=3)
+    h, t, r, probs = _batch(n_ent, n_rel, b, seed=d + n_neg)
+    want = unsharded(model, h, t, r, probs, KINDS[loss], n_neg, 99, 5)
+    eng = CudaEngine()
+    for world in (1, 2, 3, 8):
+        _compare(emulated(model, h, t, r, probs, KINDS[loss], n_neg, 99, 5, world, eng), want)
+
+
+@pytest.mark.parametrize("loss", sorted(KINDS))
+@pytest.mark.parametrize("kind,d", [("distmult", 200), ("transe_l1", 36), ("complex", 50), ("analogy", 64),
+                                    ("toruse_l2", 40)])
+def test_empty_shards_and_one_sided_draws(kind, d, loss):
+    """17 entities over 8 ranks (one row per rank or none), Bernoulli probabilities 0 and 1."""
+    n_ent, n_rel, b, n_neg = 17, 4, 64, 33
+    model = _model(kind, d, n_ent, n_rel, seed=13)
+    h, t, r, _ = _batch(n_ent, n_rel, b, seed=14)
+    probs = torch.tensor([0.0, 1.0, 0.5, 0.25], device=DEV)
+    want = unsharded(model, h, t, r, probs, KINDS[loss], n_neg, 7, 3)
+    eng = CudaEngine()
+    for world in (2, 3, 8):
+        _compare(emulated(model, h, t, r, probs, KINDS[loss], n_neg, 7, 3, world, eng), want)
+
+
+# ---------------------------------------------------------------- 2. public API, two processes
+def _free_port():
+    with socket.socket() as s:
+        s.bind(("127.0.0.1", 0))
+        return s.getsockname()[1]
+
+
+def _local_model(kind, model, lo, hi, n_rel, dim):
+    part = helpers.make_model(kind, dim, hi - lo, n_rel, seed=0)
+    part.load_state_dict({name: w[lo:hi] if "ent_emb" in name else w for name, w in model.state_dict().items()})
+    return part.to(next(model.parameters()).device)
+
+
+def _train(model, kg, batches, shard, steps, seed, crit):
+    sampler = tk.BernoulliNegativeSampler(kg, n_neg=16, seed=seed)
+    opt = torch.optim.SGD(model.parameters(), lr=0.05)
+    losses = []
+    for h, t, r in batches[:steps]:
+        opt.zero_grad()
+        loss = sampler.fused_step(model, h, t, r, criterion=crit, shard=shard)
+        loss.backward()
+        opt.step()
+        losses.append(loss.item())
+    return losses
+
+
+def _api_worker(rank, world, port, backend, ret):
+    import torch.distributed as dist
+    os.environ["MASTER_ADDR"] = "127.0.0.1"
+    os.environ["MASTER_PORT"] = str(port)
+    dev = torch.device("cuda:%d" % (rank if backend == "nccl" else 0))
+    torch.cuda.set_device(dev)
+    dist.init_process_group(backend, rank=rank, world_size=world)
+    try:
+        res = {}
+        n_ent, n_rel = 3001, 7
+        hh, tt, rr = helpers.random_graph(n_ent, n_rel, 6000, seed=5)
+        kg = tk.KnowledgeGraph(hh, tt, rr, n_ent, n_rel, dict_of_heads={}, dict_of_tails={})
+        batches = [(hh[i:i + 512].to(dev), tt[i:i + 512].to(dev), rr[i:i + 512].to(dev)) for i in range(0, 2560, 512)]
+        for kind, dim, crit in (("distmult", 200, tk.LogisticLoss()), ("complex", 50, tk.BinaryCrossEntropyLoss())):
+            full = helpers.make_model(kind, dim, n_ent, n_rel, seed=21).to(dev)
+            shard = EntityShard.from_group(n_ent, local_storage=True)
+            local = _local_model(kind, full, shard.lo, shard.hi, n_rel, dim)
+            want = _train(full, kg, batches, None, 5, 3, crit)
+            got = _train(local, kg, batches, shard, 5, 3, crit)
+            everyone = shard.stack_all(torch.tensor(got, dtype=torch.float64, device=dev))
+            res[kind + "/losses_equal_on_ranks"] = bool((everyone == everyone[0]).all())
+            res[kind + "/losses_close"] = all(abs(a - b) <= 1e-5 * abs(b) for a, b in zip(got, want))
+            for name, p in local.named_parameters():
+                ref = dict(full.named_parameters())[name]
+                if "ent_emb" in name:
+                    res[kind + "/" + name] = torch.allclose(p, ref[shard.lo:shard.hi], rtol=1e-4, atol=1e-5)
+                else:
+                    allp = shard.stack_all(p.detach())
+                    res[kind + "/" + name + "/bitwise_on_ranks"] = bool((allp == allp[0]).all())
+                    res[kind + "/" + name] = torch.allclose(p, ref, rtol=1e-4, atol=1e-5)
+        # a loss kind that differs between the ranks raises on every rank instead of hanging
+        sampler = tk.BernoulliNegativeSampler(kg, n_neg=4, seed=100)
+        crit = tk.LogisticLoss() if rank == 0 else tk.BinaryCrossEntropyLoss()
+        try:
+            sampler.fused_step(local, *batches[0], criterion=crit, shard=shard)
+            res["loss_mismatch_raises"] = False
+        except ValueError:
+            res["loss_mismatch_raises"] = True
+        ret[rank] = res
+    except Exception as e:          # reported by the parent
+        ret[rank] = {"error": "%s: %s" % (type(e).__name__, e)}
+    finally:
+        dist.destroy_process_group()
+
+
+def _run_two_ranks(backend):
+    import torch.multiprocessing as mp
+    port = _free_port()
+    mgr = mp.Manager()
+    ret = mgr.dict()
+    mp.spawn(_api_worker, args=(2, port, backend, ret), nprocs=2, join=True)
+    for rank in (0, 1):
+        res = ret[rank]
+        assert "error" not in res, "rank %d: %s" % (rank, res.get("error"))
+        bad = [k for k, v in res.items() if not v]
+        assert not bad and len(res) >= 14, "rank %d: %s" % (rank, res)
+
+
+def test_public_api_two_processes_gloo_one_gpu():
+    _run_two_ranks("gloo")
+
+
+@pytest.mark.skipif(not torch.cuda.is_available() or torch.cuda.device_count() < 2,
+                    reason="needs two GPUs (one NCCL rank per device)")
+def test_public_api_two_processes_nccl():
+    _run_two_ranks("nccl")

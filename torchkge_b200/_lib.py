@@ -15,10 +15,10 @@ LIB_PATH = os.path.join(HERE, "lib", "libkge_b200.so")
 TRANSE_L1, TRANSE_L2, DISTMULT, RESCAL, COMPLEX, ROTATE, TORUSE_L1, TORUSE_L2, ANALOGY = range(9)
 SIDE_TAIL, SIDE_HEAD, SIDE_REL = 0, 1, 2
 TILE_C, TILE_Q = 128, 64
-ABI_VERSION = 10
+ABI_VERSION = 11
 FLAG_TENSOR_CORE = 1
 FLAG_APPROX_SCAN = 2
-LOSS_LOGISTIC, LOSS_BCE = 1, 2
+LOSS_MARGIN, LOSS_LOGISTIC, LOSS_BCE = 0, 1, 2
 
 MODEL_NAMES = {TRANSE_L1: "TransE-L1", TRANSE_L2: "TransE-L2", DISTMULT: "DistMult",
                RESCAL: "RESCAL", COMPLEX: "ComplEx", ROTATE: "RotatE",
@@ -92,6 +92,7 @@ class MarginStepArgs(ctypes.Structure):
         ("stream", _p),
         ("ent_lo", _c.c_int64), ("n_rows", _c.c_int64),
         ("hrows", _p), ("trows", _p), ("grad_hrows", _p), ("grad_trows", _p),
+        ("loss_kind", _c.c_int32),
     ]
 
 

@@ -782,6 +782,7 @@ kge::MarginStepParams to_step(const kge_margin_step_args_t* a) {
   p.neg_out = a->neg_out; p.nh_out = a->nh_out; p.nt_out = a->nt_out;
   p.ent_lo = a->ent_lo; p.n_rows = a->n_rows; p.hrows = a->hrows; p.trows = a->trows;
   p.grad_hrows = a->grad_hrows; p.grad_trows = a->grad_trows;
+  p.loss_kind = a->loss_kind;
   return p;
 }
 // A shard that holds no rows (n_rows = 0) may pass no entity planes.
@@ -806,6 +807,8 @@ bool step_ok(const kge_margin_step_args_t* a) {
   if ((a->nh == nullptr) != (a->nt == nullptr)) return false;
   if (!a->nh && !a->bern_probs) return false;
   if ((a->nh_out == nullptr) != (a->nt_out == nullptr)) return false;
+  if (a->loss_kind != KGE_LOSS_MARGIN && a->loss_kind != KGE_LOSS_LOGISTIC && a->loss_kind != KGE_LOSS_BCE)
+    return false;
   if (a->hrows) {   // entity-sharded: Philox draws only, no per-negative outputs
     if (!a->trows || a->nh || a->pos_out || a->neg_out || a->nh_out) return false;
     if (a->ent_lo < 0 || a->n_rows < 0 || a->ent_lo + a->n_rows > a->n_ent) return false;

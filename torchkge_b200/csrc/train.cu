@@ -1,6 +1,6 @@
 // Training-side kernels: per-triple scoring (Model.scoring_function), Bernoulli corruption
-// (BernoulliNegativeSampler.corrupt_batch), margin loss (MarginLoss) and the fused
-// sample + score + hinge step, each with its backward.
+// (BernoulliNegativeSampler.corrupt_batch), the losses (MarginLoss, LogisticLoss,
+// BinaryCrossEntropyLoss) and the fused sample + score + loss step, each with its backward.
 //
 // Reference bodies replaced: models/translation.py:69-81, models/bilinear.py:60-71, 188-199,
 // 460-473, models/interfaces.py:39-82, sampling.py:278-327, utils/losses.py:12-44.
@@ -16,6 +16,7 @@
 #include <stdint.h>
 
 #include <stdlib.h>
+#include <type_traits>
 
 #include "../../include/kge_b200.h"
 #include "ptx.cuh"
@@ -421,8 +422,46 @@ __global__ void corrupt_batch_kernel(const int64_t* __restrict__ h, const int64_
   nh[gid] = a; nt[gid] = c;
 }
 
+// ---- per-pair loss terms: the one statement of each loss, used by pair_loss_fwd / _bwd_kernel and
+// by every fused step (kind: KGE_LOSS_*, a runtime value or a template constant).
+//   margin  : max(0, margin - pos + neg)                    (MarginRankingLoss, target +1, sum)
+//   logistic: softplus(-pos) + softplus(neg), softplus(x) = max(x, 0) + log1p(exp(-|x|))
+//             (SoftMarginLoss(sum) on (pos, +1) and (neg, -1), utils/losses.py:47-78)
+//   bce     : -max(log(sig(pos)), -100) - max(log(1 - sig(neg)), -100), sig in fp32 as torch does
+//             (BCELoss(sum) of sig(pos) vs 1 and sig(neg) vs 0, utils/losses.py:81-112)
+__device__ __forceinline__ float softplus_f(float x) { return fmaxf(x, 0.f) + log1pf(expf(-fabsf(x))); }
+__device__ __forceinline__ float sigmoid_f(float x) { return 1.0f / (1.0f + expf(-x)); }
+
+__device__ __forceinline__ float pair_loss_term(int kind, float margin, float pos, float neg) {
+  if (kind == KGE_LOSS_MARGIN) return fmaxf(0.f, margin - pos + neg);
+  if (kind == KGE_LOSS_LOGISTIC) return softplus_f(-pos) + softplus_f(neg);
+  const float pp = sigmoid_f(pos), pn = sigmoid_f(neg);
+  return -fmaxf(logf(pp), -100.f) - fmaxf(logf(1.0f - pn), -100.f);
+}
+
+// g * d(term)/d pos and g * d(term)/d neg of one pair, as torch's backward computes them
+__device__ __forceinline__ void pair_loss_grads(int kind, float margin, float g, float pos, float neg,
+                                                float* gpos, float* gneg) {
+  if (kind == KGE_LOSS_MARGIN) {   // same sub-gradient as torch: zero at the kink
+    const bool on = margin - pos + neg > 0.f;
+    *gpos = on ? -g : 0.f;
+    *gneg = on ? g : 0.f;
+    return;
+  }
+  const float pp = sigmoid_f(pos), pn = sigmoid_f(neg);
+  if (kind == KGE_LOSS_LOGISTIC) {
+    *gpos = g * (pp - 1.0f);   // d/dx log(1 + exp(-x)) = -sig(-x) = sig(x) - 1
+    *gneg = g * pn;            // d/dx log(1 + exp(x))  = sig(x)
+  } else {
+    // torch's BCELoss backward: (p - y) / max(p (1 - p), 1e-12), chained with dp/dx = p (1 - p); a
+    // saturated sigmoid (p = 0 or 1 exactly) gives exactly 0
+    *gpos = g * (pp - 1.0f) / fmaxf(pp * (1.0f - pp), 1e-12f) * (pp * (1.0f - pp));
+    *gneg = g * pn / fmaxf(pn * (1.0f - pn), 1e-12f) * (pn * (1.0f - pn));
+  }
+}
+
 // Fused step, forward: one warp per positive triple.
-//   loss += sum_j max(0, margin - pos_i + neg_ij)         (MarginRankingLoss, target +1, sum)
+//   loss += sum_j pair_loss_term(pos_i, neg_ij)
 // Negatives come from (nh, nt) if given, else from Philox; optionally written out.
 __global__ void margin_step_fwd_kernel(MarginStepParams a) {
   const long long w = ((long long)blockIdx.x * blockDim.x + threadIdx.x) >> 5;
@@ -444,14 +483,15 @@ __global__ void margin_step_fwd_kernel(MarginStepParams a) {
     if (lane == 0) {
       if (a.neg_out) a.neg_out[idx] = neg;
       if (a.nh_out) { a.nh_out[idx] = nh; a.nt_out[idx] = nt; }
-      loss += fmaxf(0.f, a.margin - pos + neg);
+      loss += pair_loss_term(a.loss_kind, a.margin, pos, neg);
     }
   }
   if (lane == 0) atomicAdd(a.loss, loss);
 }
 
-// Fused step, backward: recompute the same negatives and scores; every active hinge term
-// sends -g to the positive triple and +g to the negative one.
+// Fused step, backward: recompute the same negatives and scores; pair j sends g dl/dneg to the
+// negative triple, and the positive triple gets the sum over j of g dl/dpos in one call (the margin
+// loss: +g per active hinge to the negative, -g times the active count to the positive).
 __global__ void margin_step_bwd_kernel(MarginStepParams a, TrainGrads gr, const float* gloss) {
   const long long w = ((long long)blockIdx.x * blockDim.x + threadIdx.x) >> 5;
   const int lane = threadIdx.x & 31;
@@ -461,7 +501,7 @@ __global__ void margin_step_bwd_kernel(MarginStepParams a, TrainGrads gr, const 
   const RowPtrs pp = make_rows(a.model, a.dim, a.tb, hi, ti, ri);
   const float pos = triple_score(a.model, a.dim, pp, lane, nullptr, nullptr);
   const float p_head = a.nh ? 0.f : a.probs[ri];
-  int active = 0;
+  float gpos_sum = 0.f;
   for (int j = 0; j < a.n_neg; ++j) {
     const long long idx = (long long)j * a.b + w;
     long long nh, nt;
@@ -469,12 +509,12 @@ __global__ void margin_step_bwd_kernel(MarginStepParams a, TrainGrads gr, const 
     else corrupt_one(a.seed, a.offset, (uint64_t)idx, p_head, a.n_ent, hi, ti, &nh, &nt);
     const RowPtrs pn = make_rows(a.model, a.dim, a.tb, nh, nt, ri);
     const float neg = triple_score(a.model, a.dim, pn, lane, nullptr, nullptr);
-    if (a.margin - pos + neg > 0.f) {  // same sub-gradient as torch: zero at the kink
-      ++active;
-      triple_backward(a.model, a.dim, pn, grad_rows(a.model, a.dim, gr, nh, nt, ri), g, lane);
-    }
+    float gp, gn;
+    pair_loss_grads(a.loss_kind, a.margin, 1.f, pos, neg, &gp, &gn);
+    gpos_sum += gp;
+    triple_backward(a.model, a.dim, pn, grad_rows(a.model, a.dim, gr, nh, nt, ri), g * gn, lane);
   }
-  if (active) triple_backward(a.model, a.dim, pp, grad_rows(a.model, a.dim, gr, hi, ti, ri), -g * (float)active, lane);
+  triple_backward(a.model, a.dim, pp, grad_rows(a.model, a.dim, gr, hi, ti, ri), g * gpos_sum, lane);
 }
 
 // Entity-sharded fused step (a.hrows set), one warp per positive.  Every rank runs the same draws;
@@ -517,14 +557,15 @@ __global__ void margin_step_shard_fwd_kernel(MarginStepParams a) {
     long long loc;
     if (!owned_draw(a, (long long)j * a.b + w, p_head, &head, &loc)) continue;
     const float neg = triple_score(a.model, a.dim, shard_neg_rows(a, w, ri, head, loc), lane, nullptr, nullptr);
-    if (lane == 0) loss += fmaxf(0.f, a.margin - pos + neg);
+    if (lane == 0) loss += pair_loss_term(a.loss_kind, a.margin, pos, neg);
   }
   if (lane == 0) atomicAdd(a.loss, loss);
 }
 
 // Backward of the sharded step: the replaced row's gradient goes to the local table (this rank owns
 // it), the intact entity's and the positive's to grad_hrows / grad_trows[w], the relation's to the
-// local copy of the relation gradient; the caller sums the last three over the ranks.
+// local copy of the relation gradient; the caller sums the last three over the ranks.  The positive's
+// term is summed over the negatives this rank owns only, so the ranks' sums make up the whole.
 __global__ void margin_step_shard_bwd_kernel(MarginStepParams a, TrainGrads gr, const float* gloss) {
   const long long w = ((long long)blockIdx.x * blockDim.x + threadIdx.x) >> 5;
   const int lane = threadIdx.x & 31;
@@ -538,20 +579,20 @@ __global__ void margin_step_shard_bwd_kernel(MarginStepParams a, TrainGrads gr, 
   const Planes<float> gh = buf_planes(a.grad_hrows, np, a.dim, w);
   const Planes<float> gt = buf_planes(a.grad_trows, np, a.dim, w);
   const Planes<float> grel = rel_planes(a.model, a.dim, gr.rel0, gr.rel1, ri);
-  int active = 0;
+  float gpos_sum = 0.f;
   for (int j = 0; j < a.n_neg; ++j) {
     bool head;
     long long loc;
     if (!owned_draw(a, (long long)j * a.b + w, p_head, &head, &loc)) continue;
     const RowPtrs pn = shard_neg_rows(a, w, ri, head, loc);
     const float neg = triple_score(a.model, a.dim, pn, lane, nullptr, nullptr);
-    if (a.margin - pos + neg > 0.f) {
-      ++active;
-      const Planes<float> ge = table_planes(gr.ent0, gr.ent1, np, (size_t)loc * a.dim);
-      triple_backward(a.model, a.dim, pn, grads_of(head ? ge : gh, head ? gt : ge, grel), g, lane);
-    }
+    float gp, gn;
+    pair_loss_grads(a.loss_kind, a.margin, 1.f, pos, neg, &gp, &gn);
+    gpos_sum += gp;
+    const Planes<float> ge = table_planes(gr.ent0, gr.ent1, np, (size_t)loc * a.dim);
+    triple_backward(a.model, a.dim, pn, grads_of(head ? ge : gh, head ? gt : ge, grel), g * gn, lane);
   }
-  if (active) triple_backward(a.model, a.dim, pp, grads_of(gh, gt, grel), -g * (float)active, lane);
+  triple_backward(a.model, a.dim, pp, grads_of(gh, gt, grel), g * gpos_sum, lane);
 }
 
 // ------------------------------------------------------------------------------------------
@@ -856,7 +897,10 @@ __device__ __forceinline__ Vec vec_load_smem(const float* row, int dim, int lane
 // trows, the draw loop keeps only the negatives whose replaced entity this rank holds (ballot +
 // prefix, local row numbers in `codes`), so the ring streams owned rows only, and the positive's
 // gradients go to grad_hrows / grad_trows[w].
-template <int MODEL, bool BWD, int MINB = 0, bool SHARD = false>
+// LOSS: KGE_LOSS_*.  The backward's closed form is linear in the negatives, so a loss other than the
+// margin only turns the counts into weights: negative j enters V, its kind's sum and its own scatter
+// with weight c_j = dl/dneg_j, and the positive with -sum_j dl/dpos instead of the active count.
+template <int MODEL, bool BWD, int MINB = 0, bool SHARD = false, int LOSS = KGE_LOSS_MARGIN>
 __global__ void __launch_bounds__(WARPS_PER_BLOCK * 32, MINB == 0 ? 1 : MINB)
 margin_step_ring_kernel(MarginStepParams a, TrainGrads gr, const float* __restrict__ gloss) {
   extern __shared__ __align__(128) unsigned char ring_smem[];
@@ -957,7 +1001,10 @@ margin_step_ring_kernel(MarginStepParams a, TrainGrads gr, const float* __restri
   Vec Vt, Vh;
 #pragma unroll
   for (int i = 0; i < FAST_NCH; ++i) Vt.c[i] = Vh.c[i] = make_float4(0.f, 0.f, 0.f, 0.f);
-  int n_t = 0, n_h = 0;
+  // per kind: the active hinges (margin) or the summed weights c_j
+  using Count = std::conditional_t<LOSS == KGE_LOSS_MARGIN, int, float>;
+  Count n_t = 0, n_h = 0;
+  float gpos_sum = 0.f;   // LOSS != margin: sum of dl/dpos over the ring's negatives
   unsigned phases = 0u;   // bit s = parity of the next completion of slot s (a skipped use does not advance it)
   for (int j = 0; j < n_loop; ++j) {
     const unsigned code = codes[j];
@@ -967,15 +1014,21 @@ margin_step_ring_kernel(MarginStepParams a, TrainGrads gr, const float* __restri
       const long long nh = a.nh[idx], nt = a.nt[idx];
       const RowPtrs pn = make_rows(MODEL, dim, a.tb, nh, nt, ri);
       const float neg = triple_score(MODEL, dim, pn, lane, nullptr, nullptr);
-      const float v = a.margin - pos + neg;
+      const float term = pair_loss_term(LOSS, a.margin, pos, neg);
       if (lane == 0) {
         if (!BWD && a.neg_out) a.neg_out[idx] = neg;
-        loss += fmaxf(0.f, v);
+        loss += term;
       }
-      if (BWD && v > 0.f) {
-        triple_backward(MODEL, dim, pn, grad_rows(MODEL, dim, gr, nh, nt, ri), g, lane);
-        const RowPtrs pp = make_rows(MODEL, dim, a.tb, hi, ti, ri);
-        triple_backward(MODEL, dim, pp, grad_rows(MODEL, dim, gr, hi, ti, ri), -g, lane);
+      if constexpr (BWD) {
+        float gp, gn;   // g = 1; the margin loss: -1 and 1 on an active hinge
+        pair_loss_grads(LOSS, a.margin, 1.f, pos, neg, &gp, &gn);
+        if (gn != 0.f || gp != 0.f) {
+          triple_backward(MODEL, dim, pn, grad_rows(MODEL, dim, gr, nh, nt, ri),
+                          LOSS == KGE_LOSS_MARGIN ? g : g * gn, lane);
+          const RowPtrs pp = make_rows(MODEL, dim, a.tb, hi, ti, ri);
+          triple_backward(MODEL, dim, pp, grad_rows(MODEL, dim, gr, hi, ti, ri),
+                          LOSS == KGE_LOSS_MARGIN ? -g : g * gp, lane);
+        }
       }
       if (lane == 0 && j + RING < n_loop) request(j + RING);
       continue;
@@ -1016,36 +1069,49 @@ margin_step_ring_kernel(MarginStepParams a, TrainGrads gr, const float* __restri
       neg = -l1;
       en_dot_G = eg;
     }
-    const float v = a.margin - pos + neg;
+    const float term = pair_loss_term(LOSS, a.margin, pos, neg);
     if (lane == 0) {
       if (!BWD && a.neg_out) a.neg_out[idx] = neg;
-      loss += fmaxf(0.f, v);
+      loss += term;
     }
-    if (BWD && v > 0.f) {
+    float gp = 0.f, cj = 0.f;   // dl/dpos and dl/dneg of this pair (g = 1)
+    if constexpr (BWD) pair_loss_grads(LOSS, a.margin, 1.f, pos, neg, &gp, &cj);
+    if constexpr (LOSS != KGE_LOSS_MARGIN) gpos_sum += gp;
+    if (BWD && cj != 0.f) {
+      // c_j = 1 on every active hinge of the margin loss: the weights drop out
+      const float wj = LOSS == KGE_LOSS_MARGIN ? 1.f : cj;
       if constexpr (MODEL != KGE_TRANSE_L1) en = vec_scale(ev, inv_e);
       Vec ge, V;
-      const float c = g * inv_e;
+      const float c = LOSS == KGE_LOSS_MARGIN ? g * inv_e : g * wj * inv_e;
       if constexpr (MODEL == KGE_DISTMULT) {
         ge = vec_map(P, en, [=](float p, float q) { return c * (p - q * en_dot_G); });
-        V = en;
+        V = LOSS == KGE_LOSS_MARGIN ? en : vec_scale(en, wj);
       } else if constexpr (MODEL == KGE_TRANSE_L2) {
         ge = vec_map(P, en, [=](float p, float q) { return c * (2.f * (p - q) - q * en_dot_G); });
-        V = en;
+        V = LOSS == KGE_LOSS_MARGIN ? en : vec_scale(en, wj);
       } else {
         V = vec_map(P, en, [](float p, float q) { return sgn(p - q); });
         ge = vec_map(V, en, [=](float s_, float q) { return c * (s_ - q * en_dot_G); });
+        if constexpr (LOSS != KGE_LOSS_MARGIN) V = vec_scale(V, wj);
       }
       vec_atomic_add(gr.ent0 + (size_t)e * dim, dim, lane, ge);
-      if (head) { Vh = vec_map(Vh, V, [](float x, float y) { return x + y; }); ++n_h; }
-      else { Vt = vec_map(Vt, V, [](float x, float y) { return x + y; }); ++n_t; }
+      const Count inc = LOSS == KGE_LOSS_MARGIN ? Count(1) : Count(wj);
+      if (head) { Vh = vec_map(Vh, V, [](float x, float y) { return x + y; }); n_h += inc; }
+      else { Vt = vec_map(Vt, V, [](float x, float y) { return x + y; }); n_t += inc; }
     }
   }
   if (!BWD) {
     if (lane == 0) atomicAdd(a.loss, loss);
     return;
   }
-  if (n_t + n_h == 0) return;
-  const float fn_t = (float)n_t, fn_h = (float)n_h, fn = (float)(n_t + n_h);
+  if constexpr (LOSS == KGE_LOSS_MARGIN) {
+    if (n_t + n_h == 0) return;
+  } else {
+    if (n_t == 0.f && n_h == 0.f && gpos_sum == 0.f) return;
+  }
+  // fn: the positive's weight, -sum_j dl/dpos (the margin loss: the active count)
+  const float fn_t = (float)n_t, fn_h = (float)n_h;
+  const float fn = LOSS == KGE_LOSS_MARGIN ? (float)(n_t + n_h) : -gpos_sum;
   Vec Gh, Gt, Gr;
   if constexpr (MODEL == KGE_DISTMULT) {
     Gh = vec_map3(r, Vt, tn, [=](float rr, float vt, float tt) { return g * rr * (vt - fn * tt); });
@@ -1086,7 +1152,7 @@ __host__ inline bool ring_step_ok(const MarginStepParams& a) {
   return enabled && a.n_neg <= 8192 && rows < 0x7FFFFFFFll && ring_smem_bytes(a) <= 96 * 1024;
 }
 
-template <int MODEL, bool BWD, int MINB, bool SHARD = false>
+template <int MODEL, bool BWD, int MINB, bool SHARD = false, int LOSS = KGE_LOSS_MARGIN>
 cudaError_t launch_ring_variant(const MarginStepParams& a, const TrainGrads& gr, const float* gloss, cudaStream_t st) {
   const size_t smem = ring_smem_bytes(a);
   static bool configured[64] = {};
@@ -1094,20 +1160,26 @@ cudaError_t launch_ring_variant(const MarginStepParams& a, const TrainGrads& gr,
   cudaError_t e = cudaGetDevice(&dev);
   if (e != cudaSuccess) return e;
   if (smem > 48 * 1024 && (dev < 0 || dev >= 64 || !configured[dev])) {
-    e = cudaFuncSetAttribute(margin_step_ring_kernel<MODEL, BWD, MINB, SHARD>,
+    e = cudaFuncSetAttribute(margin_step_ring_kernel<MODEL, BWD, MINB, SHARD, LOSS>,
                              cudaFuncAttributeMaxDynamicSharedMemorySize, 96 * 1024);
     if (e != cudaSuccess) return e;
     if (dev >= 0 && dev < 64) configured[dev] = true;
   }
   const unsigned blocks = (unsigned)((a.b + WARPS_PER_BLOCK - 1) / WARPS_PER_BLOCK);
-  margin_step_ring_kernel<MODEL, BWD, MINB, SHARD><<<blocks, WARPS_PER_BLOCK * 32, smem, st>>>(a, gr, gloss);
+  margin_step_ring_kernel<MODEL, BWD, MINB, SHARD, LOSS><<<blocks, WARPS_PER_BLOCK * 32, smem, st>>>(a, gr, gloss);
   return cudaGetLastError();
 }
 
 // KGE_TRAIN_BWD_BLOCKS=5 holds the backward kernel to 96 registers (5 CTAs = 20 warps per SM; the
-// unsharded step only)
+// unsharded margin step only)
 template <int MODEL, bool BWD>
 cudaError_t launch_ring(const MarginStepParams& a, const TrainGrads& gr, const float* gloss, cudaStream_t st) {
+  if (a.loss_kind == KGE_LOSS_LOGISTIC)
+    return a.hrows ? launch_ring_variant<MODEL, BWD, 0, true, KGE_LOSS_LOGISTIC>(a, gr, gloss, st)
+                   : launch_ring_variant<MODEL, BWD, 0, false, KGE_LOSS_LOGISTIC>(a, gr, gloss, st);
+  if (a.loss_kind == KGE_LOSS_BCE)
+    return a.hrows ? launch_ring_variant<MODEL, BWD, 0, true, KGE_LOSS_BCE>(a, gr, gloss, st)
+                   : launch_ring_variant<MODEL, BWD, 0, false, KGE_LOSS_BCE>(a, gr, gloss, st);
   if (a.hrows) return launch_ring_variant<MODEL, BWD, 0, true>(a, gr, gloss, st);
   if constexpr (BWD) {
     static const bool tight = [] { const char* v = getenv("KGE_TRAIN_BWD_BLOCKS"); return v && v[0] == '5'; }();
@@ -1116,6 +1188,8 @@ cudaError_t launch_ring(const MarginStepParams& a, const TrainGrads& gr, const f
   return launch_ring_variant<MODEL, BWD, 0>(a, gr, gloss, st);
 }
 
+// margin_step_fast_kernel (the register-resident form, KGE_TRAIN_RING=0) has the margin loss only; the
+// other losses take the generic kernels there
 __host__ inline bool fast_step_ok(const MarginStepParams& a) {
   return (a.model == KGE_TRANSE_L1 || a.model == KGE_TRANSE_L2 || a.model == KGE_DISTMULT) &&
          a.dim % 4 == 0 && a.dim <= FAST_MAX_DIM;
@@ -1141,24 +1215,14 @@ __global__ void margin_loss_bwd_kernel(const float* __restrict__ pos, const floa
   gneg[i] = g;
 }
 
-// LogisticLoss / BinaryCrossEntropyLoss (utils/losses.py:47-112), sum-reduced.
-//   logistic: softplus(-pos) + softplus(neg), softplus(x) = max(x, 0) + log1p(exp(-|x|))
-//   bce     : -max(log(sig(pos)), -100) - max(log(1 - sig(neg)), -100), sig in fp32 as torch does
-__device__ __forceinline__ float softplus_f(float x) { return fmaxf(x, 0.f) + log1pf(expf(-fabsf(x))); }
-__device__ __forceinline__ float sigmoid_f(float x) { return 1.0f / (1.0f + expf(-x)); }
-
+// LogisticLoss / BinaryCrossEntropyLoss (utils/losses.py:47-112), sum-reduced: pair_loss_term /
+// pair_loss_grads element by element.
 __global__ void pair_loss_fwd_kernel(int kind, const float* __restrict__ pos, const float* __restrict__ neg,
                                      long long n, float* __restrict__ loss) {
   float s = 0.f;
   for (long long i = (long long)blockIdx.x * blockDim.x + threadIdx.x; i < n;
-       i += (long long)gridDim.x * blockDim.x) {
-    if (kind == KGE_LOSS_LOGISTIC) {
-      s += softplus_f(-pos[i]) + softplus_f(neg[i]);
-    } else {
-      const float pp = sigmoid_f(pos[i]), pn = sigmoid_f(neg[i]);
-      s += -fmaxf(logf(pp), -100.f) - fmaxf(logf(1.0f - pn), -100.f);
-    }
-  }
+       i += (long long)gridDim.x * blockDim.x)
+    s += pair_loss_term(kind, 0.f, pos[i], neg[i]);
   s = warp_sum(s);
   if ((threadIdx.x & 31) == 0 && s != 0.f) atomicAdd(loss, s);
 }
@@ -1168,16 +1232,7 @@ __global__ void pair_loss_bwd_kernel(int kind, const float* __restrict__ pos, co
                                      float* __restrict__ gpos, float* __restrict__ gneg) {
   const long long i = (long long)blockIdx.x * blockDim.x + threadIdx.x;
   if (i >= n) return;
-  const float g = *gloss;
-  const float pp = sigmoid_f(pos[i]), pn = sigmoid_f(neg[i]);
-  if (kind == KGE_LOSS_LOGISTIC) {
-    gpos[i] = g * (pp - 1.0f);   // d/dx log(1 + exp(-x)) = -sig(-x) = sig(x) - 1
-    gneg[i] = g * pn;            // d/dx log(1 + exp(x))  = sig(x)
-  } else {
-    // torch's BCELoss backward: (p - y) / max(p (1 - p), 1e-12), chained with dp/dx = p (1 - p)
-    gpos[i] = g * (pp - 1.0f) / fmaxf(pp * (1.0f - pp), 1e-12f) * (pp * (1.0f - pp));
-    gneg[i] = g * pn / fmaxf(pn * (1.0f - pn), 1e-12f) * (pn * (1.0f - pn));
-  }
+  pair_loss_grads(kind, 0.f, *gloss, pos[i], neg[i], gpos + i, gneg + i);
 }
 
 inline unsigned blocks_for_warps(long long warps) {
@@ -1256,7 +1311,7 @@ cudaError_t launch_margin_step_fwd(const MarginStepParams& a, cudaStream_t st) {
       default: return launch_ring<KGE_DISTMULT, false>(a, none, nullptr, st);
     }
   }
-  if (fast_step_ok(a)) {
+  if (fast_step_ok(a) && a.loss_kind == KGE_LOSS_MARGIN) {
     const TrainGrads none{nullptr, nullptr, nullptr, nullptr};
     const unsigned blocks = blocks_for_warps(a.b);
     switch (a.model) {
@@ -1311,7 +1366,7 @@ cudaError_t launch_margin_step_bwd(const MarginStepParams& a, const TrainGrads& 
       default: return launch_ring<KGE_DISTMULT, true>(a, gr, gloss, st);
     }
   }
-  if (fast_step_ok(a)) {
+  if (fast_step_ok(a) && a.loss_kind == KGE_LOSS_MARGIN) {
     const unsigned blocks = blocks_for_warps(a.b);
     switch (a.model) {
       case KGE_TRANSE_L1: margin_step_fast_kernel<KGE_TRANSE_L1, true><<<blocks, WARPS_PER_BLOCK * 32, 0, st>>>(a, gr, gloss); break;

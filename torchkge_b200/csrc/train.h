@@ -49,6 +49,7 @@ struct MarginStepParams {
   const float* trows;
   float* grad_hrows;   // [b][planes][dim], +=
   float* grad_trows;
+  int loss_kind;       // KGE_LOSS_MARGIN / _LOGISTIC / _BCE; margin is used by the margin loss only
 };
 
 cudaError_t launch_score_triples_fwd(int model, int dim, const TrainTables& tb, const int64_t* h,

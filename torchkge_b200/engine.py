@@ -444,11 +444,13 @@ class CudaEngine:
         a.loss, a.stream = _ptr(loss), _stream(h.device)
         a.ent_lo, a.n_rows = step.ent_lo, step.n_rows
         a.hrows, a.trows = _ptr(hrows), _ptr(trows)
+        a.loss_kind = step.loss_kind
         return a
 
     def margin_step_fwd(self, step, tables, h, t, r, probs, hrows, trows):
-        """Sum of the hinge terms of the negatives this shard scores (float32 scalar tensor): the
-        negatives whose replaced entity lies in [step.ent_lo, step.ent_lo + step.n_rows).  ``tables``:
+        """Sum of the loss terms (step.loss_kind: the hinge, logistic or BCE term of each pair) of the
+        negatives this shard scores (float32 scalar tensor): the negatives whose replaced entity lies in
+        [step.ent_lo, step.ent_lo + step.n_rows).  ``tables``:
         (ent0, ent1, rel0, rel1) with this shard's entity rows (a three-plane table as one stacked
         (3, n, dim) tensor in ent0 / rel0); hrows / trows: (b, planes, dim) rows of every positive."""
         loss = torch.zeros((), dtype=torch.float32, device=h.device)

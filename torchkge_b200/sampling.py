@@ -10,7 +10,7 @@ import torch
 
 from . import _lib
 from .engine import _ptr, _stream
-from .training import fused_margin_step
+from .training import fused_loss_step, fused_margin_step, loss_kind_of
 
 
 def get_bernoulli_probs(kg):
@@ -135,20 +135,31 @@ class BernoulliNegativeSampler(NegativeSampler):
                    "kge_corrupt_batch")
         return nh, nt
 
-    def fused_step(self, model, heads, tails, relations, margin, n_neg=None, *, shard=None):
-        """Extension: corruption + ``model(...)`` + ``MarginLoss(margin)`` in ONE kernel; returns
-        the differentiable scalar loss.  Draws the negatives ``corrupt_batch`` would draw at the
-        same call count.
+    def fused_step(self, model, heads, tails, relations, margin=None, n_neg=None, *, criterion=None,
+                   shard=None):
+        """Extension: corruption + ``model(...)`` + the loss in ONE kernel; returns the differentiable
+        scalar loss.  Draws the negatives ``corrupt_batch`` would draw at the same call count.
+
+        Give exactly one of ``margin`` (``MarginLoss(margin)``) and ``criterion`` (a ``MarginLoss``,
+        ``LogisticLoss`` or ``BinaryCrossEntropyLoss``; see ``training.fused_loss_step``).
 
         shard: ``EntityShard(local_storage=True)`` for a model holding only its entity rows (see
         ``training.fused_margin_step``); every rank uses a sampler with the same seed and call count,
         built on the whole graph, and passes the same batch."""
+        if (margin is None) == (criterion is None):
+            raise ValueError("fused_step takes exactly one of margin and criterion")
+        if criterion is not None:
+            loss_kind_of(criterion)       # an unsupported criterion raises before the call count moves
         if n_neg is None:
             n_neg = self.n_neg
         if shard is not None and getattr(shard, "n_ent", self.n_ent) != self.n_ent:
             raise ValueError("the sampler draws on %d entities, the shard partitions %d"
                              % (self.n_ent, shard.n_ent))
         self.bern_probs = self.bern_probs.to(heads.device)
+        if criterion is not None:
+            return fused_loss_step(model, heads, tails, relations, criterion, n_neg=n_neg,
+                                   bern_probs=self.bern_probs, seed=self.seed,
+                                   offset=self._next_offset(), shard=shard)
         return fused_margin_step(model, heads, tails, relations, margin, n_neg=n_neg,
                                  bern_probs=self.bern_probs, seed=self.seed,
                                  offset=self._next_offset(), shard=shard)

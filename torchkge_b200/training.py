@@ -1,5 +1,5 @@
 """Training-side entry points: differentiable per-triple scoring (``Model.scoring_function``),
-``MarginLoss`` and the fused sample + score + hinge step, as autograd Functions over the CUDA
+the three losses and the fused sample + score + loss step, as autograd Functions over the CUDA
 kernels of csrc/train.cu.  Gradients are dense tables (what ``nn.Embedding`` yields in the
 reference), accumulated with atomics.
 """
@@ -185,10 +185,33 @@ def pair_loss(pos, neg, kind):
     return _PairLoss.apply(pos, neg, kind)
 
 
+def loss_kind_of(criterion):
+    """(loss kind, margin) of the fused step for ``criterion``: a ``MarginLoss``, ``LogisticLoss`` or
+    ``BinaryCrossEntropyLoss`` of this package or of torchkge, recognised by class name as models are
+    (torchkge's ``MarginLoss`` keeps its margin in ``criterion.loss.margin``).  The margin is 0.0 for
+    the losses that have none.  Anything else raises TypeError."""
+    name = type(criterion).__name__
+    if name == "MarginLoss":
+        margin = getattr(criterion, "margin", None)
+        if margin is None:
+            margin = getattr(getattr(criterion, "loss", None), "margin", None)
+        if margin is None:
+            raise TypeError("MarginLoss without a margin attribute")
+        return _lib.LOSS_MARGIN, float(margin)
+    if name == "LogisticLoss":
+        return _lib.LOSS_LOGISTIC, 0.0
+    if name == "BinaryCrossEntropyLoss":
+        return _lib.LOSS_BCE, 0.0
+    raise TypeError("the fused training step supports MarginLoss, LogisticLoss and BinaryCrossEntropyLoss, "
+                    "not %s" % name)
+
+
 class _MarginStep(torch.autograd.Function):
+    """The fused step on the whole table; loss_kind: _lib.LOSS_* (margin is used by the margin loss only)."""
+
     @staticmethod
     def forward(ctx, code, dim, n_ent, margin, n_neg, h, t, r, nh, nt, probs, seed, offset,
-                ent0, ent1, rel0, rel1):
+                ent0, ent1, rel0, rel1, loss_kind=_lib.LOSS_MARGIN):
         tensors = [None if x is None else x.detach().contiguous() for x in (ent0, ent1, rel0, rel1)]
         _check_cuda(tensors[0], h, t, r)
         dev = tensors[0].device
@@ -199,9 +222,9 @@ class _MarginStep(torch.autograd.Function):
             probs = probs.to(device=dev, dtype=torch.float32).contiguous()
         loss = torch.zeros((), dtype=torch.float32, device=dev)
         a = _MarginStep._args(code, dim, n_ent, margin, n_neg, h, t, r, nh, nt, probs, seed, offset,
-                              tensors, loss, dev)
+                              tensors, loss, dev, loss_kind)
         _lib.check(_lib.load().kge_margin_step_fwd(ctypes.byref(a)), "kge_margin_step_fwd")
-        ctx.meta = (code, dim, n_ent, margin, n_neg, seed, offset)
+        ctx.meta = (code, dim, n_ent, margin, n_neg, seed, offset, loss_kind)
         ctx.present = [x is not None for x in tensors]
         ctx.has_neg, ctx.has_probs = nh is not None, probs is not None
         extra = ([nh, nt] if nh is not None else []) + ([probs] if probs is not None else [])
@@ -209,18 +232,20 @@ class _MarginStep(torch.autograd.Function):
         return loss
 
     @staticmethod
-    def _args(code, dim, n_ent, margin, n_neg, h, t, r, nh, nt, probs, seed, offset, tensors, loss, dev):
+    def _args(code, dim, n_ent, margin, n_neg, h, t, r, nh, nt, probs, seed, offset, tensors, loss, dev,
+              loss_kind=_lib.LOSS_MARGIN):
         a = _lib.MarginStepArgs()
         a.tb = _tables(code, dim, tensors)
         a.n_neg, a.margin, a.b, a.n_ent = n_neg, float(margin), h.shape[0], n_ent
         a.h, a.t, a.r, a.nh, a.nt, a.bern_probs = (_ptr(x) for x in (h, t, r, nh, nt, probs))
         a.seed, a.offset = int(seed), int(offset)
         a.loss, a.stream = _ptr(loss), _stream(dev)
+        a.loss_kind = int(loss_kind)
         return a
 
     @staticmethod
     def backward(ctx, gl):
-        code, dim, n_ent, margin, n_neg, seed, offset = ctx.meta
+        code, dim, n_ent, margin, n_neg, seed, offset, loss_kind = ctx.meta
         saved = list(ctx.saved_tensors)
         h, t, r = saved[:3]
         k = 3
@@ -237,19 +262,21 @@ class _MarginStep(torch.autograd.Function):
         gl = gl.contiguous().float()
         dummy = torch.zeros((), dtype=torch.float32, device=dev)
         a = _MarginStep._args(code, dim, n_ent, margin, n_neg, h, t, r, nh, nt, probs, seed, offset,
-                              tensors, dummy, dev)
+                              tensors, dummy, dev, loss_kind)
         gs, g = _zero_grads(tensors)
         _lib.check(_lib.load().kge_margin_step_bwd(ctypes.byref(a), ctypes.byref(g), _ptr(gl)),
                    "kge_margin_step_bwd")
-        return (None,) * 13 + tuple(gs)
+        return (None,) * 13 + tuple(gs) + (None,)
 
 
 #: what every rank's kernels of one sharded step are told (engine.margin_step_fwd / _bwd)
-ShardedStep = collections.namedtuple("ShardedStep", "code dim n_ent ent_lo n_rows n_neg margin seed offset")
+#: loss_kind: _lib.LOSS_* (default the margin loss)
+ShardedStep = collections.namedtuple("ShardedStep", "code dim n_ent ent_lo n_rows n_neg margin seed offset loss_kind",
+                                     defaults=(_lib.LOSS_MARGIN,))
 
 
 class _ShardedMarginStep(torch.autograd.Function):
-    """The fused margin step on a range-partitioned entity table (EntityShard, local storage):
+    """The fused step (any loss kind) on a range-partitioned entity table (EntityShard, local storage):
       1. the positives' h / t rows: each rank gathers the rows it holds, one sum-all-reduce;
       2. every rank draws all negatives with the global n_ent and scores those whose replaced entity
          it holds (the intact entity's row comes from step 1, the relation table is replicated);
@@ -326,11 +353,13 @@ def _signed64(x):
 
 
 def sharded_margin_step(model, heads, tails, relations, margin, n_neg, bern_probs, seed, offset, shard,
-                        engine=None):
-    """``fused_margin_step(..., shard=shard)`` for a model that holds only the entity rows
-    [shard.lo, shard.hi) of an EntityShard with local storage; the same (heads, tails, relations),
-    seed, offset, n_neg and margin on every rank.  Returns the full loss on every rank; its backward
-    leaves every rank with the gradient of its own rows and the (identical) relation gradient.
+                        engine=None, loss_kind=_lib.LOSS_MARGIN):
+    """``fused_margin_step(..., shard=shard)`` (``fused_loss_step`` with ``loss_kind``) for a model that
+    holds only the entity rows [shard.lo, shard.hi) of an EntityShard with local storage; the same
+    (heads, tails, relations), seed, offset, n_neg, margin and loss kind on every rank.  Returns the full
+    loss on every rank; its backward leaves every rank with the gradient of its own rows and the
+    (identical) relation gradient.  Every rank counts the positive's term of a pair only for the
+    negatives it scores, so the ranks' sums are the unsharded loss and gradients.
     ``engine``: CudaEngine or a stand-in with margin_step_fwd / margin_step_bwd / scatter_rows_add /
     gather_rows."""
     # argument errors first, on every rank: none of them may leave the others waiting in a collective
@@ -352,17 +381,56 @@ def sharded_margin_step(model, heads, tails, relations, margin, n_neg, bern_prob
                          % (held, shard.lo, shard.hi, shard.hi - shard.lo))
     b = int(heads.shape[0])
     step = ShardedStep(code, _kernel_dim(model, code), shard.n_ent, shard.lo, held, int(n_neg), float(margin),
-                       int(seed) & 0xFFFFFFFFFFFFFFFF, int(offset) & 0xFFFFFFFFFFFFFFFF)
-    # one small collective: every rank must draw the same negatives for the same batch
+                       int(seed) & 0xFFFFFFFFFFFFFFFF, int(offset) & 0xFFFFFFFFFFFFFFFF, int(loss_kind))
+    # one small collective: every rank must draw the same negatives for the same batch and loss
     mine = torch.tensor([_signed64(step.seed), _signed64(step.offset), b, step.n_neg,
-                         struct.unpack("<q", struct.pack("<d", step.margin))[0]],
+                         struct.unpack("<q", struct.pack("<d", step.margin))[0], step.loss_kind],
                         dtype=torch.int64, device=rel0.device)
     everyone = shard.stack_all(mine)
     if not bool((everyone == mine).all()):
-        raise ValueError("the ranks of a sharded step disagree on (seed, offset, batch size, n_neg, margin): "
-                         "%s" % everyone.tolist())
+        raise ValueError("the ranks of a sharded step disagree on (seed, offset, batch size, n_neg, margin, "
+                         "loss kind): %s" % everyone.tolist())
     return _ShardedMarginStep.apply(step, shard, engine or default_engine(), heads, tails, relations,
                                     bern_probs, ent0, ent1, rel0, rel1)
+
+
+def _fused_step(model, heads, tails, relations, loss_kind, margin, n_neg, negatives, bern_probs, seed, offset,
+                shard):
+    if shard is not None:
+        if negatives is not None:
+            raise ValueError("external negatives are not supported by the sharded training step")
+        return sharded_margin_step(model, heads, tails, relations, margin, n_neg, bern_probs, seed, offset,
+                                   shard, loss_kind=loss_kind)
+    spec_code = _training_code(model)
+    ent0, ent1, rel0, rel1 = _param_tensors(model, spec_code)
+    nh = nt = None
+    if negatives is not None:
+        nh, nt = negatives
+        n_neg = int(nh.shape[0] // heads.shape[0])
+    elif bern_probs is None:
+        raise ValueError("either negatives or bern_probs must be given")
+    return _MarginStep.apply(spec_code, _kernel_dim(model, spec_code), model.n_ent, margin, n_neg, heads, tails,
+                             relations, nh, nt, bern_probs, seed, offset, ent0, ent1, rel0, rel1, loss_kind)
+
+
+def fused_loss_step(model, heads, tails, relations, criterion, n_neg=1, negatives=None, bern_probs=None,
+                    seed=0, offset=0, *, shard=None):
+    """``fused_margin_step`` for any of the three losses: Bernoulli corruption (or the given
+    ``negatives``), ``model(h, t, r, nh, nt)`` and ``criterion(pos, neg)`` in a single kernel,
+    differentiable with respect to the embedding tables.
+
+    criterion: ``MarginLoss(margin)``, ``LogisticLoss()`` or ``BinaryCrossEntropyLoss()``, of this
+        package or of torchkge; anything else raises TypeError (on every rank, before any collective).
+        The loss is summed over every (positive i, negative j) pair, the positive's score repeated
+        n_neg times as in ``Model.forward``:
+          logistic: softplus(-pos_i) + softplus(neg_ij)
+          BCE     : -max(log sig(pos_i), -100) - max(log(1 - sig(neg_ij)), -100)
+        and its gradients are those torch's SoftMarginLoss / BCELoss backward give.
+    shard: as in ``fused_margin_step``; every rank must pass the same kind of loss.
+    """
+    kind, margin = loss_kind_of(criterion)
+    return _fused_step(model, heads, tails, relations, kind, margin, n_neg, negatives, bern_probs, seed, offset,
+                       shard)
 
 
 def fused_margin_step(model, heads, tails, relations, margin, n_neg=1, negatives=None,
@@ -381,19 +449,8 @@ def fused_margin_step(model, heads, tails, relations, margin, n_neg=1, negatives
         same batch, seed, offset, n_neg and margin -- the batch contents are not checked -- and gets
         the full loss; the negatives are drawn on [1, shard.n_ent).  External negatives are not
         supported in this mode.
+
+    ``fused_loss_step`` takes a criterion instead of a margin (LogisticLoss, BinaryCrossEntropyLoss).
     """
-    if shard is not None:
-        if negatives is not None:
-            raise ValueError("external negatives are not supported by the sharded training step")
-        return sharded_margin_step(model, heads, tails, relations, margin, n_neg, bern_probs, seed, offset,
-                                   shard)
-    spec_code = _training_code(model)
-    ent0, ent1, rel0, rel1 = _param_tensors(model, spec_code)
-    nh = nt = None
-    if negatives is not None:
-        nh, nt = negatives
-        n_neg = int(nh.shape[0] // heads.shape[0])
-    elif bern_probs is None:
-        raise ValueError("either negatives or bern_probs must be given")
-    return _MarginStep.apply(spec_code, _kernel_dim(model, spec_code), model.n_ent, margin, n_neg, heads, tails,
-                             relations, nh, nt, bern_probs, seed, offset, ent0, ent1, rel0, rel1)
+    return _fused_step(model, heads, tails, relations, _lib.LOSS_MARGIN, margin, n_neg, negatives, bern_probs,
+                       seed, offset, shard)
