@@ -4,8 +4,9 @@ Nothing here computes scores: torch is used for device memory, streams and (when
 table is range-partitioned) the collectives of the sharded paths.  The only engine is the CUDA one; tests
 may substitute an object with the same methods (``pack``, ``gather_rows``, ``rank_side``,
 ``score_all``; ``topk_side`` / ``topk_merge`` for top-k inference; ``margin_step_fwd`` /
-``margin_step_bwd`` / ``scatter_rows_add`` for the sharded training step) to exercise the sharding
-logic on CPU.
+``margin_step_bwd`` / ``scatter_rows_add`` for the sharded training step; ``finalize`` /
+``rescal_rel_scores`` / ``rank_dense`` for relation prediction; ``score_triples`` for triplet
+classification) to exercise the sharding logic on CPU.
 """
 import ctypes
 import os
@@ -419,6 +420,25 @@ class CudaEngine:
         self.launches += 3
         return pred, vals
 
+    def score_triples(self, code, dim, ent, rel0, rel1, h, t, r):
+        """(n,) scores of the triples (h[i], r[i], t[i]) by the per-triple kernel of
+        ``model.scoring_function`` (kge_score_triples_fwd), without autograd.  ``ent``: a plane-major
+        (planes, rows, dim) entity table (three-plane models find plane 2 at the same spacing);
+        rel0 / rel1 as in ModelSpec."""
+        _need_cuda(ent, h, t, r)
+        n = h.shape[0]
+        out = torch.empty(n, dtype=torch.float32, device=ent.device)
+        if n == 0:
+            return out
+        tb = _lib.Tables()
+        tb.model, tb.dim = code, dim
+        tb.ent0, tb.ent1 = _ptr(ent[0]), (_ptr(ent[1]) if ent.shape[0] > 1 else None)
+        tb.rel0, tb.rel1 = _ptr(rel0), _ptr(rel1)
+        _lib.check(self.lib.kge_score_triples_fwd(ctypes.byref(tb), _ptr(h), _ptr(t), _ptr(r), n, _ptr(out),
+                                                  _stream(out.device)), "kge_score_triples_fwd")
+        self.launches += 1
+        return out
+
     def finalize(self, raw_count, filt_sub):
         n = raw_count.shape[0]
         ranks = torch.empty(n, dtype=torch.int64, device=raw_count.device)
@@ -751,8 +771,22 @@ def relation_spec(spec):
     return ModelSpec(spec.code, spec.dim, spec.n_rel, spec.n_rel, cand0, cand1, None, None, ent2=cand2)
 
 
+def _check_sharded_model(spec, shard):
+    """Argument errors of an entity-sharded call, raised on every rank before the first collective:
+    the table must be this rank's rows [lo, hi) (local storage) or the whole table (full storage)."""
+    if spec.n_ent != shard.n_ent:
+        raise ValueError("the shard partitions %d entities, the model has %d" % (shard.n_ent, spec.n_ent))
+    if shard.local_storage:
+        if (spec.ent_lo, spec.n_rows) != (shard.lo, shard.hi - shard.lo):
+            raise ValueError("EntityShard(local_storage=True): rank %d holds rows [%d, %d) but the model has %d "
+                             "entity rows from %d" % (shard.rank, shard.lo, shard.hi, spec.n_rows, spec.ent_lo))
+    elif (spec.ent_lo, spec.n_rows) != (0, shard.n_ent):
+        raise ValueError("EntityShard(local_storage=False) needs the whole entity table on every rank "
+                         "(got %d rows)" % spec.n_rows)
+
+
 def rank_relation_prediction(spec, h_idx, t_idx, r_idx, filt, directed=True, engine=None,
-                             chunk=DEFAULT_CHUNK):
+                             chunk=DEFAULT_CHUNK, shard=None):
     """Rank every fact's true relation against all relations (RelationPredictionEvaluator,
     torchkge/evaluation.py:64-112).
 
@@ -760,49 +794,108 @@ def rank_relation_prediction(spec, h_idx, t_idx, r_idx, filt, directed=True, eng
                minus the true one), or None
     directed   False: the scores of (t, ?, h) are ranked together with those of (h, ?, t), against
                the directed true score (evaluation.py:99-107)
+    shard      None; QueryShard over the n facts: every rank ranks its slice of the facts (and of
+               ``filt``) against the replicated table; EntityShard: the relations, the candidates, are
+               on every rank, so the facts are split too -- under local storage (spec.ent_lo /
+               spec.n_ent set from the shard) the h / t rows of each chunk are first exchanged by one
+               all-reduce, and the chunk's facts split as QueryShard splits them; under full storage
+               the facts are split as QueryShard(n) splits them.  Either way one all-gather per split
+               brings every rank the full rank vectors, equal to the unsharded call's.
     Returns (rank_true_rels, filt_rank_true_rels), int64 device tensors.
     """
     engine = engine or default_engine()
     n = h_idx.shape[0]
     dev = spec.ent0.device
-    counters = torch.zeros((2, n), dtype=torch.int32, device=dev)
-    if spec.code == _lib.RESCAL:
-        # the candidates are the relation MATRICES: per-fact vectors h^T M_c, a dense (n, n_rel)
-        # score matrix (bilinear.py:115-121) ranked by kge_rank_dense
-        for lo in range(0, n, min(chunk, 4096)):
-            hi = min(n, lo + min(chunk, 4096))
-            h, t, r = h_idx[lo:hi], t_idx[lo:hi], r_idx[lo:hi].contiguous()
-            hrows = engine.gather_rows(spec, h).view(hi - lo, spec.dim)
-            trows = engine.gather_rows(spec, t).view(hi - lo, spec.dim)
-            f = None if filt is None else _csr_slice(filt, lo, hi, n)
-            s_true = torch.empty(hi - lo, dtype=torch.float32, device=dev)
-            scores = engine.rescal_rel_scores(spec, hrows, trows)
-            engine.rank_dense(scores, r, f, counters[0][lo:hi], counters[1][lo:hi], true_score=s_true)
+    rspec = None if spec.code == _lib.RESCAL else relation_spec(spec)   # unsupported models raise here
+    if isinstance(shard, EntityShard) and shard.world > 1:
+        _check_sharded_model(spec, shard)
+        if not shard.local_storage:
+            shard = QueryShard(n, shard.rank, shard.world, shard.group)
+    if isinstance(shard, QueryShard) and shard.world > 1:
+        if shard.n != n:
+            raise ValueError("QueryShard covers %d facts, got %d" % (shard.n, n))
+        h, t, r = shard.slice(h_idx, t_idx, r_idx)
+        mine = rank_relation_prediction(spec, h, t, r, shard.csr(filt), directed, engine, chunk)
+        return tuple(shard.all_gather(list(mine)))
+    with _device_guard(dev):
+        packed = None if rspec is None else engine.pack(rspec)
+        keep = []
+
+        def rank_rows(hrows, trows, r, f, raw, sub):
+            """Adds the counts of facts (hrows, ?, trows) with true relations r into raw / sub."""
+            m = r.shape[0]
+            s_true = torch.empty(m, dtype=torch.float32, device=dev)
+            if rspec is None:
+                # RESCAL: the candidates are the relation MATRICES: per-fact vectors h^T M_c, a dense
+                # (m, n_rel) score matrix (bilinear.py:115-121) ranked by kge_rank_dense
+                hrows, trows = hrows.reshape(m, spec.dim), trows.reshape(m, spec.dim)
+                engine.rank_dense(engine.rescal_rel_scores(spec, hrows, trows), r, f, raw, sub, true_score=s_true)
+                if not directed:
+                    engine.rank_dense(engine.rescal_rel_scores(spec, trows, hrows), r, f, raw, sub,
+                                      true_score_in=s_true)
+                return
+            rrows = engine.gather_rows(rspec, r)
+            keep.append(engine.rank_side(rspec, packed, _lib.SIDE_REL, hrows, trows, None, r, f, raw, sub,
+                                         true_score=s_true, true_rows=rrows))
             if not directed:
-                scores2 = engine.rescal_rel_scores(spec, trows, hrows)
-                engine.rank_dense(scores2, r, f, counters[0][lo:hi], counters[1][lo:hi], true_score_in=s_true)
-        return engine.finalize(counters[0], counters[1])
-    rspec = relation_spec(spec)
-    packed = engine.pack(rspec)
-    keep = []
-    for lo in range(0, n, chunk):
-        hi = min(n, lo + chunk)
-        h, t, r = h_idx[lo:hi], t_idx[lo:hi], r_idx[lo:hi]
-        hrows, trows = engine.gather_rows(spec, h), engine.gather_rows(spec, t)
-        rrows = engine.gather_rows(rspec, r)
-        f = None if filt is None else _csr_slice(filt, lo, hi, n)
-        s_true = torch.empty(hi - lo, dtype=torch.float32, device=dev)
-        keep.append(engine.rank_side(rspec, packed, _lib.SIDE_REL, hrows, trows, None, r, f,
-                                     counters[0][lo:hi], counters[1][lo:hi], true_score=s_true,
-                                     true_rows=rrows))
-        if not directed:
-            keep.append(engine.rank_side(rspec, packed, _lib.SIDE_REL, trows, hrows, None, r, f,
-                                         counters[0][lo:hi], counters[1][lo:hi], true_rows=rrows,
-                                         true_score_in=s_true))
-        keep.append((s_true, f))
-    ranks, filt_ranks = engine.finalize(counters[0], counters[1])
-    del keep
-    return ranks, filt_ranks
+                keep.append(engine.rank_side(rspec, packed, _lib.SIDE_REL, trows, hrows, None, r, f, raw, sub,
+                                             true_rows=rrows, true_score_in=s_true))
+            keep.append((s_true, f))
+
+        # the dense RESCAL branch holds (chunk, n_rel) scores: at most 4096 facts per call
+        step = min(chunk, 4096) if rspec is None else chunk
+        if shard is None or shard.world == 1:
+            counters = torch.zeros((2, n), dtype=torch.int32, device=dev)
+            for lo in range(0, n, step):
+                hi = min(n, lo + step)
+                h, t, r = h_idx[lo:hi], t_idx[lo:hi], r_idx[lo:hi].contiguous()
+                f = None if filt is None else _csr_slice(filt, lo, hi, n)
+                rank_rows(engine.gather_rows(spec, h), engine.gather_rows(spec, t), r, f,
+                          counters[0][lo:hi], counters[1][lo:hi])
+            ranks, filt_ranks = engine.finalize(counters[0], counters[1])
+            del keep
+            return ranks, filt_ranks
+        # EntityShard with local storage: the rows of every fact are exchanged, the facts are split
+        ranks = torch.empty(n, dtype=torch.int64, device=dev)
+        filt_ranks = torch.empty(n, dtype=torch.int64, device=dev)
+        for lo in range(0, n, step):
+            hi = min(n, lo + step)
+            m = hi - lo
+            rows = _exchanged_rows(spec, torch.cat([h_idx[lo:hi], t_idx[lo:hi]]), shard, engine)
+            part = QueryShard(m, shard.rank, shard.world, shard.group)
+            a, b = part.lo, part.hi
+            counters = torch.zeros((2, b - a), dtype=torch.int32, device=dev)
+            if b > a:          # a rank with no facts in this chunk still joins the all-gather
+                f = None if filt is None else _csr_slice(filt, lo + a, lo + b, n)
+                rank_rows(rows[a:b], rows[m + a:m + b], r_idx[lo + a:lo + b].contiguous(), f,
+                          counters[0], counters[1])
+            ranks[lo:hi], filt_ranks[lo:hi] = part.all_gather(list(engine.finalize(counters[0], counters[1])))
+        del keep
+        return ranks, filt_ranks
+
+
+def score_triples_entity_sharded(spec, h_idx, t_idx, r_idx, shard, engine=None, batch=DEFAULT_CHUNK):
+    """(n,) scores of the triples (h_idx[i], r_idx[i], t_idx[i]) of a model whose entity rows are split
+    over ``shard`` (EntityShard, local storage; spec.ent_lo / spec.n_ent set from it, spec over the
+    tables the per-triple kernel reads).  Per batch of ``batch`` triples the h and t rows are exchanged
+    by one all-reduce (_exchanged_rows), laid out plane-major and scored on every rank with h = i,
+    t = b + i: the kernel reads the same bits as on the whole table, so every rank gets the scores of
+    ``model.scoring_function``, bit for bit."""
+    engine = engine or default_engine()
+    _check_sharded_model(spec, shard)
+    n = h_idx.shape[0]
+    dev = spec.ent0.device
+    out = torch.empty(n, dtype=torch.float32, device=dev)
+    with _device_guard(dev):
+        for lo in range(0, n, batch):
+            hi = min(n, lo + batch)
+            m = hi - lo
+            rows = _exchanged_rows(spec, torch.cat([h_idx[lo:hi], t_idx[lo:hi]]), shard, engine)
+            ent = rows.transpose(0, 1).contiguous()          # (planes, 2m, dim)
+            ar = torch.arange(m, dtype=torch.int64, device=dev)
+            out[lo:hi] = engine.score_triples(spec.code, spec.dim, ent, spec.rel0, spec.rel1, ar, ar + m,
+                                              r_idx[lo:hi].contiguous())
+    return out
 
 
 # ------------------------------------------------------------------------------ top-k inference

@@ -7,8 +7,8 @@ import torch
 
 from . import _lib
 from .data import dict_filter_csr, filter_csr
-from .engine import (DEFAULT_CHUNK, ModelSpec, QueryShard, default_engine, rank_link_prediction,
-                     rank_relation_prediction)
+from .engine import (DEFAULT_CHUNK, EntityShard, ModelSpec, QueryShard, _check_sharded_model, default_engine,
+                     rank_link_prediction, rank_relation_prediction, score_triples_entity_sharded)
 from .exceptions import NotYetEvaluatedError
 
 
@@ -205,33 +205,47 @@ class RelationPredictionEvaluator(object):
 
     Parameters
     ----------
-    model: TransE (L1/L2), DistMult or ComplEx model on a CUDA device.
+    model: TransE (L1/L2), DistMult, RESCAL, ComplEx or Analogy model on a CUDA device.
     knowledge_graph: object exposing ``n_facts, head_idx, tail_idx, relations, dict_of_rels``.
     directed: bool (default True).  False: both (h, ?, t) and (t, ?, h) are scored and ranked
         together against the directed true score (evaluation.py:99-107).
+    shard: ``torchkge_b200.engine.EntityShard`` or ``QueryShard``, optional, keyword-only
+        (extension).  The candidates are the relations, which every rank holds, so both forms split
+        the facts over the ranks and all-gather the rank vectors.  QueryShard (over ``n_facts``):
+        every rank ranks its contiguous slice of the facts, filtered by its slice of
+        ``dict_of_rels``.  EntityShard with ``local_storage=True`` (the model holds only entity rows
+        [lo, hi) and its row 0 is entity lo): per chunk of facts the h and t rows are exchanged by one
+        all-reduce, then the chunk's facts are split as QueryShard splits them.  EntityShard with full
+        storage: the facts are split as QueryShard splits them, no rows move.  Every rank ends with
+        the rank vectors of the unsharded evaluator, exactly.
 
     Attributes: ``rank_true_rels``, ``filt_rank_true_rels`` (LongTensor (n_facts,), CPU after
     ``evaluate``), ``evaluated``, ``directed``.
     """
 
-    def __init__(self, model, knowledge_graph, directed=True):
+    def __init__(self, model, knowledge_graph, directed=True, *, shard=None):
         self.model = model
         self.kg = knowledge_graph
         self.directed = directed
+        self.shard = shard
         self.rank_true_rels = torch.empty(size=(knowledge_graph.n_facts,)).long()
         self.filt_rank_true_rels = torch.empty(size=(knowledge_graph.n_facts,)).long()
         self.evaluated = False
 
     def evaluate(self, b_size, verbose=True):
         """``b_size`` / ``verbose`` are accepted for signature compatibility (see
-        ``LinkPredictionEvaluator.evaluate``)."""
+        ``LinkPredictionEvaluator.evaluate``).  Under a shard, every rank of its group calls this."""
         if b_size is None or int(b_size) < 1:
             raise ValueError("b_size must be a positive integer")
         spec = ModelSpec.from_model(self.model)
+        if isinstance(self.shard, EntityShard) and self.shard.local_storage:
+            spec.ent_lo, spec.n_ent = self.shard.lo, self.shard.n_ent
         if not spec.ent0.is_cuda:
             raise _lib.KgeLibraryError(
                 "RelationPredictionEvaluator.evaluate needs the model on a CUDA device "
                 "(model.cuda()); this package has no CPU execution path")
+        if isinstance(self.shard, EntityShard) and self.shard.world > 1:
+            _check_sharded_model(spec, self.shard)     # a wrong table says so before the index check
         dev = spec.ent0.device
         kg = self.kg
         _check_index_range(kg.head_idx, kg.tail_idx, kg.relations, spec.n_ent, spec.n_rel)
@@ -239,7 +253,7 @@ class RelationPredictionEvaluator(object):
         csr = filter_csr(kg.dict_of_rels, kg.head_idx, kg.tail_idx, kg.relations)
         csr = tuple(x.to(dev, non_blocking=True) for x in csr)
         rr, frr = rank_relation_prediction(spec, h_d, t_d, r_d, csr, directed=self.directed,
-                                           engine=default_engine(), chunk=DEFAULT_CHUNK)
+                                           engine=default_engine(), chunk=DEFAULT_CHUNK, shard=self.shard)
         self.rank_true_rels = rr.cpu()
         self.filt_rank_true_rels = frr.cpu()
         self.evaluated = True
@@ -291,37 +305,108 @@ class TripletClassificationEvaluator(object):
     Scores come from ``model.scoring_function`` (the CUDA per-triple scorer), negatives from
     ``PositionalNegativeSampler(kg_val, kg_test=kg_test)`` as in the reference; ``sampler`` may be
     replaced after construction.
+
+    shard: ``torchkge_b200.engine.EntityShard`` or ``QueryShard``, optional, keyword-only
+    (extension); every rank of its group makes the same calls.  EntityShard with
+    ``local_storage=True`` (the model holds only entity rows [lo, hi)): per batch the h and t rows are
+    exchanged by one all-reduce and every rank scores the batch with the same per-triple kernel.
+    QueryShard, or EntityShard with full storage: every rank scores its contiguous slice of each score
+    vector (split by that vector's length; the QueryShard's own ``n`` is not used) and the slices are
+    all-gathered.  The negatives of every ``corrupt_kg`` call are rank 0's, sent to the other ranks in
+    one collective, so that ranks seeded differently still agree.  ``get_scores`` returns the full
+    score vector on every rank, equal bit for bit to the unsharded evaluator's; ``thresholds`` and
+    ``accuracy`` are the same on every rank and equal those of an unsharded evaluator whose sampler
+    draws what rank 0's sampler draws.
     """
 
-    def __init__(self, model, kg_val, kg_test):
+    def __init__(self, model, kg_val, kg_test, *, shard=None):
         from .sampling import PositionalNegativeSampler
         self.model = model
         self.kg_val = kg_val
         self.kg_test = kg_test
+        self.shard = shard
         self.is_cuda = next(self.model.parameters()).is_cuda
         self.evaluated = False
         self.thresholds = None
         self.sampler = PositionalNegativeSampler(self.kg_val, kg_test=self.kg_test)
 
-    def get_scores(self, heads, tails, relations, batch_size):
-        """Scores of the given triplets, computed batch by batch (evaluation.py:478-511)."""
-        if not self.is_cuda:
-            raise _lib.KgeLibraryError("TripletClassificationEvaluator needs the model on a CUDA device")
-        dev = next(self.model.parameters()).device
+    def _sharded(self):
+        """The shard when it splits anything; its argument errors are raised here, on every rank,
+        before any collective."""
+        shard = self.shard
+        if shard is None or shard.world == 1:
+            return None
+        if isinstance(shard, EntityShard):
+            held = shard.hi - shard.lo if shard.local_storage else shard.n_ent
+            if self.model.n_ent != held:
+                raise ValueError("EntityShard(local_storage=%s): rank %d should hold %d entity rows, the model "
+                                 "has %d" % (shard.local_storage, shard.rank, held, self.model.n_ent))
+            if shard.local_storage:
+                from .training import _training_code
+                _training_code(self.model)        # kinds the per-triple kernel does not score raise here
+        return shard
+
+    def _scoring_spec(self):
+        """ModelSpec over the tables ``model.scoring_function`` hands the per-triple kernel
+        (training._param_tensors): RotatE's (cos, sin) planes, TorusE's tables as they are (the kernel
+        takes fractional parts), Analogy's planes stacked."""
+        from .training import _kernel_dim, _param_tensors, _training_code
+        code = _training_code(self.model)
+        with torch.no_grad():
+            e0, e1, r0, r1 = (None if x is None else x.detach() for x in _param_tensors(self.model, code))
+        dim = _kernel_dim(self.model, code)
+        n_ent, n_rel = self.model.n_ent, self.model.n_rel
+        if code == _lib.ANALOGY:         # stacked (3, n, dim) copies: equally spaced planes
+            return ModelSpec(code, dim, n_ent, n_rel, e0[0], e0[1], r0[0], r0[1], ent2=e0[2], rel2=r0[2])
+        return ModelSpec(code, dim, n_ent, n_rel, e0, e1, r0, r1)
+
+    def _scores_here(self, heads, tails, relations, batch_size, dev):
         scores = []
         with torch.no_grad():
             for lo in range(0, heads.shape[0], batch_size):
                 sl = slice(lo, lo + batch_size)
                 scores.append(self.model.scoring_function(heads[sl].to(dev), tails[sl].to(dev),
                                                           relations[sl].to(dev)))
+        if not scores:           # a rank whose slice is empty
+            return torch.empty(0, dtype=torch.float32, device=dev)
         return torch.cat(scores, dim=0)
+
+    def get_scores(self, heads, tails, relations, batch_size):
+        """Scores of the given triplets, computed batch by batch (evaluation.py:478-511)."""
+        if not self.is_cuda:
+            raise _lib.KgeLibraryError("TripletClassificationEvaluator needs the model on a CUDA device")
+        dev = next(self.model.parameters()).device
+        shard = self._sharded()
+        if shard is None:
+            return self._scores_here(heads, tails, relations, batch_size, dev)
+        if isinstance(shard, EntityShard) and shard.local_storage:
+            spec = self._scoring_spec()
+            spec.ent_lo, spec.n_ent = shard.lo, shard.n_ent
+            h, t, r = (x.to(dev, torch.int64) for x in (heads, tails, relations))
+            return score_triples_entity_sharded(spec, h, t, r, shard, default_engine(), batch_size)
+        part = QueryShard(heads.shape[0], shard.rank, shard.world, shard.group)
+        mine = self._scores_here(*part.slice(heads, tails, relations), batch_size, dev)
+        return part.all_gather([mine])[0]
+
+    def _negatives(self, b_size, which):
+        """``sampler.corrupt_kg``; under a shard, rank 0's draws on every rank (the other ranks add
+        zeros into one sum-all-reduce)."""
+        nh, nt = self.sampler.corrupt_kg(b_size, self.is_cuda, which=which)
+        shard = self._sharded()
+        if shard is None:
+            return nh, nt
+        both = torch.stack([nh, nt]).to(next(self.model.parameters()).device, torch.int64)
+        if shard.rank != 0:
+            both.zero_()
+        both = shard.all_reduce_sum(both).cpu()
+        return both[0], both[1]
 
     def evaluate(self, b_size):
         """Thresholds from the validation graph (evaluation.py:513-541): for relation i the largest
         score among the negatives of its validation facts; relations absent from the validation set
         get the largest negative score overall."""
         r_idx = self.kg_val.relations
-        neg_heads, neg_tails = self.sampler.corrupt_kg(b_size, self.is_cuda, which='main')
+        neg_heads, neg_tails = self._negatives(b_size, 'main')
         neg_scores = self.get_scores(neg_heads, neg_tails, r_idx, b_size)
         n_rel = self.kg_val.n_rel
         r_dev = r_idx.to(neg_scores.device)
@@ -337,7 +422,7 @@ class TripletClassificationEvaluator(object):
         if not self.evaluated:
             self.evaluate(b_size)
         r_idx = self.kg_test.relations
-        neg_heads, neg_tails = self.sampler.corrupt_kg(b_size, self.is_cuda, which='test')
+        neg_heads, neg_tails = self._negatives(b_size, 'test')
         scores = self.get_scores(self.kg_test.head_idx, self.kg_test.tail_idx, r_idx, b_size)
         neg_scores = self.get_scores(neg_heads, neg_tails, r_idx, b_size)
         if self.is_cuda:
