@@ -296,19 +296,24 @@ def test_dict_filter_csr_equals_filter_csr_and_caches():
     assert torch.equal(o3, filter_csr(dt, qh, qr, qt)[0])
 
 
-def test_csr_slices_carry_the_row_of_entry_array():
-    """engine._csr_slice on (offs, ids, rows) triples: offsets and row ids are rebased to the slice."""
-    from torchkge_b200.engine import _csr_slice
+def test_csr_cut_carries_the_row_of_entry_array():
+    """engine._csr_cut on (offs, ids, rows) triples: offsets and row ids are rebased to each piece."""
+    from torchkge_b200.engine import _csr_cut
     offs = torch.tensor([0, 2, 2, 5, 6, 9])
     ids = torch.arange(100, 109)
     rows = torch.repeat_interleave(torch.arange(5), offs[1:] - offs[:-1]).to(torch.int32)
-    whole = _csr_slice((offs, ids, rows), 0, 5, 5)
+    whole, = _csr_cut((offs, ids, rows), [(0, 5)])
     assert whole[0] is offs and whole[2] is rows
-    o, i, q = _csr_slice((offs, ids, rows), 2, 5, 5)
+    (o, i, q), = _csr_cut((offs, ids, rows), [(2, 5)])
     assert o.tolist() == [0, 3, 4, 7] and i.tolist() == list(range(102, 109))
     assert q.tolist() == [0, 0, 0, 1, 2, 2, 2]
-    o2, i2 = _csr_slice((offs, ids), 1, 3, 5)
+    (o2, i2), = _csr_cut((offs, ids), [(1, 3)])
     assert o2.tolist() == [0, 0, 3] and i2.tolist() == [102, 103, 104]
+    # several pieces from one cut, an empty one among them; no CSR, no pieces
+    pieces = _csr_cut((offs, ids, rows), [(0, 2), (2, 2), (3, 5)])
+    assert [p[0].tolist() for p in pieces] == [[0, 2, 2], [0], [0, 1, 4]]
+    assert [p[2].tolist() for p in pieces] == [[0, 0], [], [0, 1, 1, 1]]
+    assert _csr_cut(None, [(0, 1), (1, 2)]) == [None, None] and _csr_cut((offs, ids), []) == []
 
 
 def test_data_loader_batches_in_fact_order():

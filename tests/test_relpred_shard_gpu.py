@@ -2,15 +2,13 @@
 vectors of every rank must equal the unsharded evaluator's exactly, and the oracle's.  Shards are
 emulated on one device by W threads whose collectives meet in process (tests/shard_threads.py); the
 public API then runs in two processes (gloo on one GPU; NCCL when two GPUs are present)."""
-import os
-import socket
 
 import pytest
 import torch
 
 import torchkge_b200 as tk
 from oracle import kge_oracle as oracle
-from tests import helpers
+from tests import gloo, helpers
 from tests.shard_threads import run_ranks, thread_collectives
 from torchkge_b200.engine import CudaEngine, EntityShard, ModelSpec, QueryShard, rank_relation_prediction
 
@@ -203,19 +201,9 @@ def test_argument_errors():
 
 
 # ------------------------------------------------------------------ 3. public API, two processes
-def _free_port():
-    with socket.socket() as s:
-        s.bind(("127.0.0.1", 0))
-        return s.getsockname()[1]
-
-
-def _api_worker(rank, world, port, backend, ret):
-    import torch.distributed as dist
-    os.environ["MASTER_ADDR"] = "127.0.0.1"
-    os.environ["MASTER_PORT"] = str(port)
+def _api_worker(rank, world, backend):
     dev = torch.device("cuda:%d" % (rank if backend == "nccl" else 0))
     torch.cuda.set_device(dev)
-    dist.init_process_group(backend, rank=rank, world_size=world)
     try:
         results = {}
         n_ent, n_rel, dim = 1100, 9, 16
@@ -250,19 +238,13 @@ def _api_worker(rank, world, port, backend, ret):
                 results["%s/%s/triplet" % (kind, name)] = (
                     torch.equal(got_c.thresholds.cpu().view(torch.int32), ref_c.thresholds.cpu().view(torch.int32))
                     and acc == ref_acc)
-        ret[rank] = results
+        return results
     except Exception as e:          # reported by the parent
-        ret[rank] = {"error": "%s: %s" % (type(e).__name__, e)}
-    finally:
-        dist.destroy_process_group()
+        return {"error": "%s: %s" % (type(e).__name__, e)}
 
 
 def _run_two_ranks(backend):
-    import torch.multiprocessing as mp
-    port = _free_port()
-    mgr = mp.Manager()
-    ret = mgr.dict()
-    mp.spawn(_api_worker, args=(2, port, backend, ret), nprocs=2, join=True)
+    ret = gloo.spawn(2, _api_worker, backend, backend=backend)
     for rank in (0, 1):
         res = ret[rank]
         assert "error" not in res, "rank %d: %s" % (rank, res.get("error"))

@@ -5,16 +5,12 @@ with fewer facts than ranks, chunk boundaries inside rank slices.  The CUDA engi
 oracle-backed stand-in with the same interface -- this tests the plumbing (row exchange, the fact
 split, the all-gathers, argument errors before any collective), not the kernels;
 tests/test_relpred_shard_gpu.py runs the kernels."""
-import os
-import socket
-
 import pytest
 import torch
 import torch.distributed as dist
-import torch.multiprocessing as mp
 
 from oracle import kge_oracle as oracle
-from tests import helpers
+from tests import gloo, helpers
 from torchkge_b200 import _lib
 from torchkge_b200.data import filter_csr
 from torchkge_b200.engine import (EntityShard, ModelSpec, QueryShard, rank_relation_prediction,
@@ -86,12 +82,6 @@ class OracleRelEngine:
         else:
             P = {"re_ent": ent[0], "im_ent": ent[1], "re_rel": rel0, "im_rel": rel1}
         return oracle.score_triples(kind, P, h, t, r)
-
-
-def _free_port():
-    with socket.socket() as s:
-        s.bind(("127.0.0.1", 0))
-        return s.getsockname()[1]
 
 
 class Counting:
@@ -179,27 +169,13 @@ def _run_errors(case):
     return False
 
 
-def _worker(rank, world, port, case, ret):
-    os.environ["MASTER_ADDR"] = "127.0.0.1"
-    os.environ["MASTER_PORT"] = str(port)
-    dist.init_process_group("gloo", rank=rank, world_size=world)
-    try:
-        if case[0] == "rank":
-            ret[rank] = bool(_run_ranks(*case[1:]))
-        elif case[0] == "scores":
-            ret[rank] = bool(_run_scores(*case[1:]))
-        else:
-            ret[rank] = bool(_run_errors(*case[1:]))
-    finally:
-        dist.destroy_process_group()
+def _worker(rank, world, case):
+    run = {"rank": _run_ranks, "scores": _run_scores, "errors": _run_errors}[case[0]]
+    return bool(run(*case[1:]))
 
 
 def _spawn(world, case):
-    port = _free_port()
-    mgr = mp.Manager()
-    ret = mgr.dict()
-    mp.spawn(_worker, args=(world, port, case, ret), nprocs=world, join=True)
-    assert dict(ret) == {i: True for i in range(world)}
+    assert gloo.spawn(world, _worker, case) == {i: True for i in range(world)}
 
 
 # (world, kind, storage, n_ent, n_facts, directed, chunk)

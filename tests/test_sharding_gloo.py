@@ -2,16 +2,11 @@
 torchkge_b200.engine.rank_link_prediction: range partition, query-row exchange, the single
 all-reduce of the counters.  The CUDA engine is replaced by an oracle-backed stand-in with the
 same interface -- this is a test of the sharding plumbing, not of the kernels."""
-import os
-import socket
-
 import pytest
 import torch
-import torch.distributed as dist
-import torch.multiprocessing as mp
 
 from oracle import kge_oracle as oracle
-from tests import helpers
+from tests import gloo, helpers
 from torchkge_b200 import _lib
 from torchkge_b200.data import filter_csr
 from torchkge_b200.engine import EntityShard, ModelSpec, rank_link_prediction
@@ -79,45 +74,27 @@ class OracleEngine:
         return raw.long(), raw.long() - sub.long()
 
 
-def _free_port():
-    with socket.socket() as s:
-        s.bind(("127.0.0.1", 0))
-        return s.getsockname()[1]
+def _worker(rank, world, kind, storage):
+    n_ent, n_rel, d = 203, 5, 24
+    kg, dh, dt = helpers.make_kg(n_ent, n_rel, n_facts=1500, n_test=90, seed=21)
+    model = helpers.make_model(kind, d, n_ent, n_rel, seed=21)
+    spec = ModelSpec.from_model(model)
+    shard = EntityShard.from_group(n_ent, local_storage=storage == "local_storage")
+    if storage == "local_storage":  # each rank only HOLDS its rows
+        spec = spec.narrowed(shard.lo, shard.hi)
+    csr_t = filter_csr(dt, kg.head_idx, kg.relations, kg.tail_idx)
+    csr_h = filter_csr(dh, kg.tail_idx, kg.relations, kg.head_idx)
+    out = rank_link_prediction(spec, kg.head_idx, kg.tail_idx, kg.relations, csr_t, csr_h,
+                               shard=shard, engine=OracleEngine(), chunk=32)
+    P = helpers.oracle_params(kind, model)
+    ref = oracle.link_prediction(kind, P, kg.head_idx, kg.tail_idx, kg.relations, dh, dt, 30)
+    return all(torch.equal(a, b) for a, b in zip(out, ref))
 
 
-def _worker(rank, world, port, kind, storage, ret):
-    os.environ["MASTER_ADDR"] = "127.0.0.1"
-    os.environ["MASTER_PORT"] = str(port)
-    dist.init_process_group("gloo", rank=rank, world_size=world)
-    try:
-        n_ent, n_rel, d = 203, 5, 24
-        kg, dh, dt = helpers.make_kg(n_ent, n_rel, n_facts=1500, n_test=90, seed=21)
-        model = helpers.make_model(kind, d, n_ent, n_rel, seed=21)
-        spec = ModelSpec.from_model(model)
-        shard = EntityShard.from_group(n_ent)
-        if storage == "local":  # each rank only HOLDS its rows
-            spec = spec.narrowed(shard.lo, shard.hi)
-        csr_t = filter_csr(dt, kg.head_idx, kg.relations, kg.tail_idx)
-        csr_h = filter_csr(dh, kg.tail_idx, kg.relations, kg.head_idx)
-        out = rank_link_prediction(spec, kg.head_idx, kg.tail_idx, kg.relations, csr_t, csr_h,
-                                   shard=shard, engine=OracleEngine(), chunk=32)
-        P = helpers.oracle_params(kind, model)
-        ref = oracle.link_prediction(kind, P, kg.head_idx, kg.tail_idx, kg.relations, dh, dt, 30)
-        ok = all(torch.equal(a, b) for a, b in zip(out, ref))
-        ret[rank] = bool(ok)
-    finally:
-        dist.destroy_process_group()
-
-
-@pytest.mark.parametrize("kind,storage", [("distmult", "full"), ("transe_l2", "local"),
-                                          ("complex", "local"), ("analogy", "local")])
+@pytest.mark.parametrize("kind,storage", [("distmult", "full"), ("transe_l2", "local_storage"),
+                                          ("complex", "local_storage"), ("analogy", "local_storage")])
 def test_two_rank_sharded_ranking_equals_single_process(kind, storage):
-    world = 2
-    port = _free_port()
-    mgr = mp.Manager()
-    ret = mgr.dict()
-    mp.spawn(_worker, args=(world, port, kind, storage, ret), nprocs=world, join=True)
-    assert dict(ret) == {0: True, 1: True}
+    assert gloo.spawn(2, _worker, kind, storage) == {0: True, 1: True}
 
 
 def test_single_process_stand_in_agrees_with_oracle():
@@ -136,41 +113,31 @@ def test_single_process_stand_in_agrees_with_oracle():
         assert torch.equal(a, b)
 
 
-def _worker_queries(rank, world, port, kind, n_test, ret):
+def _worker_queries(rank, world, kind, n_test):
     """The second decomposition (bench.py at N > 1 for tables that fit one GPU): replicated table,
     test triples split over the ranks, rank vectors all-gathered."""
     from torchkge_b200.engine import QueryShard
-    os.environ["MASTER_ADDR"] = "127.0.0.1"
-    os.environ["MASTER_PORT"] = str(port)
-    dist.init_process_group("gloo", rank=rank, world_size=world)
-    try:
-        n_ent, n_rel, d = 150, 4, 16
-        kg, dh, dt = helpers.make_kg(n_ent, n_rel, n_facts=1200, n_test=n_test, seed=33)
-        model = helpers.make_model(kind, d, n_ent, n_rel, seed=33)
-        spec = ModelSpec.from_model(model)
-        n = kg.n_facts
-        csr_t = filter_csr(dt, kg.head_idx, kg.relations, kg.tail_idx)
-        csr_h = filter_csr(dh, kg.tail_idx, kg.relations, kg.head_idx)
-        qs = QueryShard.from_group(n)
-        h, t, r = qs.slice(kg.head_idx, kg.tail_idx, kg.relations)
-        local = rank_link_prediction(spec, h, t, r, qs.csr(csr_t), qs.csr(csr_h), engine=OracleEngine(),
-                                     chunk=16)
-        assert all(x.shape[0] == qs.hi - qs.lo for x in local)
-        full = qs.all_gather(local)
-        P = helpers.oracle_params(kind, model)
-        ref = oracle.link_prediction(kind, P, kg.head_idx, kg.tail_idx, kg.relations, dh, dt, 30)
-        ret[rank] = bool(all(torch.equal(a, b) for a, b in zip(full, ref)))
-    finally:
-        dist.destroy_process_group()
+    n_ent, n_rel, d = 150, 4, 16
+    kg, dh, dt = helpers.make_kg(n_ent, n_rel, n_facts=1200, n_test=n_test, seed=33)
+    model = helpers.make_model(kind, d, n_ent, n_rel, seed=33)
+    spec = ModelSpec.from_model(model)
+    n = kg.n_facts
+    csr_t = filter_csr(dt, kg.head_idx, kg.relations, kg.tail_idx)
+    csr_h = filter_csr(dh, kg.tail_idx, kg.relations, kg.head_idx)
+    qs = QueryShard.from_group(n)
+    h, t, r = qs.slice(kg.head_idx, kg.tail_idx, kg.relations)
+    local = rank_link_prediction(spec, h, t, r, qs.csr(csr_t), qs.csr(csr_h), engine=OracleEngine(),
+                                 chunk=16)
+    assert all(x.shape[0] == qs.hi - qs.lo for x in local)
+    full = qs.all_gather(local)
+    P = helpers.oracle_params(kind, model)
+    ref = oracle.link_prediction(kind, P, kg.head_idx, kg.tail_idx, kg.relations, dh, dt, 30)
+    return all(torch.equal(a, b) for a, b in zip(full, ref))
 
 
 @pytest.mark.parametrize("kind,n_test,world", [("distmult", 75, 2), ("transe_l1", 1, 2), ("complex", 50, 3)])
 def test_query_sharded_ranking_equals_single_process(kind, n_test, world):
-    port = _free_port()
-    mgr = mp.Manager()
-    ret = mgr.dict()
-    mp.spawn(_worker_queries, args=(world, port, kind, n_test, ret), nprocs=world, join=True)
-    assert dict(ret) == {i: True for i in range(world)}
+    assert gloo.spawn(world, _worker_queries, kind, n_test) == {i: True for i in range(world)}
 
 
 def test_query_shard_bounds():

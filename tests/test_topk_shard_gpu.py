@@ -2,15 +2,13 @@
 through ``ent_lo``) merged by kge_topk_merge must give the unsharded result bit for bit -- ids,
 score bits and the order among exact ties.  Shards are emulated on one device, then the public API
 runs in two processes (gloo on one GPU; NCCL when two GPUs are present)."""
-import os
-import socket
 
 import numpy as np
 import pytest
 import torch
 
 import torchkge_b200 as tk
-from tests import helpers
+from tests import gloo, helpers
 from torchkge_b200 import _lib
 from torchkge_b200.engine import CudaEngine, EntityShard, ModelSpec, QueryShard
 from torchkge_b200.inference import _mask_csr
@@ -250,12 +248,6 @@ def test_merge_rejects_arguments_out_of_range():
 
 
 # ------------------------------------------------------------------ 4./5. public API, two processes
-def _free_port():
-    with socket.socket() as s:
-        s.bind(("127.0.0.1", 0))
-        return s.getsockname()[1]
-
-
 def _local_model(kind, model, lo, hi, n_rel, dim):
     """The same model holding only entity rows [lo, hi)."""
     part = helpers.make_model(kind, dim, hi - lo, n_rel, seed=0)
@@ -263,13 +255,9 @@ def _local_model(kind, model, lo, hi, n_rel, dim):
     return part.to(next(model.parameters()).device)
 
 
-def _api_worker(rank, world, port, backend, ret):
-    import torch.distributed as dist
-    os.environ["MASTER_ADDR"] = "127.0.0.1"
-    os.environ["MASTER_PORT"] = str(port)
+def _api_worker(rank, world, backend):
     dev = torch.device("cuda:%d" % (rank if backend == "nccl" else 0))
     torch.cuda.set_device(dev)
-    dist.init_process_group(backend, rank=rank, world_size=world)
     try:
         results = {}
         n_ent, n_rel, dim = 1100, 9, 16
@@ -300,19 +288,13 @@ def _api_worker(rank, world, port, backend, ret):
                 results["%s/%s/relation" % (kind, name)] = (
                     torch.equal(got_r.predictions, ref_r.predictions)
                     and torch.equal(got_r.scores.view(torch.int32), ref_r.scores.view(torch.int32)))
-        ret[rank] = results
+        return results
     except Exception as e:          # reported by the parent
-        ret[rank] = {"error": "%s: %s" % (type(e).__name__, e)}
-    finally:
-        dist.destroy_process_group()
+        return {"error": "%s: %s" % (type(e).__name__, e)}
 
 
 def _run_two_ranks(backend):
-    import torch.multiprocessing as mp
-    port = _free_port()
-    mgr = mp.Manager()
-    ret = mgr.dict()
-    mp.spawn(_api_worker, args=(2, port, backend, ret), nprocs=2, join=True)
+    ret = gloo.spawn(2, _api_worker, backend, backend=backend)
     for rank in (0, 1):
         res = ret[rank]
         assert "error" not in res, "rank %d: %s" % (rank, res.get("error"))

@@ -3,16 +3,11 @@ topk_entity_inference / topk_relation_inference under EntityShard (full and loca
 empty shard) and QueryShard (fewer queries than ranks).  The CUDA engine is replaced by an
 oracle-backed stand-in with the same interface -- this tests the sharding plumbing (row exchange,
 padding, the all-gathers, the merge), not the kernels; tests/test_topk_shard_gpu.py runs the kernels."""
-import os
-import socket
-
 import pytest
 import torch
-import torch.distributed as dist
-import torch.multiprocessing as mp
 
 from oracle import kge_oracle as oracle
-from tests import helpers
+from tests import gloo, helpers
 from torchkge_b200 import _lib
 from torchkge_b200.engine import (EntityShard, ModelSpec, QueryShard, topk_entity_inference,
                                   topk_relation_inference)
@@ -90,12 +85,6 @@ class OracleTopkEngine:
         return pred, vals
 
 
-def _free_port():
-    with socket.socket() as s:
-        s.bind(("127.0.0.1", 0))
-        return s.getsockname()[1]
-
-
 def _reference(kind, model, task, q1, q2, k, dictionary, side):
     """The oracle's dense scores, masked with -inf, then sort(descending=True)[:, :k]."""
     P = helpers.oracle_params(kind, model)
@@ -137,18 +126,8 @@ def _run(rank, world, task, kind, storage, n_ent, n_queries, k, side):
     else:
         pred, vals = topk_relation_inference(spec, q1, q2, k, mask, shard=shard, engine=eng, chunk=7)
     want_ids, want_vals = _reference(kind, model, task, q1, q2, k, dictionary, side)
-    return (pred.shape == (n_queries, k) and torch.equal(pred, want_ids)
-            and torch.equal(vals.view(torch.int32), want_vals.view(torch.int32)))
-
-
-def _worker(rank, world, port, case, ret):
-    os.environ["MASTER_ADDR"] = "127.0.0.1"
-    os.environ["MASTER_PORT"] = str(port)
-    dist.init_process_group("gloo", rank=rank, world_size=world)
-    try:
-        ret[rank] = bool(_run(rank, world, *case))
-    finally:
-        dist.destroy_process_group()
+    return bool(pred.shape == (n_queries, k) and torch.equal(pred, want_ids)
+                and torch.equal(vals.view(torch.int32), want_vals.view(torch.int32)))
 
 
 # (world, task, kind, storage, n_ent, n_queries, k, side)
@@ -167,11 +146,7 @@ CASES = [
 @pytest.mark.parametrize("case", CASES, ids=["%s-%s-%s-w%d" % (c[1], c[2], c[3], c[0]) for c in CASES])
 def test_sharded_topk_equals_oracle(case):
     world = case[0]
-    port = _free_port()
-    mgr = mp.Manager()
-    ret = mgr.dict()
-    mp.spawn(_worker, args=(world, port, case[1:], ret), nprocs=world, join=True)
-    assert dict(ret) == {i: True for i in range(world)}
+    assert gloo.spawn(world, _run, *case[1:]) == {i: True for i in range(world)}
 
 
 def test_key_order_of_the_stand_in():

@@ -4,14 +4,12 @@ unsharded fused step of the same loss -- loss within 1e-5 relative, gradients un
 rule of tests/test_train_gpu.py.  Every rank counts the positive's term only for the negatives it owns.
 Then the public API trains in two processes over gloo on one GPU; the NCCL form needs two GPUs and is
 skipped on a machine with one."""
-import os
-import socket
 
 import pytest
 import torch
 
 import torchkge_b200 as tk
-from tests import helpers
+from tests import gloo, helpers
 from torchkge_b200 import _lib
 from torchkge_b200.engine import CudaEngine, EntityShard, _exchanged_rows
 from torchkge_b200.training import ShardedStep, _kernel_dim, _MarginStep, _param_tensors, _row_spec, _training_code
@@ -143,12 +141,6 @@ def test_empty_shards_and_one_sided_draws(kind, d, loss):
 
 
 # ---------------------------------------------------------------- 2. public API, two processes
-def _free_port():
-    with socket.socket() as s:
-        s.bind(("127.0.0.1", 0))
-        return s.getsockname()[1]
-
-
 def _local_model(kind, model, lo, hi, n_rel, dim):
     part = helpers.make_model(kind, dim, hi - lo, n_rel, seed=0)
     part.load_state_dict({name: w[lo:hi] if "ent_emb" in name else w for name, w in model.state_dict().items()})
@@ -168,13 +160,9 @@ def _train(model, kg, batches, shard, steps, seed, crit):
     return losses
 
 
-def _api_worker(rank, world, port, backend, ret):
-    import torch.distributed as dist
-    os.environ["MASTER_ADDR"] = "127.0.0.1"
-    os.environ["MASTER_PORT"] = str(port)
+def _api_worker(rank, world, backend):
     dev = torch.device("cuda:%d" % (rank if backend == "nccl" else 0))
     torch.cuda.set_device(dev)
-    dist.init_process_group(backend, rank=rank, world_size=world)
     try:
         res = {}
         n_ent, n_rel = 3001, 7
@@ -206,19 +194,13 @@ def _api_worker(rank, world, port, backend, ret):
             res["loss_mismatch_raises"] = False
         except ValueError:
             res["loss_mismatch_raises"] = True
-        ret[rank] = res
+        return res
     except Exception as e:          # reported by the parent
-        ret[rank] = {"error": "%s: %s" % (type(e).__name__, e)}
-    finally:
-        dist.destroy_process_group()
+        return {"error": "%s: %s" % (type(e).__name__, e)}
 
 
 def _run_two_ranks(backend):
-    import torch.multiprocessing as mp
-    port = _free_port()
-    mgr = mp.Manager()
-    ret = mgr.dict()
-    mp.spawn(_api_worker, args=(2, port, backend, ret), nprocs=2, join=True)
+    ret = gloo.spawn(2, _api_worker, backend, backend=backend)
     for rank in (0, 1):
         res = ret[rank]
         assert "error" not in res, "rank %d: %s" % (rank, res.get("error"))

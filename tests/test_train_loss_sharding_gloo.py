@@ -4,17 +4,14 @@ unsharded loss and gradients, the collectives are the margin step's (stack_all a
 ranks that disagree on the loss kind raise on every rank, and an unsupported criterion raises before
 any collective.  The CUDA engine is an oracle-backed stand-in; tests/test_train_loss_shard_gpu.py runs
 the kernels."""
-import os
-
 import pytest
 import torch
-import torch.distributed as dist
 
 import torchkge_b200 as tk
 from oracle import kge_oracle as oracle
-from tests import helpers
+from tests import gloo, helpers
 from tests.test_train_sharding_gloo import (_ENT_KEYS, _KIND_OF_CODE, _REL_KEYS, CountingShard, OracleStepEngine,
-                                            Shard, _free_port, _local_model, draws)
+                                            Shard, _local_model, draws)
 from torchkge_b200 import _lib
 from torchkge_b200.engine import EntityShard
 from torchkge_b200.training import fused_loss_step, sharded_margin_step
@@ -100,10 +97,7 @@ def _run(rank, world, kind, loss_kind, n_ent, b, n_neg, steps):
     return ok
 
 
-def _worker(rank, world, port, case, ret):
-    os.environ["MASTER_ADDR"] = "127.0.0.1"
-    os.environ["MASTER_PORT"] = str(port)
-    dist.init_process_group("gloo", rank=rank, world_size=world)
+def _worker(rank, world, case):
     try:
         if case[0] == "mismatch":
             shard = EntityShard.from_group(30, local_storage=True)
@@ -113,24 +107,16 @@ def _worker(rank, world, port, case, ret):
             try:
                 fused_loss_step(model, h, h, h % 4, crit, n_neg=3, bern_probs=torch.full((4,), 0.5), seed=11,
                                 offset=1, shard=shard)
-                ret[rank] = {"raised": False}
+                return {"raised": False}
             except ValueError as e:
-                ret[rank] = {"raised": "loss kind" in str(e)}
-        else:
-            ret[rank] = _run(rank, world, *case)
+                return {"raised": "loss kind" in str(e)}
+        return _run(rank, world, *case)
     except Exception as e:          # reported by the parent
-        ret[rank] = {"error": "%s: %s" % (type(e).__name__, e)}
-    finally:
-        dist.destroy_process_group()
+        return {"error": "%s: %s" % (type(e).__name__, e)}
 
 
 def _spawn(world, case):
-    import torch.multiprocessing as mp
-    port = _free_port()
-    mgr = mp.Manager()
-    ret = mgr.dict()
-    mp.spawn(_worker, args=(world, port, case, ret), nprocs=world, join=True)
-    return dict(ret)
+    return gloo.spawn(world, _worker, case)
 
 
 # (world, kind, loss kind, n_ent, b, n_neg, steps)

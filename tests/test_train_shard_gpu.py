@@ -6,14 +6,13 @@ API trains in two processes (gloo on one GPU; NCCL when two GPUs are present).""
 import ctypes
 import os
 import re
-import socket
 
 import pytest
 import torch
 
 import torchkge_b200 as tk
 from oracle import kge_oracle as oracle
-from tests import helpers
+from tests import gloo, helpers
 from torchkge_b200 import _lib
 from torchkge_b200.engine import CudaEngine, EntityShard, _exchanged_rows, _ptr, _stream
 from torchkge_b200.training import (ShardedStep, _kernel_dim, _MarginStep, _param_tensors, _row_spec,
@@ -273,12 +272,6 @@ def test_legacy_calls_still_accept_their_arguments():
 
 
 # ---------------------------------------------------------------- 5. public API, two processes
-def _free_port():
-    with socket.socket() as s:
-        s.bind(("127.0.0.1", 0))
-        return s.getsockname()[1]
-
-
 def _local_model(kind, model, lo, hi, n_rel, dim):
     part = helpers.make_model(kind, dim, hi - lo, n_rel, seed=0)
     part.load_state_dict({name: w[lo:hi] if "ent_emb" in name else w for name, w in model.state_dict().items()})
@@ -298,13 +291,9 @@ def _train(model, kg, batches, shard, steps, seed):
     return losses
 
 
-def _api_worker(rank, world, port, backend, ret):
-    import torch.distributed as dist
-    os.environ["MASTER_ADDR"] = "127.0.0.1"
-    os.environ["MASTER_PORT"] = str(port)
+def _api_worker(rank, world, backend):
     dev = torch.device("cuda:%d" % (rank if backend == "nccl" else 0))
     torch.cuda.set_device(dev)
-    dist.init_process_group(backend, rank=rank, world_size=world)
     try:
         res = {}
         n_ent, n_rel = 3001, 7
@@ -335,19 +324,13 @@ def _api_worker(rank, world, port, backend, ret):
             res["seed_mismatch_raises"] = False
         except ValueError:
             res["seed_mismatch_raises"] = True
-        ret[rank] = res
+        return res
     except Exception as e:          # reported by the parent
-        ret[rank] = {"error": "%s: %s" % (type(e).__name__, e)}
-    finally:
-        dist.destroy_process_group()
+        return {"error": "%s: %s" % (type(e).__name__, e)}
 
 
 def _run_two_ranks(backend):
-    import torch.multiprocessing as mp
-    port = _free_port()
-    mgr = mp.Manager()
-    ret = mgr.dict()
-    mp.spawn(_api_worker, args=(2, port, backend, ret), nprocs=2, join=True)
+    ret = gloo.spawn(2, _api_worker, backend, backend=backend)
     for rank in (0, 1):
         res = ret[rank]
         assert "error" not in res, "rank %d: %s" % (rank, res.get("error"))

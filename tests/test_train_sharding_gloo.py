@@ -4,16 +4,11 @@ backward all-reduce of grad_hrows / grad_trows / relation gradients, the scatter
 gradient, and the argument errors raised before any collective.  The CUDA engine is replaced by an
 oracle-backed stand-in with the same methods -- this tests the plumbing, not the kernels;
 tests/test_train_shard_gpu.py runs the kernels."""
-import os
-import socket
-
 import pytest
 import torch
-import torch.distributed as dist
-import torch.multiprocessing as mp
 
 from oracle import kge_oracle as oracle
-from tests import helpers
+from tests import gloo, helpers
 from torchkge_b200 import _lib
 from torchkge_b200.engine import EntityShard, QueryShard
 from torchkge_b200.training import fused_margin_step, sharded_margin_step
@@ -169,10 +164,7 @@ def _run(rank, world, kind, n_ent, b, n_neg, steps):
     return ok
 
 
-def _worker(rank, world, port, case, ret):
-    os.environ["MASTER_ADDR"] = "127.0.0.1"
-    os.environ["MASTER_PORT"] = str(port)
-    dist.init_process_group("gloo", rank=rank, world_size=world)
+def _worker(rank, world, case):
     try:
         if case[0] == "mismatch":
             shard = EntityShard.from_group(30, local_storage=True)
@@ -181,29 +173,16 @@ def _worker(rank, world, port, case, ret):
             try:
                 sharded_margin_step(model, h, h, h % 4, 1.0, 3, torch.full((4,), 0.5), 11 + rank, 1, shard,
                                     engine=OracleStepEngine())
-                ret[rank] = {"raised": False}
+                return {"raised": False}
             except ValueError:
-                ret[rank] = {"raised": True}
-        else:
-            ret[rank] = _run(rank, world, *case)
+                return {"raised": True}
+        return _run(rank, world, *case)
     except Exception as e:          # reported by the parent
-        ret[rank] = {"error": "%s: %s" % (type(e).__name__, e)}
-    finally:
-        dist.destroy_process_group()
-
-
-def _free_port():
-    with socket.socket() as s:
-        s.bind(("127.0.0.1", 0))
-        return s.getsockname()[1]
+        return {"error": "%s: %s" % (type(e).__name__, e)}
 
 
 def _spawn(world, case):
-    port = _free_port()
-    mgr = mp.Manager()
-    ret = mgr.dict()
-    mp.spawn(_worker, args=(world, port, case, ret), nprocs=world, join=True)
-    return dict(ret)
+    return gloo.spawn(world, _worker, case)
 
 
 # (world, kind, n_ent, b, n_neg, steps)

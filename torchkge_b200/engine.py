@@ -514,23 +514,21 @@ def default_engine():
     return _default_engine
 
 
-class EntityShard:
-    """Range partition of the entity table over the ranks of a process group
-    (SURVEY.md section 8e): rank g holds rows [g*ceil(nE/G), (g+1)*ceil(nE/G))."""
+class _RangeSplit:
+    """n items split over the ranks of a process group: rank g gets [g*per, (g+1)*per), clipped to n,
+    with per = ceil(n / world).  Every collective of a sharded call goes through ``all_reduce_sum`` /
+    ``stack_all`` of the shard object the caller passed (tests substitute them)."""
 
-    def __init__(self, n_ent, rank=0, world=1, group=None, local_storage=False):
-        per = (n_ent + world - 1) // world
-        self.n_ent, self.rank, self.world, self.group = n_ent, rank, world, group
-        #: True when the model on this rank HOLDS only rows [lo, hi) (its row 0 is entity lo);
-        #: False when every rank holds the full table and merely scans its own range
-        self.local_storage = local_storage
-        self.lo = min(n_ent, rank * per)
-        self.hi = min(n_ent, (rank + 1) * per)
+    def __init__(self, n, rank, world, group):
+        self.rank, self.world, self.group = rank, world, group
+        self.per = (n + world - 1) // world
+        self.lo = min(n, rank * self.per)
+        self.hi = min(n, (rank + 1) * self.per)
 
     @classmethod
-    def from_group(cls, n_ent, group=None, local_storage=False):
+    def from_group(cls, n, group=None, *args, **kwargs):
         import torch.distributed as dist
-        return cls(n_ent, dist.get_rank(group), dist.get_world_size(group), group, local_storage)
+        return cls(n, dist.get_rank(group), dist.get_world_size(group), group, *args, **kwargs)
 
     def all_reduce_sum(self, t):
         if self.world > 1:
@@ -547,23 +545,34 @@ class EntityShard:
         dist.all_gather(list(everyone.unbind(0)), t.contiguous(), group=self.group)
         return everyone
 
+    def split(self, m):
+        """The QueryShard of m items over the same ranks; its collectives go through this shard's."""
+        part = QueryShard(m, self.rank, self.world, self.group)
+        part.all_reduce_sum, part.stack_all = self.all_reduce_sum, self.stack_all
+        return part
 
-class QueryShard:
+
+class EntityShard(_RangeSplit):
+    """Range partition of the entity table over the ranks of a process group
+    (SURVEY.md section 8e): rank g holds rows [g*ceil(nE/G), (g+1)*ceil(nE/G))."""
+
+    def __init__(self, n_ent, rank=0, world=1, group=None, local_storage=False):
+        super().__init__(n_ent, rank, world, group)
+        self.n_ent = n_ent
+        #: True when the model on this rank HOLDS only rows [lo, hi) (its row 0 is entity lo);
+        #: False when every rank holds the full table and merely scans its own range (_check_table)
+        self.local_storage = local_storage
+
+
+class QueryShard(_RangeSplit):
     """Contiguous split of n test triples over the ranks of a process group, for tables that fit
     one GPU (SURVEY.md section 8e, second form): the entity table is replicated, every rank ranks
     ITS triples against all entities -- independent units, no collective on the data path -- and
     the rank vectors are all-gathered at the end."""
 
     def __init__(self, n, rank=0, world=1, group=None):
-        self.n, self.rank, self.world, self.group = int(n), rank, world, group
-        self.per = (self.n + world - 1) // world
-        self.lo = min(self.n, rank * self.per)
-        self.hi = min(self.n, (rank + 1) * self.per)
-
-    @classmethod
-    def from_group(cls, n, group=None):
-        import torch.distributed as dist
-        return cls(n, dist.get_rank(group), dist.get_world_size(group), group)
+        self.n = int(n)
+        super().__init__(self.n, rank, world, group)
 
     def slice(self, *tensors):
         """This rank's rows of each (n,) tensor."""
@@ -571,13 +580,7 @@ class QueryShard:
 
     def csr(self, filt):
         """This rank's rows of a CSR over the n triples (offsets rebased)."""
-        return None if filt is None else _csr_slice(filt, self.lo, self.hi, self.n)
-
-    def all_reduce_sum(self, t):
-        if self.world > 1:
-            import torch.distributed as dist
-            dist.all_reduce(t, op=dist.ReduceOp.SUM, group=self.group)
-        return t
+        return _csr_cut(filt, [(self.lo, self.hi)])[0]
 
     def all_gather(self, parts):
         """Per-rank results (one row per local triple: vectors, or tensors with the same trailing
@@ -585,30 +588,85 @@ class QueryShard:
         all of them."""
         if self.world == 1:
             return list(parts)
-        import torch.distributed as dist
         k = len(parts)
         trail = tuple(parts[0].shape[1:])
         mine = torch.zeros((k, self.per) + trail, dtype=parts[0].dtype, device=parts[0].device)
         for i, x in enumerate(parts):
             mine[i, :x.shape[0]] = x
-        everyone = torch.empty((self.world,) + tuple(mine.shape), dtype=mine.dtype, device=mine.device)
-        dist.all_gather([everyone[i] for i in range(self.world)], mine, group=self.group)
+        everyone = self.stack_all(mine)
         # rank-major slices of length `per` concatenate to the original order of the triples
         full = everyone.transpose(0, 1).reshape((k, self.world * self.per) + trail)[:, :self.n]
         return [full[i] for i in range(k)]
 
 
-def _csr_slice(filt, lo, hi, n):
-    """CSR rows [lo, hi) with offsets (and row ids, when present) rebased to 0."""
-    offs, ids = filt[0], filt[1]
-    if lo == 0 and hi == n:
-        return filt
-    base = int(offs[lo].item())
-    end = int(offs[hi].item())
-    out = ((offs[lo:hi + 1] - base).contiguous(), ids[base:end].contiguous())
-    if len(filt) > 2 and filt[2] is not None:
-        out = out + ((filt[2][base:end] - lo).contiguous(),)
+def _csr_cut(csr, ranges):
+    """Rows [lo, hi) of a CSR (offs (n+1,), ids[, row ids]) for every (lo, hi) of ``ranges``, offsets
+    rebased to 0 and row ids (when present) to lo; host or device tensors.  One device -> host read
+    for all ranges, none when the only range is the whole CSR."""
+    if csr is None:
+        return [None] * len(ranges)
+    offs, ids = csr[0], csr[1]
+    if not ranges or ranges == [(0, offs.shape[0] - 1)]:
+        return [csr] * len(ranges)
+    qid = csr[2] if len(csr) > 2 else None
+    at = offs[torch.tensor([x for r in ranges for x in r], device=offs.device)].tolist()
+    out = []
+    for (lo, hi), a, b in zip(ranges, at[0::2], at[1::2]):
+        part = ((offs[lo:hi + 1] - a).contiguous(), ids[a:b].contiguous())
+        out.append(part if qid is None else part + ((qid[a:b] - lo).contiguous(),))
     return out
+
+
+def _check_table(spec, shard):
+    """The table rule of an EntityShard (DESIGN.md section 6), checked on every rank before the first
+    collective: under local storage the model holds exactly rows [lo, hi) (ent_lo == lo), under full
+    storage the whole table (ent_lo == 0, n_rows == n_ent).  ``spec``: anything with n_ent, ent_lo
+    and n_rows."""
+    lo, rows = (shard.lo, shard.hi - shard.lo) if shard.local_storage else (0, shard.n_ent)
+    if (spec.n_ent, spec.ent_lo, spec.n_rows) != (shard.n_ent, lo, rows):
+        raise ValueError("EntityShard(local_storage=%s): rank %d should hold %d entity rows (entities [%d, %d)), "
+                         "the model holds %d entity rows from entity %d (the shard partitions %d entities, the "
+                         "model has %d)" % (shard.local_storage, shard.rank, rows, lo, lo + rows, spec.n_rows,
+                                            spec.ent_lo, shard.n_ent, spec.n_ent))
+
+
+def _scanned(spec, shard):
+    """The rows [lo, hi) this rank scans (after _check_table): the model's own rows under local storage,
+    views into the whole table under full storage."""
+    if (spec.ent_lo, spec.n_rows) == (shard.lo, shard.hi - shard.lo):
+        return spec
+    return spec.narrowed(shard.lo, shard.hi)
+
+
+def _check_queries(shard, n):
+    """A QueryShard splits exactly the n facts or queries of the call."""
+    if shard.n != n:
+        raise ValueError("QueryShard covers %d facts or queries, got %d" % (shard.n, n))
+
+
+def shard_spec(model, shard=None, who="evaluate", n=None, build=ModelSpec.from_model):
+    """The ModelSpec the engine reads for ``model`` (``build(model)``) under ``shard``, after the shard's
+    argument checks: under an EntityShard with local storage the model holds entity rows [lo, hi) and its
+    row 0 is entity lo (_check_table); a QueryShard must cover ``n`` facts, when ``n`` is given.  The
+    checks come first, then the model must be on a CUDA device."""
+    spec = build(model)
+    if isinstance(shard, EntityShard):
+        if shard.local_storage:
+            spec = ModelSpec(spec.code, spec.dim, shard.n_ent, spec.n_rel, spec.ent0, spec.ent1, spec.rel0,
+                             spec.rel1, ent_lo=shard.lo, ent2=spec.ent2, rel2=spec.rel2)
+        _check_table(spec, shard)
+    elif isinstance(shard, QueryShard) and n is not None:
+        _check_queries(shard, n)
+    if not spec.ent0.is_cuda:
+        raise _lib.KgeLibraryError("%s needs the model on a CUDA device (model.cuda()); this package has no "
+                                   "CPU execution path" % who)
+    return spec
+
+
+def _by_query_slices(shard, run, idx, csr=None):
+    """``run(*this rank's slice of every tensor of idx, its rows of csr)`` -> (n_local, ...) results, then
+    ONE all-gather: the full results on every rank."""
+    return shard.all_gather(list(run(*shard.slice(*idx), shard.csr(csr))))
 
 
 class LazyRanks:
@@ -651,9 +709,11 @@ def rank_link_prediction(spec, h_idx, t_idx, r_idx, filt_tail, filt_head, shard=
     """
     engine = engine or default_engine()
     n = h_idx.shape[0]
-    if shard is not None and shard.world > 1:
-        if (spec.ent_lo, spec.n_rows) != (shard.lo, shard.hi - shard.lo):
-            spec = spec.narrowed(shard.lo, shard.hi)
+    table = spec
+    if shard is not None:
+        _check_table(spec, shard)
+        spec = _scanned(spec, shard)
+        if spec is not table:
             packed = None
     mark = getattr(engine, "mark", lambda label: None)
     mark("step begin")
@@ -681,8 +741,8 @@ def rank_link_prediction(spec, h_idx, t_idx, r_idx, filt_tail, filt_head, shard=
                      if (tc_packed is not None or refine) else None)
         pending = []
         call = 0
-        for lo in range(0, n, chunk):
-            hi = min(n, lo + chunk)
+        chunks = [(lo, min(n, lo + chunk)) for lo in range(0, n, chunk)]
+        for c, (lo, hi) in enumerate(chunks):
             h, t, r = h_idx[lo:hi], t_idx[lo:hi], r_idx[lo:hi]
             hrows = engine.gather_rows(spec, h)
             trows = engine.gather_rows(spec, t)
@@ -703,31 +763,13 @@ def rank_link_prediction(spec, h_idx, t_idx, r_idx, filt_tail, filt_head, shard=
                     handle = engine.rank_side(spec, packed, side, hrows, trows, r, true_idx, None,
                                               raw[lo:hi], sub[lo:hi])
                 call += 1
-                pending.append((handle, which, lo, hi, sub))
+                pending.append((handle, which, c, lo, hi, sub))
                 mark("rank_side %d enqueued" % side)
-        filts = [filt_tail, filt_head]
-        for k in (0, 1):
-            if callable(filts[k]):
-                filts[k] = filts[k]()
-        # chunk boundaries of the CSRs: one device -> host read for all of them (none for a single chunk)
-        cuts = [None, None]
-        if n > chunk:
-            starts = torch.tensor(list(range(0, n, chunk)) + [n], device=dev)
-            for k in (0, 1):
-                if filts[k] is not None:
-                    cuts[k] = dict(zip(starts.tolist(), filts[k][0][starts].tolist()))
-        for handle, which, lo, hi, sub in pending:
+        filts = [f() if callable(f) else f for f in (filt_tail, filt_head)]
+        parts = [_csr_cut(f, chunks) for f in filts]   # one device -> host read per CSR, none for one chunk
+        for handle, which, c, lo, hi, sub in pending:
             if filts[which] is not None:
-                offs, ids = filts[which][0], filts[which][1]
-                qid = filts[which][2] if len(filts[which]) > 2 else None
-                if cuts[which] is None:
-                    part = filts[which]
-                else:
-                    a, b = cuts[which][lo], cuts[which][hi]
-                    part = ((offs[lo:hi + 1] - a).contiguous(), ids[a:b].contiguous())
-                    if qid is not None:
-                        part = part + ((qid[a:b] - lo).contiguous(),)
-                engine.filter_side(handle, part, sub[lo:hi])
+                engine.filter_side(handle, parts[which][c], sub[lo:hi])
         mark("filters enqueued")
         del pending
         overflow = None
@@ -746,7 +788,7 @@ def rank_link_prediction(spec, h_idx, t_idx, r_idx, filt_tail, filt_head, shard=
     result = (rank_h, rank_t, filt_h, filt_t)
 
     def redo():
-        return rank_link_prediction(spec, h_idx, t_idx, r_idx, filts[0], filts[1], shard=shard,
+        return rank_link_prediction(table, h_idx, t_idx, r_idx, filts[0], filts[1], shard=shard,
                                     engine=engine, chunk=chunk, exact=True)
 
     lazy = LazyRanks(result, overflow, redo)
@@ -771,20 +813,6 @@ def relation_spec(spec):
     return ModelSpec(spec.code, spec.dim, spec.n_rel, spec.n_rel, cand0, cand1, None, None, ent2=cand2)
 
 
-def _check_sharded_model(spec, shard):
-    """Argument errors of an entity-sharded call, raised on every rank before the first collective:
-    the table must be this rank's rows [lo, hi) (local storage) or the whole table (full storage)."""
-    if spec.n_ent != shard.n_ent:
-        raise ValueError("the shard partitions %d entities, the model has %d" % (shard.n_ent, spec.n_ent))
-    if shard.local_storage:
-        if (spec.ent_lo, spec.n_rows) != (shard.lo, shard.hi - shard.lo):
-            raise ValueError("EntityShard(local_storage=True): rank %d holds rows [%d, %d) but the model has %d "
-                             "entity rows from %d" % (shard.rank, shard.lo, shard.hi, spec.n_rows, spec.ent_lo))
-    elif (spec.ent_lo, spec.n_rows) != (0, shard.n_ent):
-        raise ValueError("EntityShard(local_storage=False) needs the whole entity table on every rank "
-                         "(got %d rows)" % spec.n_rows)
-
-
 def rank_relation_prediction(spec, h_idx, t_idx, r_idx, filt, directed=True, engine=None,
                              chunk=DEFAULT_CHUNK, shard=None):
     """Rank every fact's true relation against all relations (RelationPredictionEvaluator,
@@ -796,27 +824,25 @@ def rank_relation_prediction(spec, h_idx, t_idx, r_idx, filt, directed=True, eng
                the directed true score (evaluation.py:99-107)
     shard      None; QueryShard over the n facts: every rank ranks its slice of the facts (and of
                ``filt``) against the replicated table; EntityShard: the relations, the candidates, are
-               on every rank, so the facts are split too -- under local storage (spec.ent_lo /
-               spec.n_ent set from the shard) the h / t rows of each chunk are first exchanged by one
-               all-reduce, and the chunk's facts split as QueryShard splits them; under full storage
-               the facts are split as QueryShard(n) splits them.  Either way one all-gather per split
-               brings every rank the full rank vectors, equal to the unsharded call's.
+               on every rank, so the facts are split too -- under local storage the h / t rows of each
+               chunk are first exchanged by one all-reduce, and the chunk's facts split as
+               ``shard.split`` splits them (_exchanged_chunks); under full storage the facts are split
+               as ``shard.split(n)`` splits them.  Either way one all-gather per split brings every
+               rank the full rank vectors, equal to the unsharded call's.
     Returns (rank_true_rels, filt_rank_true_rels), int64 device tensors.
     """
     engine = engine or default_engine()
     n = h_idx.shape[0]
     dev = spec.ent0.device
     rspec = None if spec.code == _lib.RESCAL else relation_spec(spec)   # unsupported models raise here
-    if isinstance(shard, EntityShard) and shard.world > 1:
-        _check_sharded_model(spec, shard)
+    if isinstance(shard, EntityShard):
+        _check_table(spec, shard)
         if not shard.local_storage:
-            shard = QueryShard(n, shard.rank, shard.world, shard.group)
+            shard = shard.split(n)
     if isinstance(shard, QueryShard) and shard.world > 1:
-        if shard.n != n:
-            raise ValueError("QueryShard covers %d facts, got %d" % (shard.n, n))
-        h, t, r = shard.slice(h_idx, t_idx, r_idx)
-        mine = rank_relation_prediction(spec, h, t, r, shard.csr(filt), directed, engine, chunk)
-        return tuple(shard.all_gather(list(mine)))
+        _check_queries(shard, n)
+        return tuple(_by_query_slices(shard, lambda h, t, r, f: rank_relation_prediction(
+            spec, h, t, r, f, directed, engine, chunk), (h_idx, t_idx, r_idx), filt))
     with _device_guard(dev):
         packed = None if rspec is None else engine.pack(rspec)
         keep = []
@@ -844,32 +870,25 @@ def rank_relation_prediction(spec, h_idx, t_idx, r_idx, filt, directed=True, eng
 
         # the dense RESCAL branch holds (chunk, n_rel) scores: at most 4096 facts per call
         step = min(chunk, 4096) if rspec is None else chunk
+        chunks = [(lo, min(n, lo + step)) for lo in range(0, n, step)]
         if shard is None or shard.world == 1:
             counters = torch.zeros((2, n), dtype=torch.int32, device=dev)
-            for lo in range(0, n, step):
-                hi = min(n, lo + step)
+            for (lo, hi), f in zip(chunks, _csr_cut(filt, chunks)):
                 h, t, r = h_idx[lo:hi], t_idx[lo:hi], r_idx[lo:hi].contiguous()
-                f = None if filt is None else _csr_slice(filt, lo, hi, n)
                 rank_rows(engine.gather_rows(spec, h), engine.gather_rows(spec, t), r, f,
                           counters[0][lo:hi], counters[1][lo:hi])
             ranks, filt_ranks = engine.finalize(counters[0], counters[1])
             del keep
             return ranks, filt_ranks
-        # EntityShard with local storage: the rows of every fact are exchanged, the facts are split
-        ranks = torch.empty(n, dtype=torch.int64, device=dev)
-        filt_ranks = torch.empty(n, dtype=torch.int64, device=dev)
-        for lo in range(0, n, step):
-            hi = min(n, lo + step)
-            m = hi - lo
-            rows = _exchanged_rows(spec, torch.cat([h_idx[lo:hi], t_idx[lo:hi]]), shard, engine)
-            part = QueryShard(m, shard.rank, shard.world, shard.group)
-            a, b = part.lo, part.hi
-            counters = torch.zeros((2, b - a), dtype=torch.int32, device=dev)
-            if b > a:          # a rank with no facts in this chunk still joins the all-gather
-                f = None if filt is None else _csr_slice(filt, lo + a, lo + b, n)
-                rank_rows(rows[a:b], rows[m + a:m + b], r_idx[lo + a:lo + b].contiguous(), f,
-                          counters[0], counters[1])
-            ranks[lo:hi], filt_ranks[lo:hi] = part.all_gather(list(engine.finalize(counters[0], counters[1])))
+
+        def run(lo, hi, hrows, trows, f):
+            counters = torch.zeros((2, hi - lo), dtype=torch.int32, device=dev)
+            if hi > lo:        # a rank with no facts in this chunk still joins the all-gather
+                rank_rows(hrows, trows, r_idx[lo:hi].contiguous(), f, counters[0], counters[1])
+            return engine.finalize(counters[0], counters[1])
+
+        out = [torch.empty(n, dtype=torch.int64, device=dev) for _ in range(2)]
+        ranks, filt_ranks = _exchanged_chunks(spec, shard, engine, h_idx, t_idx, chunks, filt, run, out)
         del keep
         return ranks, filt_ranks
 
@@ -882,7 +901,7 @@ def score_triples_entity_sharded(spec, h_idx, t_idx, r_idx, shard, engine=None, 
     t = b + i: the kernel reads the same bits as on the whole table, so every rank gets the scores of
     ``model.scoring_function``, bit for bit."""
     engine = engine or default_engine()
-    _check_sharded_model(spec, shard)
+    _check_table(spec, shard)
     n = h_idx.shape[0]
     dev = spec.ent0.device
     out = torch.empty(n, dtype=torch.float32, device=dev)
@@ -904,22 +923,25 @@ TOPK_CHUNK = 16384
 TOPK_MAX_K = 1024          # csrc/kernels.h
 
 
+def _check_k(k, n_cand):
+    from .exceptions import WrongArgumentsError
+    if k > n_cand:
+        raise WrongArgumentsError("top_k = %d exceeds the %d candidates" % (k, n_cand))
+
+
+def _on(csr, device):
+    return None if csr is None else tuple(x.to(device) for x in csr)
+
+
 def _topk_chunks(n, n_cand, k, topk_chunk, mask_csr, device, chunk):
     """Runs topk_chunk(lo, hi, mask) -> (pred, vals) over chunks of queries; ``mask_csr`` is a host
     CSR over all n queries, each chunk gets its rows (offsets rebased) on the device."""
-    if k > n_cand:
-        from .exceptions import WrongArgumentsError
-        raise WrongArgumentsError("top_k = %d exceeds the %d candidates" % (k, n_cand))
+    _check_k(k, n_cand)
     pred = torch.empty((n, k), dtype=torch.int64, device=device)
     vals = torch.empty((n, k), dtype=torch.float32, device=device)
-    for lo in range(0, n, chunk):
-        hi = min(n, lo + chunk)
-        mask = None
-        if mask_csr is not None:
-            offs, ids = mask_csr
-            a, b = int(offs[lo]), int(offs[hi])
-            mask = ((offs[lo:hi + 1] - a).to(device), ids[a:b].to(device))
-        pred[lo:hi], vals[lo:hi] = topk_chunk(lo, hi, mask)
+    chunks = [(lo, min(n, lo + chunk)) for lo in range(0, n, chunk)]
+    for (lo, hi), mask in zip(chunks, _csr_cut(mask_csr, chunks)):
+        pred[lo:hi], vals[lo:hi] = topk_chunk(lo, hi, _on(mask, device))
     return pred, vals
 
 
@@ -937,21 +959,9 @@ def _pair_unpack(t):
 def _check_sharded_k(k, n_cand):
     """Argument errors of a sharded call, raised on every rank before the first collective (a rank
     with nothing to compute must not wait in a collective that the others never reach)."""
-    if k > n_cand:
-        from .exceptions import WrongArgumentsError
-        raise WrongArgumentsError("top_k = %d exceeds the %d candidates" % (k, n_cand))
+    _check_k(k, n_cand)
     if not 1 <= k <= TOPK_MAX_K:
         raise _lib.KgeLibraryError("top-k inference: k must be in [1, %d]" % TOPK_MAX_K)
-
-
-def _by_query_slices(shard, n, mask, run, *idx):
-    """QueryShard: ``run(*local idx, local mask)`` on this rank's slice of the n queries, then one
-    all-gather of the (n_local, k) results."""
-    if shard.n != n:
-        raise ValueError("QueryShard covers %d queries, got %d" % (shard.n, n))
-    pred, vals = run(*shard.slice(*idx), shard.csr(mask))
-    full, = shard.all_gather([_pair_pack(pred, vals)])
-    return _pair_unpack(full)
 
 
 def _exchanged_rows(spec, idx, shard, engine):
@@ -962,6 +972,23 @@ def _exchanged_rows(spec, idx, shard, engine):
     else:                  # an empty shard (n_ent < world) has no table to read
         rows = torch.zeros((idx.shape[0], spec.cand_planes, spec.dim), dtype=torch.float32, device=idx.device)
     return shard.all_reduce_sum(rows)
+
+
+def _exchanged_chunks(spec, shard, engine, e1, e2, chunks, csr, run, out):
+    """Facts or queries (e1[i], ?, e2[i]) under an EntityShard, for tasks whose candidates every rank
+    holds, chunk by chunk: the rows of the chunk's e1 and e2 are exchanged by one all-reduce, this rank
+    runs its part [lo, hi) of the chunk (as ``shard.split`` splits it) -- ``run(lo, hi, rows1, rows2,
+    csr rows)`` -> (hi - lo, ...) results, as many as ``out`` has tensors -- and ONE all-gather brings
+    every rank the chunk's results, written into ``out``."""
+    parts = [shard.split(hi - lo) for lo, hi in chunks]
+    mine = [(lo + p.lo, lo + p.hi) for (lo, _), p in zip(chunks, parts)]
+    for (lo, hi), part, (a, b), f in zip(chunks, parts, mine, _csr_cut(csr, mine)):
+        m = hi - lo
+        rows = _exchanged_rows(spec, torch.cat([e1[lo:hi], e2[lo:hi]]), shard, engine)
+        full = part.all_gather(list(run(a, b, rows[part.lo:part.hi], rows[m + part.lo:m + part.hi], f)))
+        for o, x in zip(out, full):
+            o[lo:hi] = x
+    return out
 
 
 def topk_entity_inference(spec, ents, rels, side, k, mask=None, shard=None, engine=None, chunk=TOPK_CHUNK):
@@ -983,10 +1010,15 @@ def topk_entity_inference(spec, ents, rels, side, k, mask=None, shard=None, engi
     engine = engine or default_engine()
     n = ents.shape[0]
     dev = spec.ent0.device
-    if isinstance(shard, QueryShard) and shard.world > 1:
+    if shard is not None and shard.world > 1:
         _check_sharded_k(k, spec.n_ent)
-        return _by_query_slices(shard, n, mask, lambda e, r, m: topk_entity_inference(
-            spec, e, r, side, k, m, engine=engine, chunk=chunk), ents, rels)
+    if isinstance(shard, EntityShard):
+        _check_table(spec, shard)
+    if isinstance(shard, QueryShard) and shard.world > 1:
+        _check_queries(shard, n)
+        full, = _by_query_slices(shard, lambda e, r, m: [_pair_pack(*topk_entity_inference(
+            spec, e, r, side, k, m, engine=engine, chunk=chunk))], (ents, rels), mask)
+        return _pair_unpack(full)
     with _device_guard(dev):
         if shard is None or shard.world == 1:
             packed = engine.pack(spec)
@@ -996,10 +1028,7 @@ def topk_entity_inference(spec, ents, rels, side, k, mask=None, shard=None, engi
                 return engine.topk_side(spec, packed, side, rows, rows, rels[lo:hi].contiguous(), k, m)
 
             return _topk_chunks(n, spec.n_rows, k, topk_chunk, mask, dev, chunk)
-        # EntityShard
-        _check_sharded_k(k, spec.n_ent)
-        if (spec.ent_lo, spec.n_rows) != (shard.lo, shard.hi - shard.lo):
-            spec = spec.narrowed(shard.lo, shard.hi)
+        spec = _scanned(spec, shard)
         k_loc = min(k, spec.n_rows)
         packed = engine.pack(spec) if k_loc > 0 else None
 
@@ -1029,8 +1058,10 @@ def topk_relation_inference(spec, e1, e2, k, mask=None, shard=None, engine=None,
     dev = spec.ent0.device
     if isinstance(shard, QueryShard) and shard.world > 1:
         _check_sharded_k(k, spec.n_rel)
-        return _by_query_slices(shard, n, mask, lambda a, b, m: topk_relation_inference(
-            spec, a, b, k, m, engine=engine, chunk=chunk), e1, e2)
+        _check_queries(shard, n)
+        full, = _by_query_slices(shard, lambda a, b, m: [_pair_pack(*topk_relation_inference(
+            spec, a, b, k, m, engine=engine, chunk=chunk))], (e1, e2), mask)
+        return _pair_unpack(full)
     if spec.code == _lib.RESCAL:
         # candidates are relation matrices: dense (n, n_rel) scores, then the same selection kernels
         rspec, packed, n_cand = None, None, spec.n_rel
@@ -1045,27 +1076,23 @@ def topk_relation_inference(spec, e1, e2, k, mask=None, shard=None, engine=None,
             return engine.topk_dense(scores, k, m)
         return engine.topk_side(rspec, packed, _lib.SIDE_REL, hrows, trows, None, k, m)
 
+    if isinstance(shard, EntityShard):
+        if shard.world > 1:
+            _check_sharded_k(k, n_cand)
+        _check_table(spec, shard)
     with _device_guard(dev):
         if shard is None or shard.world == 1:
             def topk_chunk(lo, hi, m):
                 return local_topk(engine.gather_rows(spec, e1[lo:hi]), engine.gather_rows(spec, e2[lo:hi]), m)
 
             return _topk_chunks(n, n_cand, k, topk_chunk, mask, dev, chunk)
-        # EntityShard: the entity table is split, the relations are not
-        _check_sharded_k(k, n_cand)
-        if (spec.ent_lo, spec.n_rows) != (shard.lo, shard.hi - shard.lo):
-            spec = spec.narrowed(shard.lo, shard.hi)
 
-        def topk_chunk(lo, hi, m):
-            rows = _exchanged_rows(spec, torch.cat([e1[lo:hi], e2[lo:hi]]), shard, engine)
-            part = QueryShard(hi - lo, shard.rank, shard.world, shard.group)
-            a, b = part.lo, part.hi
-            if b > a:
-                pred, vals = local_topk(rows[a:b], rows[hi - lo + a:hi - lo + b], part.csr(m))
-            else:
-                pred = torch.empty((0, k), dtype=torch.int64, device=dev)
-                vals = torch.empty((0, k), dtype=torch.float32, device=dev)
-            full, = part.all_gather([_pair_pack(pred, vals)])
-            return _pair_unpack(full)
+        def run(lo, hi, rows1, rows2, m):
+            if hi > lo:
+                return [_pair_pack(*local_topk(rows1, rows2, _on(m, dev)))]
+            return [torch.empty((0, 2, k), dtype=torch.int64, device=dev)]
 
-        return _topk_chunks(n, n_cand, k, topk_chunk, mask, dev, chunk)
+        chunks = [(lo, min(n, lo + chunk)) for lo in range(0, n, chunk)]
+        full, = _exchanged_chunks(_scanned(spec, shard), shard, engine, e1, e2, chunks, mask, run,
+                                  [torch.empty((n, 2, k), dtype=torch.int64, device=dev)])
+        return _pair_unpack(full)

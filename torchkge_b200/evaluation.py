@@ -3,12 +3,15 @@ methods (torchkge/evaluation.py:207-425).  ``evaluate`` hands the whole job -- s
 entity as head and as tail of every fact, discounting the filter sets, ranking -- to the
 CUDA engine; no (batch, n_entities) score matrix exists at any point.
 """
+from types import SimpleNamespace
+
 import torch
 
 from . import _lib
 from .data import dict_filter_csr, filter_csr
-from .engine import (DEFAULT_CHUNK, EntityShard, ModelSpec, QueryShard, _check_sharded_model, default_engine,
-                     rank_link_prediction, rank_relation_prediction, score_triples_entity_sharded)
+from .engine import (DEFAULT_CHUNK, EntityShard, ModelSpec, QueryShard, _by_query_slices, _check_table,
+                     default_engine, rank_link_prediction, rank_relation_prediction, score_triples_entity_sharded,
+                     shard_spec)
 from .exceptions import NotYetEvaluatedError
 
 
@@ -66,20 +69,14 @@ class LinkPredictionEvaluator(object):
         """
         if b_size is None or int(b_size) < 1:
             raise ValueError("b_size must be a positive integer")
-        spec = ModelSpec.from_model(self.model)
+        kg = self.kg
+        spec = shard_spec(self.model, self.shard, "LinkPredictionEvaluator.evaluate", n=kg.n_facts)
         qshard = self.shard if isinstance(self.shard, QueryShard) else None
         eshard = None if qshard is not None else self.shard
-        if eshard is not None and eshard.local_storage:
-            spec.ent_lo, spec.n_ent = eshard.lo, eshard.n_ent
-        if not spec.ent0.is_cuda:
-            raise _lib.KgeLibraryError(
-                "LinkPredictionEvaluator.evaluate needs the model on a CUDA device "
-                "(model.cuda()); this package has no CPU execution path")
         dev = spec.ent0.device
-        kg = self.kg
         heads, tails, rels = kg.head_idx, kg.tail_idx, kg.relations
         if qshard is not None:      # this rank's contiguous slice of the facts
-            heads, tails, rels = (x[qshard.lo:qshard.hi] for x in (heads, tails, rels))
+            heads, tails, rels = qshard.slice(heads, tails, rels)
         n_here = int(heads.shape[0])
         _check_index_range(heads, tails, rels, spec.n_ent, spec.n_rel)
         h_d = heads.to(dev, non_blocking=True)
@@ -237,15 +234,7 @@ class RelationPredictionEvaluator(object):
         ``LinkPredictionEvaluator.evaluate``).  Under a shard, every rank of its group calls this."""
         if b_size is None or int(b_size) < 1:
             raise ValueError("b_size must be a positive integer")
-        spec = ModelSpec.from_model(self.model)
-        if isinstance(self.shard, EntityShard) and self.shard.local_storage:
-            spec.ent_lo, spec.n_ent = self.shard.lo, self.shard.n_ent
-        if not spec.ent0.is_cuda:
-            raise _lib.KgeLibraryError(
-                "RelationPredictionEvaluator.evaluate needs the model on a CUDA device "
-                "(model.cuda()); this package has no CPU execution path")
-        if isinstance(self.shard, EntityShard) and self.shard.world > 1:
-            _check_sharded_model(spec, self.shard)     # a wrong table says so before the index check
+        spec = shard_spec(self.model, self.shard, "RelationPredictionEvaluator.evaluate")
         dev = spec.ent0.device
         kg = self.kg
         _check_index_range(kg.head_idx, kg.tail_idx, kg.relations, spec.n_ent, spec.n_rel)
@@ -331,31 +320,31 @@ class TripletClassificationEvaluator(object):
         self.sampler = PositionalNegativeSampler(self.kg_val, kg_test=self.kg_test)
 
     def _sharded(self):
-        """The shard when it splits anything; its argument errors are raised here, on every rank,
-        before any collective."""
+        """(shard, spec) when the shard splits anything, else (None, None); its argument errors are raised
+        here, on every rank, before any collective.  ``spec``: under an EntityShard, the tables the
+        per-triple kernel reads (_scoring_spec)."""
         shard = self.shard
         if shard is None or shard.world == 1:
-            return None
-        if isinstance(shard, EntityShard):
-            held = shard.hi - shard.lo if shard.local_storage else shard.n_ent
-            if self.model.n_ent != held:
-                raise ValueError("EntityShard(local_storage=%s): rank %d should hold %d entity rows, the model "
-                                 "has %d" % (shard.local_storage, shard.rank, held, self.model.n_ent))
-            if shard.local_storage:
-                from .training import _training_code
-                _training_code(self.model)        # kinds the per-triple kernel does not score raise here
-        return shard
+            return None, None
+        spec = None
+        if isinstance(shard, EntityShard) and shard.local_storage:
+            spec = shard_spec(self.model, shard, "TripletClassificationEvaluator", build=self._scoring_spec)
+        elif isinstance(shard, EntityShard):
+            # the slices are scored by model.scoring_function, which takes kinds the kernel does not
+            _check_table(SimpleNamespace(n_ent=self.model.n_ent, ent_lo=0, n_rows=self.model.n_ent), shard)
+        return shard, spec
 
-    def _scoring_spec(self):
+    @staticmethod
+    def _scoring_spec(model):
         """ModelSpec over the tables ``model.scoring_function`` hands the per-triple kernel
         (training._param_tensors): RotatE's (cos, sin) planes, TorusE's tables as they are (the kernel
-        takes fractional parts), Analogy's planes stacked."""
+        takes fractional parts), Analogy's planes stacked.  Kinds the kernel does not score raise here."""
         from .training import _kernel_dim, _param_tensors, _training_code
-        code = _training_code(self.model)
+        code = _training_code(model)
         with torch.no_grad():
-            e0, e1, r0, r1 = (None if x is None else x.detach() for x in _param_tensors(self.model, code))
-        dim = _kernel_dim(self.model, code)
-        n_ent, n_rel = self.model.n_ent, self.model.n_rel
+            e0, e1, r0, r1 = (None if x is None else x.detach() for x in _param_tensors(model, code))
+        dim = _kernel_dim(model, code)
+        n_ent, n_rel = model.n_ent, model.n_rel
         if code == _lib.ANALOGY:         # stacked (3, n, dim) copies: equally spaced planes
             return ModelSpec(code, dim, n_ent, n_rel, e0[0], e0[1], r0[0], r0[1], ent2=e0[2], rel2=r0[2])
         return ModelSpec(code, dim, n_ent, n_rel, e0, e1, r0, r1)
@@ -373,26 +362,24 @@ class TripletClassificationEvaluator(object):
 
     def get_scores(self, heads, tails, relations, batch_size):
         """Scores of the given triplets, computed batch by batch (evaluation.py:478-511)."""
+        shard, spec = self._sharded()
         if not self.is_cuda:
             raise _lib.KgeLibraryError("TripletClassificationEvaluator needs the model on a CUDA device")
         dev = next(self.model.parameters()).device
-        shard = self._sharded()
         if shard is None:
             return self._scores_here(heads, tails, relations, batch_size, dev)
         if isinstance(shard, EntityShard) and shard.local_storage:
-            spec = self._scoring_spec()
-            spec.ent_lo, spec.n_ent = shard.lo, shard.n_ent
             h, t, r = (x.to(dev, torch.int64) for x in (heads, tails, relations))
             return score_triples_entity_sharded(spec, h, t, r, shard, default_engine(), batch_size)
-        part = QueryShard(heads.shape[0], shard.rank, shard.world, shard.group)
-        mine = self._scores_here(*part.slice(heads, tails, relations), batch_size, dev)
-        return part.all_gather([mine])[0]
+        # split by this vector's length, not by a QueryShard's own n
+        return _by_query_slices(shard.split(heads.shape[0]), lambda h, t, r, _: [
+            self._scores_here(h, t, r, batch_size, dev)], (heads, tails, relations))[0]
 
     def _negatives(self, b_size, which):
         """``sampler.corrupt_kg``; under a shard, rank 0's draws on every rank (the other ranks add
         zeros into one sum-all-reduce)."""
         nh, nt = self.sampler.corrupt_kg(b_size, self.is_cuda, which=which)
-        shard = self._sharded()
+        shard, _ = self._sharded()
         if shard is None:
             return nh, nt
         both = torch.stack([nh, nt]).to(next(self.model.parameters()).device, torch.int64)

@@ -22,8 +22,7 @@ IndexError for every usual argument.  Here ``scores[i]`` holds the scores of ``p
 import torch
 
 from . import _lib
-from .engine import (TOPK_CHUNK, EntityShard, ModelSpec, default_engine, topk_entity_inference,
-                     topk_relation_inference)
+from .engine import TOPK_CHUNK, default_engine, shard_spec, topk_entity_inference, topk_relation_inference
 from .exceptions import WrongArgumentsError
 
 #: queries per top-k call
@@ -41,17 +40,6 @@ def _mask_csr(dictionary, key1, key2):
             ids.extend(sorted(s))
         offs.append(len(ids))
     return torch.tensor(offs, dtype=torch.int64), torch.tensor(ids, dtype=torch.int64)
-
-
-def _cuda_spec(model, shard, who):
-    spec = ModelSpec.from_model(model)
-    if isinstance(shard, EntityShard) and shard.local_storage:
-        # the model holds only this rank's rows: its row 0 is entity shard.lo
-        spec.ent_lo, spec.n_ent = shard.lo, shard.n_ent
-    if not spec.ent0.is_cuda:
-        raise _lib.KgeLibraryError("%s.evaluate needs the model on a CUDA device; "
-                                   "this package has no CPU execution path" % who)
-    return spec
 
 
 class EntityInference(object):
@@ -93,7 +81,7 @@ class EntityInference(object):
 
     def evaluate(self, b_size, verbose=True):
         """``b_size`` / ``verbose``: accepted for signature compatibility (chunking is by memory)."""
-        spec = _cuda_spec(self.model, self.shard, "EntityInference")
+        spec = shard_spec(self.model, self.shard, "EntityInference.evaluate")
         dev = spec.ent0.device
         ents = self.known_entities.long().to(dev)
         rels = self.known_relations.long().to(dev)
@@ -130,7 +118,7 @@ class RelationInference(object):
         self.scores = torch.empty(size=(len(entities2), top_k))
 
     def evaluate(self, b_size, verbose=True):
-        spec = _cuda_spec(self.model, self.shard, "RelationInference")
+        spec = shard_spec(self.model, self.shard, "RelationInference.evaluate")
         dev = spec.ent0.device
         e1, e2 = self.entities1.long().to(dev), self.entities2.long().to(dev)
         mask = None

@@ -10,8 +10,8 @@ import struct
 import torch
 
 from . import _lib
-from .engine import (EntityShard, ModelSpec, QueryShard, _device_guard, _exchanged_rows, _plane_ptrs, _ptr,
-                     _stream, default_engine)
+from .engine import (EntityShard, ModelSpec, QueryShard, _check_table, _device_guard, _exchanged_rows, _plane_ptrs,
+                     _ptr, _stream, default_engine)
 
 
 def _param_tensors(model, code):
@@ -375,13 +375,11 @@ def sharded_margin_step(model, heads, tails, relations, margin, n_neg, bern_prob
         raise ValueError("bern_probs must be given (a sharded step draws its own negatives)")
     code = _training_code(model)
     ent0, ent1, rel0, rel1 = _param_tensors(model, code)
-    held = int(ent0.shape[-2])
-    if held != shard.hi - shard.lo or int(model.n_ent) != held:
-        raise ValueError("the model holds %d entity rows, the shard's range [%d, %d) has %d"
-                         % (held, shard.lo, shard.hi, shard.hi - shard.lo))
     b = int(heads.shape[0])
-    step = ShardedStep(code, _kernel_dim(model, code), shard.n_ent, shard.lo, held, int(n_neg), float(margin),
-                       int(seed) & 0xFFFFFFFFFFFFFFFF, int(offset) & 0xFFFFFFFFFFFFFFFF, int(loss_kind))
+    step = ShardedStep(code, _kernel_dim(model, code), shard.n_ent, shard.lo, int(ent0.shape[-2]), int(n_neg),
+                       float(margin), int(seed) & 0xFFFFFFFFFFFFFFFF, int(offset) & 0xFFFFFFFFFFFFFFFF,
+                       int(loss_kind))
+    _check_table(step, shard)
     # one small collective: every rank must draw the same negatives for the same batch and loss
     mine = torch.tensor([_signed64(step.seed), _signed64(step.offset), b, step.n_neg,
                          struct.unpack("<q", struct.pack("<d", step.margin))[0], step.loss_kind],
