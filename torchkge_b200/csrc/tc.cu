@@ -46,7 +46,10 @@ constexpr int PRODUCER_REGS = 40, CONSUMER_REGS = 232;
 constexpr int ACC = BN / 2;          // fp32 accumulator registers per thread (m64n256)
 constexpr int MAX_STAGES = 4;
 constexpr int BAR_SLOTS = 32;        // full[4] empty[4] a_full[8] a_empty[1] ...
-constexpr size_t SMEM_TAIL = BAR_SLOTS * sizeof(uint64_t) + MMA_WARPS * AMB_BUF * sizeof(int2);
+constexpr int BLOCKS = TC_BN / 32;   // 32-column blocks of a candidate tile
+// barriers, near-tie buffers, and (T_hi, T_lo) of both rows of each lane quad for each block
+constexpr size_t SMEM_TAIL = BAR_SLOTS * sizeof(uint64_t) + MMA_WARPS * AMB_BUF * sizeof(int2) +
+                             MMA_WARPS * BLOCKS * 8 * sizeof(float4);
 constexpr size_t SMEM_LIMIT = 232448;  // 227 KB opt-in maximum per CTA on sm_90
 
 // Geometry of one kernel variant: BKT half-precision values per k-block (= one swizzle span of
@@ -170,6 +173,24 @@ __device__ __forceinline__ void wgmma_fp16(float (&d)[128], uint64_t desc_a, uin
       : "memory");
 }
 
+// Threshold tests as one FSET each: the bits of 1.0f (0x3F800000) when the test passes, else 0.
+// (ptxas lowers an integer-valued set to FSETP + SEL, two instructions.)  A sum of n such words is
+// n * 127 * 2^23 (mod 2^32): equal sums mean equal counts for n < 512, and ones_count() recovers n.
+// a > b (false when either is NaN)
+__device__ __forceinline__ uint32_t one_if_gt(float a, float b) {
+  float r;
+  asm("set.gt.f32.f32 %0, %1, %2;" : "=f"(r) : "f"(a), "f"(b));
+  return __float_as_uint(r);
+}
+// a >= b or unordered (true when either is NaN)
+__device__ __forceinline__ uint32_t one_if_geu(float a, float b) {
+  float r;
+  asm("set.geu.f32.f32 %0, %1, %2;" : "=f"(r) : "f"(a), "f"(b));
+  return __float_as_uint(r);
+}
+// n from the sum of n words 0x3F800000, n < 512: 127 is odd and 383 * 127 = 1 (mod 512)
+__device__ __forceinline__ int ones_count(uint32_t sum) { return (int)(((sum >> 23) * 383u) & 511u); }
+
 
 // Work order: a unit = (group of p.ct_group consecutive candidate tiles, query tile); a CTA
 // takes units round-robin and walks the group's candidate tiles for that query tile.  CTAs
@@ -259,6 +280,7 @@ __global__ void __launch_bounds__(THREADS, 1) tc_scan_kernel(const __grid_consta
   uint64_t* afull_bar = bars + 8;        // [8]  one per resident A k-block
   uint64_t* aempty_bar = bars + 16;      // [1]  resident A region free again (one arrival per consumer warp)
   int2* s_amb = reinterpret_cast<int2*>(bars + BAR_SLOTS);  // [MMA_WARPS][AMB_BUF]
+  float4* s_thr = reinterpret_cast<float4*>(s_amb + MMA_WARPS * AMB_BUF);   // [MMA_WARPS][BLOCKS][8 quads]
 
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
   const Units units(p.n_qt, p.n_ct, p.ct_group);
@@ -335,6 +357,7 @@ __global__ void __launch_bounds__(THREADS, 1) tc_scan_kernel(const __grid_consta
   float k1[2] = {0.f, 0.f}, k0[2] = {0.f, 0.f}, tbase[2] = {0.f, 0.f};
   int cnt[2] = {0, 0};
   NearTies amb{s_amb + warp * AMB_BUF, 0};
+  float4* const thr = s_thr + warp * BLOCKS * 8 + (lane >> 2);   // [b * 8]: this quad's block b
   constexpr float INFL = 1.f + 0x1p-19f;      // covers the fp32 rounding of E's evaluation
   // the accumulator holds S * (a.b [- |b|^2/2]), S = scale_a * scale_b (a power of two; NaN when an
   // operand could not be represented: both threshold tests then fail and every pair is rechecked)
@@ -349,52 +372,6 @@ __global__ void __launch_bounds__(THREADS, 1) tc_scan_kernel(const __grid_consta
   for (long long u = blockIdx.x; u < units.n_units; u += gridDim.x, ++unit_no) {
    long long qt, ct_lo, ct_hi; units.decode(u, &qt, &ct_lo, &ct_hi);
    for (long long ct = ct_lo; ct < ct_hi; ++ct) {
-    // ---- MMAs: one commit group per k-block, the previous block's stage released once its group is done
-    int prev = -1;
-    fence_acc(acc);
-    for (int kb = 0; kb < n_kb; ++kb) {
-      if constexpr (RES) {
-        if (ct == ct_lo) ptx::mbar_wait(&afull_bar[kb], unit_no & 1u);
-      }
-      ptx::mbar_wait(&full_bar[stage], phase);
-      const uint32_t sb = ptx::smem_u32(stage_base + (size_t)stage * G::STAGE_BYTES);
-      const uint32_t sa = (RES ? ptx::smem_u32(a_res + (size_t)kb * G::A_BLOCK) : sb) + a_off;
-      const uint32_t sbb = RES ? sb : sb + G::A_BLOCK;
-      const uint64_t a_hi = make_desc<G>(sa), a_lo = make_desc<G>(sa + G::A_PLANE);
-      const uint64_t b_hi = make_desc<G>(sbb), b_lo = make_desc<G>(sbb + G::B_PLANE);
-      const int k16s = min(G::K16, (p.k_total - kb * BKT + 15) / 16);
-      wg_fence();
-#pragma unroll
-      for (int k = 0; k < G::K16; ++k) {
-        if (k < k16s) {
-          const uint64_t adv = (uint64_t)(k * 2);  // 16 values = 32 B = 2 x 16-B units
-          if constexpr (FP16) {
-            wgmma_fp16(acc, a_hi + adv, b_hi + adv, (kb | k) ? 1u : 0u);
-            wgmma_fp16(acc, a_lo + adv, b_hi + adv, 1u);
-            wgmma_fp16(acc, a_hi + adv, b_lo + adv, 1u);
-          } else {
-            wgmma_bf16(acc, a_hi + adv, b_hi + adv, (kb | k) ? 1u : 0u);
-            wgmma_bf16(acc, a_lo + adv, b_hi + adv, 1u);
-            wgmma_bf16(acc, a_hi + adv, b_lo + adv, 1u);
-          }
-        }
-      }
-      wg_commit();
-      wg_wait<1>();
-      if (prev >= 0 && lane == 0) ptx::mbar_arrive(&empty_bar[prev]);
-      prev = stage;
-      if (++stage == STAGES) { stage = 0; phase ^= 1u; }
-    }
-    wg_wait<0>();
-    fence_acc(acc);
-    if (lane == 0) {
-      ptx::mbar_arrive(&empty_bar[prev]);
-      if constexpr (RES) {
-        if (ct == ct_hi - 1) ptx::mbar_arrive(aempty_bar);   // every MMA of the unit has read A
-      }
-    }
-
-    // ---- epilogue ----
     const long long q0 = qt * BM + row0;
     if (qt != cur_qt) {
       if (cur_qt >= 0) {
@@ -431,64 +408,160 @@ __global__ void __launch_bounds__(THREADS, 1) tc_scan_kernel(const __grid_consta
       }
     }
     const int ncols = (int)min((long long)BN, p.n_rows - ct * BN);
+    // ---- MMAs: one commit group per k-block, the previous block's stage released once its group is done
+    int prev = -1;
+    fence_acc(acc);
+    for (int kb = 0; kb < n_kb; ++kb) {
+      if constexpr (RES) {
+        if (ct == ct_lo) ptx::mbar_wait(&afull_bar[kb], unit_no & 1u);
+      }
+      ptx::mbar_wait(&full_bar[stage], phase);
+      const uint32_t sb = ptx::smem_u32(stage_base + (size_t)stage * G::STAGE_BYTES);
+      const uint32_t sa = (RES ? ptx::smem_u32(a_res + (size_t)kb * G::A_BLOCK) : sb) + a_off;
+      const uint32_t sbb = RES ? sb : sb + G::A_BLOCK;
+      const uint64_t a_hi = make_desc<G>(sa), a_lo = make_desc<G>(sa + G::A_PLANE);
+      const uint64_t b_hi = make_desc<G>(sbb), b_lo = make_desc<G>(sbb + G::B_PLANE);
+      const int k16s = min(G::K16, (p.k_total - kb * BKT + 15) / 16);
+      wg_fence();
+#pragma unroll
+      for (int k = 0; k < G::K16; ++k) {
+        if (k < k16s) {
+          const uint64_t adv = (uint64_t)(k * 2);  // 16 values = 32 B = 2 x 16-B units
+          if constexpr (FP16) {
+            wgmma_fp16(acc, a_hi + adv, b_hi + adv, (kb | k) ? 1u : 0u);
+            wgmma_fp16(acc, a_lo + adv, b_hi + adv, 1u);
+            wgmma_fp16(acc, a_hi + adv, b_lo + adv, 1u);
+          } else {
+            wgmma_bf16(acc, a_hi + adv, b_hi + adv, (kb | k) ? 1u : 0u);
+            wgmma_bf16(acc, a_lo + adv, b_hi + adv, 1u);
+            wgmma_bf16(acc, a_hi + adv, b_lo + adv, 1u);
+          }
+        }
+      }
+      wg_commit();
+      if constexpr (!DUMP) {
+        if (kb == 0) {
+          // The tile's thresholds, while the tensor cores run the first k-block: the four lanes
+          // that share two query rows split the 8 column blocks, 2 each, and leave (T_hi, T_lo) of
+          // both rows in shared memory for the epilogue.
+          __syncwarp();   // the previous tile's epilogue has read its thresholds
+#pragma unroll
+          for (int i = 0; i < 2; ++i) {
+            const int b = 2 * (lane & 3) + i;
+            if (32 * b < ncols) {
+              // largest candidate norm bound / running-magnitude factor of the block's 32
+              // candidates (maxima over aligned blocks of 32 rows, precomputed with the image)
+              const long long blk = (ct * BN) / 32 + b;
+              const float cb = __fadd_ru(__ldg(p.cbmax32 + blk), kappa_b), cpm = __ldg(p.cpmax32 + blk);
+              float t[4];
+#pragma unroll
+              for (int h = 0; h < 2; ++h) {
+                float e;
+                if constexpr (L2) e = fmaf(cb, fmaf(p.gamma2 * INFL, cb, k1[h]), k0[h]) * INFL;
+                else e = k1[h] * cb;
+                e = __fadd_ru(__fmaf_ru(kp[h], cpm, e), e_abs);
+                float t_hi = __fadd_ru(tbase[h], e), t_lo = __fadd_rd(tbase[h], -e);
+                if constexpr (L2) { t_hi = __fmul_ru(t_hi, 0.5f); t_lo = __fmul_rd(t_lo, 0.5f); }
+                // exact (power of two) unless it overflows, then still on the safe side
+                t[2 * h] = __fmul_ru(t_hi, S);
+                t[2 * h + 1] = __fmul_rd(t_lo, S);
+              }
+              thr[b * 8] = make_float4(t[0], t[1], t[2], t[3]);
+            }
+          }
+        }
+      }
+      wg_wait<1>();
+      if (prev >= 0 && lane == 0) ptx::mbar_arrive(&empty_bar[prev]);
+      prev = stage;
+      if (++stage == STAGES) { stage = 0; phase ^= 1u; }
+    }
+    wg_wait<0>();
+    fence_acc(acc);
+    if (lane == 0) {
+      ptx::mbar_arrive(&empty_bar[prev]);
+      if constexpr (RES) {
+        if (ct == ct_hi - 1) ptx::mbar_arrive(aempty_bar);   // every MMA of the unit has read A
+      }
+    }
+
+    // ---- epilogue ----
+    __syncwarp();   // this tile's thresholds are in shared memory
+    uint32_t ones_gt[2] = {0u, 0u};   // per row: the hot path's "count" results of the tile (<= 64)
 #pragma unroll
     for (int b = 0; b < BN / 32; ++b) {
       const int c0 = 32 * b;
       if (c0 >= ncols) break;
-      // largest candidate norm bound / running-magnitude factor of the block's 32 candidates
-      // (maxima over aligned blocks of 32 rows, precomputed with the image)
-      const long long blk = (ct * BN) / 32 + b;
-      const float cb = __fadd_ru(__ldg(p.cbmax32 + blk), kappa_b), cpm = __ldg(p.cpmax32 + blk);
       float t_hi[2], t_lo[2];
-#pragma unroll
-      for (int h = 0; h < 2; ++h) {
-        float e;
-        if constexpr (L2) e = fmaf(cb, fmaf(p.gamma2 * INFL, cb, k1[h]), k0[h]) * INFL;
-        else e = k1[h] * cb;
-        e = __fadd_ru(__fmaf_ru(kp[h], cpm, e), e_abs);
-        t_hi[h] = __fadd_ru(tbase[h], e);
-        t_lo[h] = __fadd_rd(tbase[h], -e);
-        if constexpr (L2) { t_hi[h] = __fmul_ru(t_hi[h], 0.5f); t_lo[h] = __fmul_rd(t_lo[h], 0.5f); }
-        t_hi[h] = __fmul_ru(t_hi[h], S);   // exact (power of two) unless it overflows, then still on the safe side
-        t_lo[h] = __fmul_rd(t_lo[h], S);
+      if constexpr (!DUMP) {
+        const float4 t = thr[b * 8];
+        t_hi[0] = t.x; t_lo[0] = t.y; t_hi[1] = t.z; t_lo[1] = t.w;
       }
-      // 16 independent threshold tests -> two bit masks per thread (no per-element branches)
-      // (NaN / inf anywhere -- accumulator, thresholds, norm bounds -- fails both tests and lands
-      // in the near-tie list, i.e. is adjudicated by the exact arithmetic)
-      unsigned lt_mask = 0, gt_mask = 0;
+      // Each of the thread's 16 values gets two tests: f > T_hi ("count") and f >= T_lo or
+      // unordered ("not below"); a pair is a near-tie when it passes the second test only.  (A NaN
+      // accumulator or threshold -- what a NaN or inf operand, norm bound or scale leads to -- fails
+      // the first test and passes the second: it lands in the near-tie list, i.e. is adjudicated by
+      // the exact arithmetic.)
+      if constexpr (DUMP) {
 #pragma unroll
-      for (int e = 0; e < 16; ++e) {
-        const float f = acc[16 * b + e];
-        const int h = (e >> 1) & 1;
-        if constexpr (DUMP) {
+        for (int e = 0; e < 16; ++e) {
+          const float f = acc[16 * b + e];
+          const int h = (e >> 1) & 1;
           const long long q = q0 + 8 * h;
           const int c = c0 + 8 * (e >> 2) + cq + (e & 1);
           if (c < ncols && q < p.n_q)
             p.dump[(size_t)q * p.n_rows + ct * BN + c] = L2 ? fmaf(2.f, f * inv_S, -qn[h]) : f * inv_S;
-        } else {
-          gt_mask |= (f > t_hi[h] ? 1u : 0u) << e;
-          lt_mask |= (f < t_lo[h] ? 1u : 0u) << e;
         }
-      }
-      if constexpr (!DUMP) {
-        unsigned amb_mask = ~(gt_mask | lt_mask) & 0xFFFFu;
-        if (c0 + 32 > ncols) {  // columns past the table (last tile only)
-          unsigned keep = 0u;
+      } else {
+        // Hot path: no bit masks, only sums of the test results -- per row for "count", over both
+        // rows for "not below".  T_hi >= T_lo whenever neither is NaN (directed rounding of
+        // tbase +- e, e >= 0), and a NaN threshold makes one test uniform over the row, so a value
+        // that passes "count" also passes "not below": the two sums differ exactly when the
+        // thread has a near-tie in the block.
+        uint32_t s_gt0 = 0u, s_gt1 = 0u, s_ge = 0u;
 #pragma unroll
-          for (int e = 0; e < 16; ++e)
-            if (c0 + 8 * (e >> 2) + cq + (e & 1) < ncols) keep |= 1u << e;
-          amb_mask &= keep; gt_mask &= keep;
+        for (int e = 0; e < 16; ++e) {
+          const float f = acc[16 * b + e];
+          const int h = (e >> 1) & 1;
+          if (h == 0) s_gt0 += one_if_gt(f, t_hi[0]);
+          else s_gt1 += one_if_gt(f, t_hi[1]);
+          s_ge += one_if_geu(f, t_lo[h]);
         }
-        // padding rows of the last query tile have no list entries (their thresholds are +inf,
-        // but a non-finite candidate norm bound turns them into NaN, which fails both tests)
-        if (q0 >= p.n_q) amb_mask &= 0xCCCCu;
-        if (q0 + 8 >= p.n_q) amb_mask &= 0x3333u;
-        cnt[0] += __popc(gt_mask & 0x3333u);
-        cnt[1] += __popc(gt_mask & 0xCCCCu);
-        if (__any_sync(0xffffffffu, amb_mask != 0))
+        ones_gt[0] += s_gt0;
+        ones_gt[1] += s_gt1;
+        const bool edge = c0 + 32 > ncols;   // columns past the table (last tile only)
+        // Cold path (blocks with a near-tie, and partial blocks): the same tests as bit masks
+        if (__any_sync(0xffffffffu, edge || s_ge != s_gt0 + s_gt1)) {
+          unsigned lt_mask = 0, gt_mask = 0;
+#pragma unroll
+          for (int e = 0; e < 16; ++e) {
+            const float f = acc[16 * b + e];
+            const int h = (e >> 1) & 1;
+            gt_mask |= (f > t_hi[h] ? 1u : 0u) << e;
+            lt_mask |= (f < t_lo[h] ? 1u : 0u) << e;
+          }
+          unsigned amb_mask = ~(gt_mask | lt_mask) & 0xFFFFu;
+          if (edge) {
+            unsigned keep = 0u;
+#pragma unroll
+            for (int e = 0; e < 16; ++e)
+              if (c0 + 8 * (e >> 2) + cq + (e & 1) < ncols) keep |= 1u << e;
+            amb_mask &= keep;
+            // the sums above also counted the columns past the table
+            const unsigned past = gt_mask & ~keep;
+            cnt[0] -= __popc(past & 0x3333u);
+            cnt[1] -= __popc(past & 0xCCCCu);
+          }
+          // padding rows of the last query tile have no list entries (their thresholds are +inf,
+          // but a non-finite candidate norm bound turns them into NaN, which fails both tests)
+          if (q0 >= p.n_q) amb_mask &= 0xCCCCu;
+          if (q0 + 8 >= p.n_q) amb_mask &= 0x3333u;
           amb.append(p, qt, lane, amb_mask, q0, ct * BN + c0 + cq);
+        }
       }
     }
+    cnt[0] += ones_count(ones_gt[0]);
+    cnt[1] += ones_count(ones_gt[1]);
    }
   }
   if (cur_qt >= 0) {
