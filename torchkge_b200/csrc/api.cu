@@ -2,6 +2,7 @@
 #include <mutex>
 #include <map>
 #include <memory>
+#include <optional>
 #include <stdio.h>
 #include <string.h>
 #include <vector>
@@ -18,6 +19,12 @@ thread_local char g_err[512] = "";
 
 int fail(int code, const char* msg) {
   snprintf(g_err, sizeof(g_err), "%s", msg);
+  return code;
+}
+
+// "fn: what", the form of every argument error of the entry points
+int fail(int code, const char* fn, const char* what) {
+  snprintf(g_err, sizeof(g_err), "%s: %s", fn, what);
   return code;
 }
 
@@ -78,7 +85,20 @@ const HostSchedule* get_schedule(int model, int dim) {
 
 size_t align_up(size_t x, size_t a) { return (x + a - 1) / a * a; }
 
-// Workspace carve-up shared by kge_rank_side and kge_score_all.
+// Bump allocator over a caller's workspace: 256-byte aligned pieces from `off` on; base = nullptr
+// only sizes them.
+struct Carver {
+  void* base;
+  size_t off = 0;
+  template <class T>
+  T* take(size_t bytes) {
+    void* p = base ? static_cast<char*>(base) + off : nullptr;
+    off += align_up(bytes, 256);
+    return static_cast<T*>(p);
+  }
+};
+
+// Workspace carve-up shared by kge_rank_side, kge_filter_side, kge_score_all and kge_topk_side.
 struct Workspace {
   float* qplain;
   float* qpacked;
@@ -86,14 +106,15 @@ struct Workspace {
   int32_t* perm;
   uint8_t* code;
   // tensor-core path
-  unsigned char* apack;
-  float* qbound;
-  float* qnorm2;
-  float* qprefix;
-  kge::tc::TcMeta* meta_a;
-  unsigned long long* amb_count;
-  int2* amb_pairs;
-  unsigned long long amb_cap;
+  unsigned char* apack = nullptr;
+  float* qbound = nullptr;
+  float* qnorm2 = nullptr;
+  float* qprefix = nullptr;
+  kge::tc::TcMeta* meta_a = nullptr;
+  // near-tie list (tensor-core and approximate scans)
+  unsigned long long* amb_count = nullptr;
+  int2* amb_pairs = nullptr;
+  unsigned long long amb_cap = 0;
   size_t bytes;
 };
 
@@ -102,8 +123,6 @@ bool tc_supported(int el) {
          el == kge::EL_L2_HEAD;
 }
 bool tc_is_l2(int el) { return el == kge::EL_L2_TAIL || el == kge::EL_L2_HEAD; }
-// contraction length of the operand images: all planes for ComplEx / Analogy; L2 carries the candidate's
-// squared norm in three extra k slots (tc.h: launch_pack_b)
 // bound-and-refine on the fp32 pipes (approximate element arithmetic + exact recheck): RotatE
 bool approx_supported(int el) { return el == kge::EL_ROT; }
 // Byte offsets inside a tensor-core candidate image (kge_tc_pack_table): operand planes, then per-row
@@ -124,51 +143,61 @@ struct TcImageLayout {
     total = meta + kge::tc::TC_META_BYTES;
   }
 };
+// The pieces of a candidate image at `bpack`, typed: writable for the pack (Byte = unsigned char),
+// read-only for the scan (Byte = const unsigned char).
+template <class Byte>
+struct TcImage {
+  template <class T>
+  using Ptr = std::conditional_t<std::is_const<Byte>::value, const T*, T*>;
+  Byte* bpack;
+  Ptr<float> cbound, cnorm2, cprefix, cbmax32, cpmax32;
+  Ptr<kge::tc::TcMeta> meta;
+  TcImage(Byte* base, int64_t n_rows, int n_kb) : bpack(base) {
+    const TcImageLayout L(n_rows, n_kb);
+    auto at = [&](size_t off) { return reinterpret_cast<Ptr<float>>(base + off); };
+    cbound = at(L.cbound); cnorm2 = at(L.cnorm2); cprefix = at(L.cprefix);
+    cbmax32 = at(L.cbmax32); cpmax32 = at(L.cpmax32);
+    meta = reinterpret_cast<Ptr<kge::tc::TcMeta>>(base + L.meta);
+  }
+};
+// contraction length of the operand images: all planes for ComplEx / Analogy; L2 carries the candidate's
+// squared norm in three extra k slots (tc.h: launch_pack_b)
 int tc_k_total(int el, int dim) {
   if (el == kge::EL_DOT3) return 3 * dim;   // all three planes of Analogy
   return el == kge::EL_DOT2 ? 2 * dim : (tc_is_l2(el) ? dim + 3 : dim);
 }
 
-Workspace carve(void* base, int qw, int dim, int64_t n, int el = -1, int64_t n_rows = 0,
-                int flags = 0) {
+Workspace carve(void* base, int qw, int dim, int64_t n, int el = -1, int64_t n_rows = 0, int flags = 0) {
   const int64_t n_qt = (n + kge::TILE_Q - 1) / kge::TILE_Q;
+  Carver c{base};
   Workspace w;
-  size_t off = 0;
-  auto take = [&](size_t bytes) {
-    void* p = base ? static_cast<char*>(base) + off : nullptr;
-    off += align_up(bytes, 256);
-    return p;
-  };
-  w.qplain = static_cast<float*>(take((size_t)n * qw * dim * sizeof(float)));
-  w.qpacked = static_cast<float*>(take((size_t)n_qt * dim * qw * kge::TILE_Q * sizeof(float)));
-  w.s_true = static_cast<float*>(take((size_t)n_qt * kge::TILE_Q * sizeof(float)));
-  w.perm = static_cast<int32_t*>(take((size_t)dim * sizeof(int32_t)));
-  w.code = static_cast<uint8_t*>(take((size_t)dim));
-  w.apack = nullptr; w.qbound = w.qnorm2 = w.qprefix = nullptr; w.amb_count = nullptr; w.amb_pairs = nullptr;
-  w.meta_a = nullptr;
-  w.amb_cap = 0;
+  w.qplain = c.take<float>((size_t)n * qw * dim * sizeof(float));
+  w.qpacked = c.take<float>((size_t)n_qt * dim * qw * kge::TILE_Q * sizeof(float));
+  w.s_true = c.take<float>((size_t)n_qt * kge::TILE_Q * sizeof(float));
+  w.perm = c.take<int32_t>((size_t)dim * sizeof(int32_t));
+  w.code = c.take<uint8_t>((size_t)dim);
   const bool want_tc = (flags & KGE_FLAG_TENSOR_CORE) && el >= 0 && tc_supported(el) && n_rows > 0;
   const bool want_approx = (flags & KGE_FLAG_APPROX_SCAN) && approx_supported(el) && n_rows > 0;
   if (want_tc) {
     const int n_kb = kge::tc::n_kblocks(tc_k_total(el, dim));
-    w.apack = static_cast<unsigned char*>(take(kge::tc::a_image_bytes(n, n_kb)));
-    w.qbound = static_cast<float*>(take((size_t)n * sizeof(float)));
-    w.qnorm2 = static_cast<float*>(take((size_t)n * sizeof(float)));
-    w.qprefix = static_cast<float*>(take((size_t)n * sizeof(float)));
-    w.meta_a = static_cast<kge::tc::TcMeta*>(take(kge::tc::TC_META_BYTES));
+    w.apack = c.take<unsigned char>(kge::tc::a_image_bytes(n, n_kb));
+    w.qbound = c.take<float>((size_t)n * sizeof(float));
+    w.qnorm2 = c.take<float>((size_t)n * sizeof(float));
+    w.qprefix = c.take<float>((size_t)n * sizeof(float));
+    w.meta_a = c.take<kge::tc::TcMeta>(kge::tc::TC_META_BYTES);
   }
   if (want_tc || want_approx) {
     const int64_t n_tc_qt = (n + kge::tc::TC_BM - 1) / kge::tc::TC_BM;
-    w.amb_count = static_cast<unsigned long long*>(take((size_t)n_tc_qt * sizeof(unsigned long long)));
+    w.amb_count = c.take<unsigned long long>((size_t)n_tc_qt * sizeof(unsigned long long));
     // near-tie list, one region per query tile: room for 1/128 of all pairs (the band is
     // 0.1-0.3 % on average), at least 8 Ki entries per tile, at most 256 Mi in total
     unsigned long long cap = (unsigned long long)n * (unsigned long long)n_rows / 128ull;
     if (cap < (unsigned long long)n_tc_qt * 8192ull) cap = (unsigned long long)n_tc_qt * 8192ull;
     if (cap > (1ull << 28)) cap = 1ull << 28;
     w.amb_cap = cap;
-    w.amb_pairs = static_cast<int2*>(take((size_t)cap * sizeof(int2)));
+    w.amb_pairs = c.take<int2>((size_t)cap * sizeof(int2));
   }
-  w.bytes = off;
+  w.bytes = c.off;
   return w;
 }
 
@@ -226,6 +255,88 @@ cudaError_t timed_scan(int el, bool casc, const kge::ScanParams& p, cudaStream_t
   return timed_launch(0, st, [&] { return kge::launch_scan(el, casc, p, st); });
 }
 
+// The setup kge_rank_side, kge_score_all and kge_topk_side share, over their argument structs (which
+// name the shared fields alike).  Each entry point runs checks of its own between these steps; that
+// order decides which error a call with several bad arguments gets.
+template <class Args>
+struct QueryCall {
+  const char* fn;
+  const Args* a;
+  int el = -1;
+  const HostSchedule* hs = nullptr;
+  std::optional<DeviceScope> device;
+
+  int error(int code, const char* what) const { return fail(code, fn, what); }
+  int lookup_kind() {
+    el = kge::elem_kind_for(a->model, a->side);
+    return el < 0 ? error(KGE_ERR_ARG, "unknown model/side") : KGE_OK;
+  }
+  // the query tables and the workspace; own_ok: the pointers only this entry point requires
+  int check_tables(bool own_ok, bool ent1_missing = false) const {
+    const bool rel_side = a->side == KGE_SIDE_REL;  // candidates = relation rows; rel0 / rel1 unused
+    if (!own_ok || (!a->rel0 && !rel_side) || !a->hrows || !a->trows || !a->workspace)
+      return error(KGE_ERR_ARG, "null pointer");
+    if (ent1_missing) return error(KGE_ERR_ARG, "ent1 required");
+    if (!rel_side && model_needs_rel1(a->model) && !a->rel1) return error(KGE_ERR_ARG, "rel1 required");
+    return KGE_OK;
+  }
+  int lookup_schedule() {
+    hs = get_schedule(a->model, a->dim);
+    return hs ? KGE_OK : error(KGE_ERR_UNSUPPORTED, "unsupported dim");
+  }
+  // On the device of `device_ptr` for the rest of the call: check the size of the carved workspace,
+  // upload the schedule and build the queries.
+  int prepare(const void* device_ptr, const Workspace& w, size_t bytes, bool scalar_layout = true) {
+    device.emplace(device_ptr);
+    if (bytes > a->workspace_bytes) return error(KGE_ERR_ARG, "workspace too small");
+    return prepare_queries(a->model, a->side, a->dim, a->n, a->hrows, a->trows, a->rel0, a->rel1, a->r_idx, hs, w,
+                           el, stream(), scalar_layout);
+  }
+  cudaStream_t stream() const { return static_cast<cudaStream_t>(a->stream); }
+};
+
+// The scalar scan of n_q queries (qpacked) against n_rows candidates (packed); the caller sets what
+// it produces: counts, scores, the near-tie list or the collect lists.
+kge::ScanParams scan_params(const float* packed, const float* qpacked, const float* s_true, const HostSchedule* hs,
+                            int dim, int64_t n_q, int64_t n_rows) {
+  kge::ScanParams p;
+  p.packed = packed;
+  p.qpacked = qpacked;
+  p.s_true = s_true;
+  p.code_host = hs->s.code.data();
+  p.dim = dim;
+  p.n_q = n_q;
+  p.n_rows = n_rows;
+  p.n_ct = (n_rows + kge::TILE_C - 1) / kge::TILE_C;
+  p.n_qt = (n_q + kge::TILE_Q - 1) / kge::TILE_Q;
+  return p;
+}
+
+// Bound-and-refine, the tensor-core scan (tc) or RotatE's approximate scan: scan(region_cap) decides
+// every pair outside the near-tie band and lists the rest, one region per 128-query tile; the
+// recheck re-scores those exactly.
+template <class Scan>
+int refine(bool tc, const kge_rank_args_t* a, int el, const Workspace& w, cudaStream_t st, Scan&& scan) {
+  const int regions = (int)((a->n + kge::tc::TC_BM - 1) / kge::tc::TC_BM);
+  const unsigned long long region_cap = w.amb_cap / (unsigned long long)regions;
+  KGE_CUDA_TRY(cudaMemsetAsync(w.amb_count, 0, (size_t)regions * sizeof(unsigned long long), st),
+               tc ? "tc reset list" : "approx reset list");
+  KGE_CUDA_TRY(timed_launch(tc ? 1 : 0, st, [&] { return scan(region_cap); }), tc ? "tc scan" : "approx rank scan");
+  KGE_CUDA_TRY(timed_launch(2, st, [&] {
+                 return kge::tc::launch_recheck(el, a->dim, w.amb_count, regions, region_cap, w.amb_pairs, w.qplain,
+                                                a->ent0, a->ent1, w.s_true, a->raw_count,
+                                                reinterpret_cast<unsigned long long*>(a->tc_stats), st);
+               }),
+               tc ? "tc recheck" : "approx recheck");
+  return KGE_OK;
+}
+
+// The sparse filter pass over the CSR of `a`, after either scan
+cudaError_t launch_filter_pass(const kge_rank_args_t* a, int el, bool casc, const Workspace& w, cudaStream_t st) {
+  return kge::launch_filter(el, casc, a->dim, a->n, a->n_filt, w.qplain, a->ent0, a->ent1, a->ent_lo, a->n_rows,
+                            a->filt_offs, a->filt_ids, a->filt_qid, w.perm, w.code, w.s_true, a->filt_sub, st);
+}
+
 }  // namespace
 
 extern "C" {
@@ -275,9 +386,7 @@ int kge_pack_table(int model, const float* ent0, const float* ent1, int64_t n_ro
   if (!hs) return fail(KGE_ERR_UNSUPPORTED, "kge_pack_table: unsupported dim");
   DeviceScope device_scope(ent0);
   cudaStream_t st = static_cast<cudaStream_t>(stream);
-  // inv_perm is staged in the tail of the packed buffer?  No: it would be overwritten.  Use a
-  // small stream-ordered allocation instead (freed on the same stream).
-  int32_t* d_inv = nullptr;
+  int32_t* d_inv = nullptr;   // a stream-ordered allocation, freed on the same stream
   KGE_CUDA_TRY(cudaMallocAsync(reinterpret_cast<void**>(&d_inv), (size_t)dim * sizeof(int32_t), st),
                "pack_table: cudaMallocAsync");
   cudaError_t e = cudaMemcpyAsync(d_inv, hs->inv_perm.data(), (size_t)dim * sizeof(int32_t),
@@ -353,12 +462,9 @@ int kge_tc_pack_table_cached(int model, const float* ent0, const float* ent1, in
   DeviceScope device_scope(ent0);
   const int k_total = tc_k_total(el, dim);
   const int n_kb = kge::tc::n_kblocks(k_total);
-  unsigned char* bpack = static_cast<unsigned char*>(tc_packed);
-  const TcImageLayout L(n_rows, n_kb);
-  auto fptr = [&](size_t off) { return reinterpret_cast<float*>(bpack + off); };
-  KGE_CUDA_TRY(kge::tc::launch_pack_b(ent0, ent1, n_rows, dim, k_total, n_kb, tc_is_l2(el), bpack, fptr(L.cbound),
-                                      fptr(L.cnorm2), fptr(L.cprefix), fptr(L.cbmax32), fptr(L.cpmax32),
-                                      reinterpret_cast<kge::tc::TcMeta*>(bpack + L.meta),
+  const TcImage<unsigned char> b(static_cast<unsigned char*>(tc_packed), n_rows, n_kb);
+  KGE_CUDA_TRY(kge::tc::launch_pack_b(ent0, ent1, n_rows, dim, k_total, n_kb, tc_is_l2(el), b.bpack, b.cbound,
+                                      b.cnorm2, b.cprefix, b.cbmax32, b.cpmax32, b.meta,
                                       reinterpret_cast<unsigned long long*>(guard),
                                       static_cast<cudaStream_t>(stream)),
                "tc pack table");
@@ -366,38 +472,30 @@ int kge_tc_pack_table_cached(int model, const float* ent0, const float* ent1, in
 }
 
 int kge_rank_side(const kge_rank_args_t* a) {
-  if (!a) return fail(KGE_ERR_ARG, "kge_rank_side: null args");
-  const int el = kge::elem_kind_for(a->model, a->side);
-  if (el < 0) return fail(KGE_ERR_ARG, "kge_rank_side: unknown model/side");
+  QueryCall<kge_rank_args_t> q{"kge_rank_side", a};
+  if (!a) return q.error(KGE_ERR_ARG, "null args");
+  if (int rc = q.lookup_kind()) return rc;
   if (a->n == 0) return KGE_OK;
-  if (a->n < 0 || a->n_rows < 0 || a->dim < 1) return fail(KGE_ERR_ARG, "kge_rank_side: bad sizes");
+  if (a->n < 0 || a->n_rows < 0 || a->dim < 1) return q.error(KGE_ERR_ARG, "bad sizes");
+  const int el = q.el;
   const bool rel_side = a->side == KGE_SIDE_REL;
-  if (!a->ent0 || (!a->rel0 && !rel_side) || !a->hrows || !a->trows || !a->raw_count || !a->workspace)
-    return fail(KGE_ERR_ARG, "kge_rank_side: null pointer");
-  if (kge::elem_cw(el) >= 2 && !a->ent1) return fail(KGE_ERR_ARG, "kge_rank_side: ent1 required");
-  if (!rel_side && model_needs_rel1(a->model) && !a->rel1)
-    return fail(KGE_ERR_ARG, "kge_rank_side: rel1 required");
+  if (int rc = q.check_tables(a->ent0 && a->raw_count, kge::elem_cw(el) >= 2 && !a->ent1)) return rc;
   if (rel_side && !a->true_rows && !a->true_score_in)
-    return fail(KGE_ERR_ARG, "kge_rank_side: true_rows required for KGE_SIDE_REL");
+    return q.error(KGE_ERR_ARG, "true_rows required for KGE_SIDE_REL");
   if (a->filt_offs && (!a->filt_ids || !a->filt_sub) && a->n_filt > 0)
-    return fail(KGE_ERR_ARG, "kge_rank_side: filter arrays incomplete");
-  const HostSchedule* hs = get_schedule(a->model, a->dim);
-  if (!hs) return fail(KGE_ERR_UNSUPPORTED, "kge_rank_side: unsupported dim");
-  DeviceScope device_scope(a->ent0);
-  const int qw = kge::elem_qw(el);
+    return q.error(KGE_ERR_ARG, "filter arrays incomplete");
+  if (int rc = q.lookup_schedule()) return rc;
   const bool use_tc = (a->flags & KGE_FLAG_TENSOR_CORE) && tc_supported(el) && a->n_rows > 0;
-  if (use_tc && !a->tc_packed) return fail(KGE_ERR_ARG, "kge_rank_side: tc_packed required with KGE_FLAG_TENSOR_CORE");
-  if (!use_tc && !a->packed) return fail(KGE_ERR_ARG, "kge_rank_side: packed table required (scalar scan)");
+  if (use_tc && !a->tc_packed) return q.error(KGE_ERR_ARG, "tc_packed required with KGE_FLAG_TENSOR_CORE");
+  if (!use_tc && !a->packed) return q.error(KGE_ERR_ARG, "packed table required (scalar scan)");
   const bool use_approx = !use_tc && (a->flags & KGE_FLAG_APPROX_SCAN) && approx_supported(el) && a->n_rows > 0;
-  Workspace w = carve(a->workspace, qw, a->dim, a->n, el, a->n_rows,
-                      use_tc ? KGE_FLAG_TENSOR_CORE : (use_approx ? KGE_FLAG_APPROX_SCAN : 0));
-  if (w.bytes > a->workspace_bytes) return fail(KGE_ERR_ARG, "kge_rank_side: workspace too small");
-  cudaStream_t st = static_cast<cudaStream_t>(a->stream);
+  const int qw = kge::elem_qw(el);
+  const Workspace w = carve(a->workspace, qw, a->dim, a->n, el, a->n_rows,
+                            use_tc ? KGE_FLAG_TENSOR_CORE : (use_approx ? KGE_FLAG_APPROX_SCAN : 0));
+  if (int rc = q.prepare(a->ent0, w, w.bytes, !use_tc)) return rc;
+  cudaStream_t st = q.stream();
+  const HostSchedule* hs = q.hs;
   const bool casc = hs->s.has_cascade;
-
-  int rc = prepare_queries(a->model, a->side, a->dim, a->n, a->hrows, a->trows, a->rel0, a->rel1,
-                           a->r_idx, hs, w, el, st, !use_tc);
-  if (rc != KGE_OK) return rc;
 
   // true scores: the true entity's row is the gathered tail (tail side) / head (head side) row
   const int64_t n_qt = (a->n + kge::TILE_Q - 1) / kge::TILE_Q;
@@ -417,98 +515,63 @@ int kge_rank_side(const kge_rank_args_t* a) {
     KGE_CUDA_TRY(cudaMemcpyAsync(a->true_score, w.s_true, (size_t)a->n * sizeof(float),
                                  cudaMemcpyDeviceToDevice, st),
                  "copy true_score");
+  if (a->n_rows == 0) return KGE_OK;
 
   if (use_tc) {
     // tensor-core bound-and-refine: approximate scores decide all but the near-tie band,
     // which is re-scored exactly (same device functions as the scalar scan)
     const int k_total = tc_k_total(el, a->dim);
     const int n_kb = kge::tc::n_kblocks(k_total);
-    const int64_t n_ct = (a->n_rows + kge::tc::TC_BN - 1) / kge::tc::TC_BN;
-    const bool l2 = el == kge::EL_L2_TAIL || el == kge::EL_L2_HEAD;
-    const unsigned char* bpack = static_cast<const unsigned char*>(a->tc_packed);
-    const TcImageLayout L(a->n_rows, n_kb);
-    const kge::tc::TcMeta* meta_b = reinterpret_cast<const kge::tc::TcMeta*>(bpack + L.meta);
+    const bool l2 = tc_is_l2(el);
+    const TcImage<const unsigned char> b(static_cast<const unsigned char*>(a->tc_packed), a->n_rows, n_kb);
     KGE_CUDA_TRY(kge::tc::launch_pack_a(w.qplain, qw, a->n, a->dim, k_total, n_kb,
                                         el == kge::EL_L2_HEAD ? 1 : 0, l2, w.apack, w.qbound, w.qnorm2, w.qprefix,
-                                        w.meta_a, meta_b, st),
+                                        w.meta_a, b.meta, st),
                  "tc pack queries");
     if (kge::tc::scan_grid_size(a->n, a->n_rows, n_kb) <= 0)
       return fail(KGE_ERR_CUDA, "kge_rank_side: cannot size the tensor-core grid");
-    const int regions = (int)((a->n + kge::tc::TC_BM - 1) / kge::tc::TC_BM);  // one per query tile
-    const unsigned long long region_cap = w.amb_cap / (unsigned long long)regions;
-    KGE_CUDA_TRY(cudaMemsetAsync(w.amb_count, 0, (size_t)regions * sizeof(unsigned long long), st), "tc reset list");
-    auto fptr = [&](size_t off) { return reinterpret_cast<const float*>(bpack + off); };
     kge::tc::TcScanParams tp;
-    tp.meta_a = w.meta_a; tp.meta_b = meta_b; tp.fp16 = 0;
-    tp.apack = w.apack; tp.bpack = bpack; tp.s_true = w.s_true;
+    tp.meta_a = w.meta_a; tp.meta_b = b.meta;
+    tp.apack = w.apack; tp.bpack = b.bpack; tp.s_true = w.s_true;
     tp.qbound = w.qbound; tp.qnorm2 = w.qnorm2;
-    tp.cbound = fptr(L.cbound); tp.cnorm2 = fptr(L.cnorm2); tp.cprefix = fptr(L.cprefix);
-    tp.cbmax32 = fptr(L.cbmax32); tp.cpmax32 = fptr(L.cpmax32); tp.qprefix = w.qprefix;
+    tp.cbound = b.cbound; tp.cnorm2 = b.cnorm2; tp.cprefix = b.cprefix;
+    tp.cbmax32 = b.cbmax32; tp.cpmax32 = b.cpmax32; tp.qprefix = w.qprefix;
     tp.gamma_p = kge::tc::tc_gamma_p();
     tp.counts = a->raw_count; tp.amb_count = w.amb_count; tp.amb_pairs = w.amb_pairs;
-    tp.amb_cap = region_cap; tp.dump = a->tc_dump;
+    tp.dump = a->tc_dump;
     const int ref_depth = kge::schedule_depth(hs->s);
     tp.gamma = kge::tc::tc_gamma(k_total, ref_depth, l2, kge::tc::fp16()); tp.gamma2 = kge::tc::tc_gamma2(ref_depth);
     tp.l2 = l2 ? 1 : 0;
-    tp.n_kb = n_kb; tp.k_total = k_total; tp.ct_group = 0;
+    tp.n_kb = n_kb; tp.k_total = k_total;
     tp.n_q = a->n; tp.n_rows = a->n_rows;
-    tp.n_qt = (a->n + kge::tc::TC_BM - 1) / kge::tc::TC_BM; tp.n_ct = n_ct;
-    KGE_CUDA_TRY(timed_launch(1, st, [&] { return kge::tc::launch_tc_scan(tp, st); }), "tc scan");
-    KGE_CUDA_TRY(timed_launch(2, st, [&] {
-                   return kge::tc::launch_recheck(el, a->dim, w.amb_count, regions, region_cap, w.amb_pairs,
-                                                  w.qplain, a->ent0, a->ent1, w.s_true, a->raw_count,
-                                                  reinterpret_cast<unsigned long long*>(a->tc_stats), st);
-                 }),
-                 "tc recheck");
-    if (a->filt_offs && a->n_filt > 0)
-      KGE_CUDA_TRY(kge::launch_filter(el, casc, a->dim, a->n, a->n_filt, w.qplain, a->ent0, a->ent1,
-                                      a->ent_lo, a->n_rows, a->filt_offs, a->filt_ids, a->filt_qid, w.perm,
-                                      w.code, w.s_true, a->filt_sub, st),
-                   "filter pass");
-  } else if (a->n_rows > 0) {
-    kge::ScanParams p;
-    p.packed = a->packed;
-    p.qpacked = w.qpacked;
-    p.s_true = w.s_true;
-    p.code_host = hs->s.code.data();
+    tp.n_qt = (a->n + kge::tc::TC_BM - 1) / kge::tc::TC_BM; tp.n_ct = (a->n_rows + kge::tc::TC_BN - 1) / kge::tc::TC_BN;
+    if (int rc = refine(true, a, el, w, st, [&](unsigned long long region_cap) {
+          tp.amb_cap = region_cap;
+          return kge::tc::launch_tc_scan(tp, st);
+        }))
+      return rc;
+  } else {
+    kge::ScanParams p = scan_params(a->packed, w.qpacked, w.s_true, hs, a->dim, a->n, a->n_rows);
     p.counts = a->raw_count;
-    p.scores = nullptr;
-    p.dim = a->dim;
-    p.n_q = a->n;
-    p.n_rows = a->n_rows;
-    p.n_ct = (a->n_rows + kge::TILE_C - 1) / kge::TILE_C;
-    p.n_qt = n_qt;
-    p.amb_count = nullptr; p.amb_pairs = nullptr; p.amb_cap = 0; p.rel_eps = 0.f; p.abs_eps = 0.f;
-    p.col_buf = nullptr; p.col_count = nullptr; p.col_cap = 0; p.col_id_base = 0; p.col_dense = 0;
     if (use_approx) {
       // RotatE bound-and-refine: |s~ - s_ATen| <= rel_eps |s~| (all terms >= 0).  Per element the
       // exact path is within 4 u and the approximate one within 3 u + 2^-21 (sqrt.approx) of the
       // real modulus; the sums add depth * u each: ATen's cascade (schedule_depth) for the exact
       // path, 32 per stage + one per stage for the approximate one.
-      const int regions = (int)((a->n + kge::tc::TC_BM - 1) / kge::tc::TC_BM);
-      const unsigned long long region_cap = w.amb_cap / (unsigned long long)regions;
-      KGE_CUDA_TRY(cudaMemsetAsync(w.amb_count, 0, (size_t)regions * sizeof(unsigned long long), st), "approx reset list");
       const int depth_a = 32 + (a->dim + 31) / 32, depth_e = kge::schedule_depth(hs->s);
-      p.amb_count = w.amb_count; p.amb_pairs = w.amb_pairs; p.amb_cap = region_cap;
+      p.amb_count = w.amb_count; p.amb_pairs = w.amb_pairs;
       p.rel_eps = (float)((depth_a + depth_e + 4 + 11 + 8) * 0x1p-24 * 1.001);
       p.abs_eps = (float)(a->dim * 1.1e-19);
-      KGE_CUDA_TRY(timed_launch(0, st, [&] { return kge::launch_scan(el, casc, p, st, true); }), "approx rank scan");
-      KGE_CUDA_TRY(timed_launch(2, st, [&] {
-                     return kge::tc::launch_recheck(el, a->dim, w.amb_count, regions, region_cap, w.amb_pairs,
-                                                    w.qplain, a->ent0, a->ent1, w.s_true, a->raw_count,
-                                                    reinterpret_cast<unsigned long long*>(a->tc_stats), st);
-                   }),
-                   "approx recheck");
+      if (int rc = refine(false, a, el, w, st, [&](unsigned long long region_cap) {
+            p.amb_cap = region_cap;
+            return kge::launch_scan(el, casc, p, st, true);
+          }))
+        return rc;
     } else {
       KGE_CUDA_TRY(timed_scan(el, casc, p, st), "rank scan");
     }
-
-    if (a->filt_offs && a->n_filt > 0)
-      KGE_CUDA_TRY(kge::launch_filter(el, casc, a->dim, a->n, a->n_filt, w.qplain, a->ent0, a->ent1,
-                                      a->ent_lo, a->n_rows, a->filt_offs, a->filt_ids, a->filt_qid, w.perm,
-                                      w.code, w.s_true, a->filt_sub, st),
-                   "filter pass");
   }
+  if (a->filt_offs && a->n_filt > 0) KGE_CUDA_TRY(launch_filter_pass(a, el, casc, w, st), "filter pass");
   return KGE_OK;
 }
 
@@ -525,10 +588,7 @@ int kge_filter_side(const kge_rank_args_t* a) {
   DeviceScope device_scope(a->ent0);
   Workspace w = carve(a->workspace, kge::elem_qw(el), a->dim, a->n);  // leading part only
   if (w.bytes > a->workspace_bytes) return fail(KGE_ERR_ARG, "kge_filter_side: workspace too small");
-  KGE_CUDA_TRY(kge::launch_filter(el, hs->s.has_cascade, a->dim, a->n, a->n_filt, w.qplain, a->ent0,
-                                  a->ent1, a->ent_lo, a->n_rows, a->filt_offs, a->filt_ids, a->filt_qid, w.perm,
-                                  w.code, w.s_true, a->filt_sub, static_cast<cudaStream_t>(a->stream)),
-               "filter pass");
+  KGE_CUDA_TRY(launch_filter_pass(a, el, hs->s.has_cascade, w, static_cast<cudaStream_t>(a->stream)), "filter pass");
   return KGE_OK;
 }
 
@@ -545,42 +605,20 @@ int kge_finalize_ranks(const int32_t* raw_count, const int32_t* filt_sub, int64_
 }
 
 int kge_score_all(const kge_score_all_args_t* a) {
-  if (!a) return fail(KGE_ERR_ARG, "kge_score_all: null args");
-  const int el = kge::elem_kind_for(a->model, a->side);
-  if (el < 0) return fail(KGE_ERR_ARG, "kge_score_all: unknown model/side");
+  QueryCall<kge_score_all_args_t> q{"kge_score_all", a};
+  if (!a) return q.error(KGE_ERR_ARG, "null args");
+  if (int rc = q.lookup_kind()) return rc;
   if (a->n == 0 || a->n_rows == 0) return KGE_OK;
-  const bool rel_side = a->side == KGE_SIDE_REL;  // candidates = relation rows; rel0 / rel1 unused
-  if (!a->packed || (!a->rel0 && !rel_side) || !a->hrows || !a->trows || !a->scores || !a->workspace)
-    return fail(KGE_ERR_ARG, "kge_score_all: null pointer");
-  if (!rel_side && model_needs_rel1(a->model) && !a->rel1)
-    return fail(KGE_ERR_ARG, "kge_score_all: rel1 required");
-  const HostSchedule* hs = get_schedule(a->model, a->dim);
-  if (!hs) return fail(KGE_ERR_UNSUPPORTED, "kge_score_all: unsupported dim");
-  DeviceScope device_scope(a->packed);
-  const int qw = kge::elem_qw(el);
-  Workspace w = carve(a->workspace, qw, a->dim, a->n);
-  if (w.bytes > a->workspace_bytes) return fail(KGE_ERR_ARG, "kge_score_all: workspace too small");
-  cudaStream_t st = static_cast<cudaStream_t>(a->stream);
-  int rc = prepare_queries(a->model, a->side, a->dim, a->n, a->hrows, a->trows, a->rel0, a->rel1,
-                           a->r_idx, hs, w, el, st);
-  if (rc != KGE_OK) return rc;
+  if (int rc = q.check_tables(a->packed && a->scores)) return rc;
+  if (int rc = q.lookup_schedule()) return rc;
+  const Workspace w = carve(a->workspace, kge::elem_qw(q.el), a->dim, a->n);
+  if (int rc = q.prepare(a->packed, w, w.bytes)) return rc;
+  cudaStream_t st = q.stream();
   const int64_t n_qt = (a->n + kge::TILE_Q - 1) / kge::TILE_Q;
   KGE_CUDA_TRY(kge::launch_fill_f32(w.s_true, 0.f, n_qt * kge::TILE_Q, st), "fill s_true");
-  kge::ScanParams p;
-  p.packed = a->packed;
-  p.qpacked = w.qpacked;
-  p.s_true = w.s_true;
-  p.code_host = hs->s.code.data();
-  p.counts = nullptr;
-  p.amb_count = nullptr; p.amb_pairs = nullptr; p.amb_cap = 0; p.rel_eps = 0.f; p.abs_eps = 0.f;
-  p.col_buf = nullptr; p.col_count = nullptr; p.col_cap = 0; p.col_id_base = 0; p.col_dense = 0;
+  kge::ScanParams p = scan_params(a->packed, w.qpacked, w.s_true, q.hs, a->dim, a->n, a->n_rows);
   p.scores = a->scores;
-  p.dim = a->dim;
-  p.n_q = a->n;
-  p.n_rows = a->n_rows;
-  p.n_ct = (a->n_rows + kge::TILE_C - 1) / kge::TILE_C;
-  p.n_qt = n_qt;
-  KGE_CUDA_TRY(timed_scan(el, hs->s.has_cascade, p, st), "score scan");
+  KGE_CUDA_TRY(timed_scan(q.el, q.hs->s.has_cascade, p, st), "score scan");
   return KGE_OK;
 }
 
@@ -608,19 +646,14 @@ struct TopkWorkspace {
 TopkWorkspace carve_topk(void* base, int qw, int dim, int64_t n, int64_t n_rows, int k) {
   TopkWorkspace t;
   t.w = carve(base, qw, dim, n);
-  size_t off = align_up(t.w.bytes, 256);
-  auto take = [&](size_t bytes) {
-    void* p = base ? static_cast<char*>(base) + off : nullptr;
-    off += align_up(bytes, 256);
-    return p;
-  };
+  Carver c{base, t.w.bytes};
   const int64_t n_qt = (n + kge::TILE_Q - 1) / kge::TILE_Q;
   t.chunk_rows = topk_chunk_rows(n, n_rows);
-  t.thr = static_cast<float*>(take((size_t)n_qt * kge::TILE_Q * sizeof(float)));
-  t.col_count = static_cast<unsigned*>(take((size_t)n * sizeof(unsigned)));
-  t.col_buf = static_cast<int2*>(take((size_t)n * t.chunk_rows * sizeof(int2)));
-  t.best = static_cast<unsigned long long*>(take((size_t)n * k * sizeof(unsigned long long)));
-  t.bytes = off;
+  t.thr = c.take<float>((size_t)n_qt * kge::TILE_Q * sizeof(float));
+  t.col_count = c.take<unsigned>((size_t)n * sizeof(unsigned));
+  t.col_buf = c.take<int2>((size_t)n * t.chunk_rows * sizeof(int2));
+  t.best = c.take<unsigned long long>((size_t)n * k * sizeof(unsigned long long));
+  t.bytes = c.off;
   return t;
 }
 }  // namespace
@@ -632,31 +665,23 @@ size_t kge_topk_workspace_bytes(int model, int side, int dim, int64_t n, int64_t
 }
 
 int kge_topk_side(const kge_topk_args_t* a) {
-  if (!a) return fail(KGE_ERR_ARG, "kge_topk_side: null args");
-  const int el = kge::elem_kind_for(a->model, a->side);
-  if (el < 0) return fail(KGE_ERR_ARG, "kge_topk_side: unknown model/side");
-  if (a->k < 1 || a->k > kge::TOPK_MAX_K) return fail(KGE_ERR_ARG, "kge_topk_side: k must be in [1, 1024]");
-  if (a->n < 0 || a->n_rows < 0 || a->dim < 1) return fail(KGE_ERR_ARG, "kge_topk_side: bad sizes");
-  if ((int64_t)a->k > a->n_rows) return fail(KGE_ERR_ARG, "kge_topk_side: k exceeds the number of candidates");
+  QueryCall<kge_topk_args_t> q{"kge_topk_side", a};
+  if (!a) return q.error(KGE_ERR_ARG, "null args");
+  if (int rc = q.lookup_kind()) return rc;
+  if (a->k < 1 || a->k > kge::TOPK_MAX_K) return q.error(KGE_ERR_ARG, "k must be in [1, 1024]");
+  if (a->n < 0 || a->n_rows < 0 || a->dim < 1) return q.error(KGE_ERR_ARG, "bad sizes");
+  if ((int64_t)a->k > a->n_rows) return q.error(KGE_ERR_ARG, "k exceeds the number of candidates");
   // candidate ids travel as int32 through the collect lists and the 64-bit keys
   if (a->ent_lo < 0 || a->ent_lo + a->n_rows > (int64_t)INT32_MAX)
-    return fail(KGE_ERR_ARG, "kge_topk_side: ent_lo + n_rows must lie in [0, 2^31 - 1]");
+    return q.error(KGE_ERR_ARG, "ent_lo + n_rows must lie in [0, 2^31 - 1]");
   if (a->n == 0) return KGE_OK;
-  const bool rel_side = a->side == KGE_SIDE_REL;
-  if (!a->packed || (!a->rel0 && !rel_side) || !a->hrows || !a->trows || !a->pred || !a->scores || !a->workspace)
-    return fail(KGE_ERR_ARG, "kge_topk_side: null pointer");
-  if (!rel_side && model_needs_rel1(a->model) && !a->rel1) return fail(KGE_ERR_ARG, "kge_topk_side: rel1 required");
-  if (a->mask_offs && !a->mask_ids) return fail(KGE_ERR_ARG, "kge_topk_side: mask arrays incomplete");
-  const HostSchedule* hs = get_schedule(a->model, a->dim);
-  if (!hs) return fail(KGE_ERR_UNSUPPORTED, "kge_topk_side: unsupported dim");
-  DeviceScope device_scope(a->packed);
-  const int qw = kge::elem_qw(el), cw = kge::elem_cw(el);
-  TopkWorkspace t = carve_topk(a->workspace, qw, a->dim, a->n, a->n_rows, a->k);
-  if (t.bytes > a->workspace_bytes) return fail(KGE_ERR_ARG, "kge_topk_side: workspace too small");
-  cudaStream_t st = static_cast<cudaStream_t>(a->stream);
-  int rc = prepare_queries(a->model, a->side, a->dim, a->n, a->hrows, a->trows, a->rel0, a->rel1, a->r_idx, hs,
-                           t.w, el, st);
-  if (rc != KGE_OK) return rc;
+  if (int rc = q.check_tables(a->packed && a->pred && a->scores)) return rc;
+  if (a->mask_offs && !a->mask_ids) return q.error(KGE_ERR_ARG, "mask arrays incomplete");
+  if (int rc = q.lookup_schedule()) return rc;
+  const int cw = kge::elem_cw(q.el);
+  const TopkWorkspace t = carve_topk(a->workspace, kge::elem_qw(q.el), a->dim, a->n, a->n_rows, a->k);
+  if (int rc = q.prepare(a->packed, t.w, t.bytes)) return rc;
+  cudaStream_t st = q.stream();
   const int64_t n_qt = (a->n + kge::TILE_Q - 1) / kge::TILE_Q;
   KGE_CUDA_TRY(kge::launch_fill_f32(t.thr, -__builtin_inff(), n_qt * kge::TILE_Q, st), "topk: thresholds");
   KGE_CUDA_TRY(cudaMemsetAsync(t.best, 0, (size_t)a->n * a->k * sizeof(unsigned long long), st), "topk: reset lists");
@@ -664,18 +689,11 @@ int kge_topk_side(const kge_topk_args_t* a) {
     const int64_t rows = a->n_rows - c0 < t.chunk_rows ? a->n_rows - c0 : t.chunk_rows;
     const bool first = c0 == 0;   // thresholds are -inf: every candidate is collected, slot = row
     if (!first) KGE_CUDA_TRY(cudaMemsetAsync(t.col_count, 0, (size_t)a->n * sizeof(unsigned), st), "topk: reset counts");
-    kge::ScanParams p;
-    p.packed = a->packed + (size_t)(c0 / kge::TILE_C) * a->dim * cw * kge::TILE_C;
-    p.qpacked = t.w.qpacked;
-    p.s_true = t.thr;
-    p.code_host = hs->s.code.data();
-    p.counts = nullptr; p.scores = nullptr;
-    p.amb_count = nullptr; p.amb_pairs = nullptr; p.amb_cap = 0; p.rel_eps = 0.f; p.abs_eps = 0.f;
+    kge::ScanParams p = scan_params(a->packed + (size_t)(c0 / kge::TILE_C) * a->dim * cw * kge::TILE_C, t.w.qpacked,
+                                    t.thr, q.hs, a->dim, a->n, rows);
     p.col_buf = t.col_buf; p.col_count = t.col_count; p.col_cap = (unsigned long long)t.chunk_rows;
     p.col_id_base = a->ent_lo + c0; p.col_dense = first ? 1 : 0;
-    p.dim = a->dim; p.n_q = a->n; p.n_rows = rows;
-    p.n_ct = (rows + kge::TILE_C - 1) / kge::TILE_C; p.n_qt = n_qt;
-    KGE_CUDA_TRY(timed_scan(el, hs->s.has_cascade, p, st), "topk: collect scan");
+    KGE_CUDA_TRY(timed_scan(q.el, q.hs->s.has_cascade, p, st), "topk: collect scan");
     KGE_CUDA_TRY(kge::launch_topk_merge(t.best, a->k, t.col_buf, t.col_count, (unsigned long long)t.chunk_rows,
                                         first ? rows : -1, a->mask_offs, a->mask_ids, t.thr, a->n, st),
                  "topk: merge");

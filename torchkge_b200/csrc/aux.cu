@@ -447,34 +447,17 @@ cudaError_t launch_fill_f32(float* dst, float value, int64_t n, cudaStream_t str
   return cudaGetLastError();
 }
 
-#define KGE_DISPATCH_EL(el, cascade, CALL)                                  \
-  switch (el) {                                                             \
-    case EL_DOT1: if (cascade) { CALL(EL_DOT1, true); } else { CALL(EL_DOT1, false); } break; \
-    case EL_DOT2: if (cascade) { CALL(EL_DOT2, true); } else { CALL(EL_DOT2, false); } break; \
-    case EL_DOT3: if (cascade) { CALL(EL_DOT3, true); } else { CALL(EL_DOT3, false); } break; \
-    case EL_ROT: if (cascade) { CALL(EL_ROT, true); } else { CALL(EL_ROT, false); } break;    \
-    case EL_DOT_MID: if (cascade) { CALL(EL_DOT_MID, true); } else { CALL(EL_DOT_MID, false); } break; \
-    case EL_TL1_TAIL: if (cascade) { CALL(EL_TL1_TAIL, true); } else { CALL(EL_TL1_TAIL, false); } break; \
-    case EL_TL1_HEAD: if (cascade) { CALL(EL_TL1_HEAD, true); } else { CALL(EL_TL1_HEAD, false); } break; \
-    case EL_TL2_TAIL: if (cascade) { CALL(EL_TL2_TAIL, true); } else { CALL(EL_TL2_TAIL, false); } break; \
-    case EL_TL2_HEAD: if (cascade) { CALL(EL_TL2_HEAD, true); } else { CALL(EL_TL2_HEAD, false); } break; \
-    case EL_L1_TAIL: CALL(EL_L1_TAIL, false); break;                        \
-    case EL_L1_HEAD: CALL(EL_L1_HEAD, false); break;                        \
-    case EL_L2_TAIL: CALL(EL_L2_TAIL, false); break;                        \
-    case EL_L2_HEAD: CALL(EL_L2_HEAD, false); break;                        \
-    default: return cudaErrorInvalidValue;                                  \
-  }
-
 cudaError_t launch_true_scores(int el, bool cascade, int dim, int64_t n, const float* qplain,
                                const float* rows, const int32_t* perm, const uint8_t* code,
                                float* s_true, cudaStream_t stream) {
   if (n <= 0) return cudaSuccess;
-#define CALL_TRUE(EL, C)                                                                                   \
-  true_scores_kernel<EL, C><<<blocks_for(n * (ElemTraits<EL>::RED == RED_SEQ ? 1 : (ElemTraits<EL>::RED == RED_NORM2 ? 8 : 32)), 128), \
-                              128, 0, stream>>>(dim, n, qplain, rows, perm, code, s_true)
-  KGE_DISPATCH_EL(el, cascade, CALL_TRUE)
-#undef CALL_TRUE
-  return cudaGetLastError();
+  return dispatch_elem(el, cascade, [&](auto kind, auto casc) {
+    constexpr int EL = decltype(kind)::value;
+    constexpr int LANES = ElemTraits<EL>::RED == RED_SEQ ? 1 : (ElemTraits<EL>::RED == RED_NORM2 ? 8 : 32);
+    true_scores_kernel<EL, decltype(casc)::value><<<blocks_for(n * LANES, 128), 128, 0, stream>>>(
+        dim, n, qplain, rows, perm, code, s_true);
+    return cudaGetLastError();
+  });
 }
 
 cudaError_t launch_filter(int el, bool cascade, int dim, int64_t n, int64_t n_filt,
@@ -483,13 +466,11 @@ cudaError_t launch_filter(int el, bool cascade, int dim, int64_t n, int64_t n_fi
                           const int64_t* ids, const int32_t* qid, const int32_t* perm, const uint8_t* code,
                           const float* s_true, int32_t* filt_sub, cudaStream_t stream) {
   if (n <= 0 || n_filt <= 0) return cudaSuccess;
-#define CALL_FILT(EL, C)                                                                   \
-  filter_kernel<EL, C><<<filter_blocks(n_filt), 128, 0, stream>>>(                         \
-      dim, n, n_filt, qplain, ent0, ent1, ent_lo, n_rows, offs, ids, qid, perm, code, s_true,   \
-      filt_sub)
-  KGE_DISPATCH_EL(el, cascade, CALL_FILT)
-#undef CALL_FILT
-  return cudaGetLastError();
+  return dispatch_elem(el, cascade, [&](auto kind, auto casc) {
+    filter_kernel<decltype(kind)::value, decltype(casc)::value><<<filter_blocks(n_filt), 128, 0, stream>>>(
+        dim, n, n_filt, qplain, ent0, ent1, ent_lo, n_rows, offs, ids, qid, perm, code, s_true, filt_sub);
+    return cudaGetLastError();
+  });
 }
 
 cudaError_t launch_finalize(const int32_t* raw, const int32_t* sub, int64_t n, int64_t* ranks,

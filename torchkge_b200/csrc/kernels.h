@@ -3,6 +3,8 @@
 #include <cuda_runtime.h>
 #include <stdint.h>
 
+#include <type_traits>
+
 #include "../../include/kge_b200.h"
 #include "reduce.cuh"
 
@@ -32,34 +34,65 @@ constexpr int SCAN_MAX_DIM = 8192;   // schedule bytes carried in the kernel par
 // schedule then lives in the constant bank, indexed with uniform registers, so that every
 // test on it is a uniform branch (no convergence barriers, no shared-memory latency).
 struct ScanParams {
-  const float* packed;   // [n_ct][dim][CW][TILE_C]
-  const float* qpacked;  // [n_qt][dim][QW][TILE_Q]
-  const float* s_true;   // [n_qt*TILE_Q], NaN padded
-  const uint8_t* code_host;  // [dim] schedule codes (HOST pointer; copied into `code` at launch)
-  int32_t* counts;       // [n_q] (+=) or nullptr
-  float* scores;         // [n_q][n_rows] or nullptr
+  const float* packed = nullptr;   // [n_ct][dim][CW][TILE_C]
+  const float* qpacked = nullptr;  // [n_qt][dim][QW][TILE_Q]
+  const float* s_true = nullptr;   // [n_qt*TILE_Q], NaN padded
+  const uint8_t* code_host = nullptr;  // [dim] schedule codes (HOST pointer; copied into `code` at launch)
+  int32_t* counts = nullptr;       // [n_q] (+=) or nullptr
+  float* scores = nullptr;         // [n_q][n_rows] or nullptr
   // bound-and-refine form (RotatE): approximate element arithmetic, pairs whose approximate
   // score is within rel_eps * |score| of s_true go to the near-tie list (regions of 128 queries)
-  unsigned long long* amb_count;  // [ceil(n_q / 128)] or nullptr (exact scan)
-  int2* amb_pairs;                // [regions][amb_cap]
-  unsigned long long amb_cap;
-  float rel_eps;
-  float abs_eps;   // flushed subnormal terms: dim * 1.1e-19
+  unsigned long long* amb_count = nullptr;  // [ceil(n_q / 128)] or nullptr (exact scan)
+  int2* amb_pairs = nullptr;                // [regions][amb_cap]
+  unsigned long long amb_cap = 0;
+  float rel_eps = 0.f;
+  float abs_eps = 0.f;   // flushed subnormal terms: dim * 1.1e-19
   // top-k collect form (kge_topk_side): s_true holds a per-query THRESHOLD; every candidate whose
   // exact score is not below it is appended to the query's list as (score bits, global id)
-  int2* col_buf;                  // [n_q][col_cap] or nullptr
-  unsigned* col_count;            // [n_q] fill counts (unused when col_dense)
-  unsigned long long col_cap;
-  long long col_id_base;          // global id of candidate row 0 of this launch
-  int col_dense;                  // 1: slot = row index (first chunk: everything is collected)
-  int dim;
-  int64_t n_q;
-  int64_t n_rows;
-  int64_t n_ct;
-  int64_t n_qt;
+  int2* col_buf = nullptr;        // [n_q][col_cap] or nullptr
+  unsigned* col_count = nullptr;  // [n_q] fill counts (unused when col_dense)
+  unsigned long long col_cap = 0;
+  long long col_id_base = 0;      // global id of candidate row 0 of this launch
+  int col_dense = 0;              // 1: slot = row index (first chunk: everything is collected)
+  int dim = 0;
+  int64_t n_q = 0;
+  int64_t n_rows = 0;
+  int64_t n_ct = 0;
+  int64_t n_qt = 0;
+  // filled by launch_scan from code_host
   uint32_t mask[SCAN_MAX_DIM / SCAN_KC];  // per stage: bit kk set <=> position needs the slow path
   uint8_t code[SCAN_MAX_DIM];
 };
+static_assert(std::is_trivially_copyable<ScanParams>::value, "ScanParams is a kernel parameter");
+
+// Calls f(std::integral_constant<int, EL>{}, std::bool_constant<CASC>{}) for the element kind `el`
+// and the schedule's cascade flag, and returns what f returns.  Only the kinds reduced by the cascade
+// sum (RED_SUM) have a CASC = true form; the norm kinds are always called with CASC = false.  An
+// unknown kind gives cudaErrorInvalidValue.
+template <class F>
+cudaError_t dispatch_elem(int el, bool cascade, F&& f) {
+  auto with = [&](auto kind) -> cudaError_t {
+    if constexpr (ElemTraits<decltype(kind)::value>::RED == RED_SUM)
+      if (cascade) return f(kind, std::true_type{});
+    return f(kind, std::false_type{});
+  };
+  switch (el) {
+    case EL_DOT1: return with(std::integral_constant<int, EL_DOT1>{});
+    case EL_DOT2: return with(std::integral_constant<int, EL_DOT2>{});
+    case EL_DOT3: return with(std::integral_constant<int, EL_DOT3>{});
+    case EL_ROT: return with(std::integral_constant<int, EL_ROT>{});
+    case EL_DOT_MID: return with(std::integral_constant<int, EL_DOT_MID>{});
+    case EL_TL1_TAIL: return with(std::integral_constant<int, EL_TL1_TAIL>{});
+    case EL_TL1_HEAD: return with(std::integral_constant<int, EL_TL1_HEAD>{});
+    case EL_TL2_TAIL: return with(std::integral_constant<int, EL_TL2_TAIL>{});
+    case EL_TL2_HEAD: return with(std::integral_constant<int, EL_TL2_HEAD>{});
+    case EL_L1_TAIL: return with(std::integral_constant<int, EL_L1_TAIL>{});
+    case EL_L1_HEAD: return with(std::integral_constant<int, EL_L1_HEAD>{});
+    case EL_L2_TAIL: return with(std::integral_constant<int, EL_L2_TAIL>{});
+    case EL_L2_HEAD: return with(std::integral_constant<int, EL_L2_HEAD>{});
+    default: return cudaErrorInvalidValue;
+  }
+}
 
 // dense scan: counts[q] += #{c < n_rows : score(q,c) >= s_true[q]}  (or writes scores)
 // approx = true (EL_ROT only): the bound-and-refine form above; p.amb_* and p.rel_eps must be set

@@ -364,31 +364,9 @@ cudaError_t launch_scan_g(int el, bool cascade, ScanParams& p, cudaStream_t stre
       return cudaErrorInvalidValue;
     return cascade ? launch_one<EL_ROT, true, G, true>(p, stream) : launch_one<EL_ROT, false, G, true>(p, stream);
   }
-  switch (el) {
-    case EL_DOT1:
-      return cascade ? launch_one<EL_DOT1, true, G>(p, stream) : launch_one<EL_DOT1, false, G>(p, stream);
-    case EL_DOT2:
-      return cascade ? launch_one<EL_DOT2, true, G>(p, stream) : launch_one<EL_DOT2, false, G>(p, stream);
-    case EL_DOT3:
-      return cascade ? launch_one<EL_DOT3, true, G>(p, stream) : launch_one<EL_DOT3, false, G>(p, stream);
-    case EL_ROT:
-      return cascade ? launch_one<EL_ROT, true, G>(p, stream) : launch_one<EL_ROT, false, G>(p, stream);
-    case EL_DOT_MID:
-      return cascade ? launch_one<EL_DOT_MID, true, G>(p, stream) : launch_one<EL_DOT_MID, false, G>(p, stream);
-    case EL_TL1_TAIL:
-      return cascade ? launch_one<EL_TL1_TAIL, true, G>(p, stream) : launch_one<EL_TL1_TAIL, false, G>(p, stream);
-    case EL_TL1_HEAD:
-      return cascade ? launch_one<EL_TL1_HEAD, true, G>(p, stream) : launch_one<EL_TL1_HEAD, false, G>(p, stream);
-    case EL_TL2_TAIL:
-      return cascade ? launch_one<EL_TL2_TAIL, true, G>(p, stream) : launch_one<EL_TL2_TAIL, false, G>(p, stream);
-    case EL_TL2_HEAD:
-      return cascade ? launch_one<EL_TL2_HEAD, true, G>(p, stream) : launch_one<EL_TL2_HEAD, false, G>(p, stream);
-    case EL_L1_TAIL: return launch_one<EL_L1_TAIL, false, G>(p, stream);
-    case EL_L1_HEAD: return launch_one<EL_L1_HEAD, false, G>(p, stream);
-    case EL_L2_TAIL: return launch_one<EL_L2_TAIL, false, G>(p, stream);
-    case EL_L2_HEAD: return launch_one<EL_L2_HEAD, false, G>(p, stream);
-    default: return cudaErrorInvalidValue;
-  }
+  return dispatch_elem(el, cascade, [&](auto kind, auto casc) {
+    return launch_one<decltype(kind)::value, decltype(casc)::value, G>(p, stream);
+  });
 }
 
 }  // namespace

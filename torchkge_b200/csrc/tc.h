@@ -3,6 +3,8 @@
 #include <cuda_runtime.h>
 #include <stdint.h>
 
+#include <type_traits>
+
 namespace kge {
 namespace tc {
 
@@ -38,34 +40,35 @@ struct TcMeta {
 constexpr size_t TC_META_BYTES = 256;
 
 struct TcScanParams {
-  const unsigned char* apack;  // [n_qt][n_kb][hi,lo][128 rows x 2*bk() B, swizzled]
-  const unsigned char* bpack;  // [n_ct][n_kb][hi,lo][256 rows x 2*bk() B, swizzled]
-  const float* s_true;         // [n_q] exact (ATen-order) true scores
-  const float* qbound;         // [n_q] >= |a|_2
-  const float* qnorm2;         // [n_q] |a|_2^2 (L2 only)
-  const float* cbound;         // [n_rows] >= |b|_2
-  const float* cnorm2;         // [n_rows]
-  const float* qprefix;        // [n_q]    P(a) = sqrt(sum_i |a_{<=16 i}|^2): running-magnitude factor (tc_gamma_p)
-  const float* cprefix;        // [n_rows] P(b)
-  const float* cbmax32;        // [n_ct * 8] max of cbound over each aligned block of 32 rows
-  const float* cpmax32;        // [n_ct * 8] max of cprefix over each aligned block of 32 rows
-  int32_t* counts;             // [n_q] +=
-  unsigned long long* amb_count;  // [n_qt] fill count of each query tile's region
-  int2* amb_pairs;                // [n_qt][amb_cap]
-  unsigned long long amb_cap;     // capacity of ONE region
-  float* dump;                 // debug: write approximate scores [n_q][n_rows] instead of counting
-  const TcMeta* meta_a;        // device: facts of the query image (this call)
-  const TcMeta* meta_b;        // device: facts of the candidate image
-  int fp16;                    // operand format of the images: 1 = fp16, 0 = bf16 (set by launch_tc_scan)
-  float gamma;                 // tc_gamma(k): multiplies |a| |b|
-  float gamma2;                // tc_gamma2(k) (L2 only): multiplies (|a| + |b|)^2
-  float gamma_p;               // tc_gamma_p(): multiplies P(a) P(b) (accumulation inside the tensor core)
-  int l2;                      // 1: score = -(|a|^2 + |b|^2 - 2 a.b)
-  int n_kb;
-  int k_total;
-  int ct_group;                // candidate tiles a CTA walks per query tile (set by launch_tc_scan)
-  long long n_q, n_rows, n_qt, n_ct;
+  const unsigned char* apack = nullptr;  // [n_qt][n_kb][hi,lo][128 rows x 2*bk() B, swizzled]
+  const unsigned char* bpack = nullptr;  // [n_ct][n_kb][hi,lo][256 rows x 2*bk() B, swizzled]
+  const float* s_true = nullptr;         // [n_q] exact (ATen-order) true scores
+  const float* qbound = nullptr;         // [n_q] >= |a|_2
+  const float* qnorm2 = nullptr;         // [n_q] |a|_2^2 (L2 only)
+  const float* cbound = nullptr;         // [n_rows] >= |b|_2
+  const float* cnorm2 = nullptr;         // [n_rows]
+  const float* qprefix = nullptr;        // [n_q]    P(a) = sqrt(sum_i |a_{<=16 i}|^2): running-magnitude factor (tc_gamma_p)
+  const float* cprefix = nullptr;        // [n_rows] P(b)
+  const float* cbmax32 = nullptr;        // [n_ct * 8] max of cbound over each aligned block of 32 rows
+  const float* cpmax32 = nullptr;        // [n_ct * 8] max of cprefix over each aligned block of 32 rows
+  int32_t* counts = nullptr;             // [n_q] +=
+  unsigned long long* amb_count = nullptr;  // [n_qt] fill count of each query tile's region
+  int2* amb_pairs = nullptr;                // [n_qt][amb_cap]
+  unsigned long long amb_cap = 0;           // capacity of ONE region
+  float* dump = nullptr;                 // debug: write approximate scores [n_q][n_rows] instead of counting
+  const TcMeta* meta_a = nullptr;        // device: facts of the query image (this call)
+  const TcMeta* meta_b = nullptr;        // device: facts of the candidate image
+  int fp16 = 0;                          // operand format of the images: 1 = fp16, 0 = bf16 (set by launch_tc_scan)
+  float gamma = 0.f;                     // tc_gamma(k): multiplies |a| |b|
+  float gamma2 = 0.f;                    // tc_gamma2(k) (L2 only): multiplies (|a| + |b|)^2
+  float gamma_p = 0.f;                   // tc_gamma_p(): multiplies P(a) P(b) (accumulation inside the tensor core)
+  int l2 = 0;                            // 1: score = -(|a|^2 + |b|^2 - 2 a.b)
+  int n_kb = 0;
+  int k_total = 0;
+  int ct_group = 0;                      // candidate tiles a CTA walks per query tile (set by launch_tc_scan)
+  long long n_q = 0, n_rows = 0, n_qt = 0, n_ct = 0;
 };
+static_assert(std::is_trivially_copyable<TcScanParams>::value, "TcScanParams is a kernel parameter");
 
 // Rigorous bound eps >= |s_tc - s_ATen| used by the threshold test:
 //   dot models : eps = gamma  * |a| |b|

@@ -1170,22 +1170,24 @@ cudaError_t launch_ring_variant(const MarginStepParams& a, const TrainGrads& gr,
   return cudaGetLastError();
 }
 
-// KGE_TRAIN_BWD_BLOCKS=5 holds the backward kernel to 96 registers (5 CTAs = 20 warps per SM; the
-// unsharded margin step only)
+// One ring kernel per (loss kind, sharded).  KGE_TRAIN_BWD_BLOCKS=5 holds the backward kernel to 96
+// registers (5 CTAs = 20 warps per SM; the unsharded margin step only).
 template <int MODEL, bool BWD>
 cudaError_t launch_ring(const MarginStepParams& a, const TrainGrads& gr, const float* gloss, cudaStream_t st) {
-  if (a.loss_kind == KGE_LOSS_LOGISTIC)
-    return a.hrows ? launch_ring_variant<MODEL, BWD, 0, true, KGE_LOSS_LOGISTIC>(a, gr, gloss, st)
-                   : launch_ring_variant<MODEL, BWD, 0, false, KGE_LOSS_LOGISTIC>(a, gr, gloss, st);
-  if (a.loss_kind == KGE_LOSS_BCE)
-    return a.hrows ? launch_ring_variant<MODEL, BWD, 0, true, KGE_LOSS_BCE>(a, gr, gloss, st)
-                   : launch_ring_variant<MODEL, BWD, 0, false, KGE_LOSS_BCE>(a, gr, gloss, st);
-  if (a.hrows) return launch_ring_variant<MODEL, BWD, 0, true>(a, gr, gloss, st);
-  if constexpr (BWD) {
-    static const bool tight = [] { const char* v = getenv("KGE_TRAIN_BWD_BLOCKS"); return v && v[0] == '5'; }();
-    if (tight) return launch_ring_variant<MODEL, true, 5>(a, gr, gloss, st);
+  auto by_shard = [&](auto loss) -> cudaError_t {
+    constexpr int LOSS = decltype(loss)::value;
+    if (a.hrows) return launch_ring_variant<MODEL, BWD, 0, true, LOSS>(a, gr, gloss, st);
+    if constexpr (BWD && LOSS == KGE_LOSS_MARGIN) {
+      static const bool tight = [] { const char* v = getenv("KGE_TRAIN_BWD_BLOCKS"); return v && v[0] == '5'; }();
+      if (tight) return launch_ring_variant<MODEL, true, 5, false, LOSS>(a, gr, gloss, st);
+    }
+    return launch_ring_variant<MODEL, BWD, 0, false, LOSS>(a, gr, gloss, st);
+  };
+  switch (a.loss_kind) {
+    case KGE_LOSS_LOGISTIC: return by_shard(std::integral_constant<int, KGE_LOSS_LOGISTIC>{});
+    case KGE_LOSS_BCE: return by_shard(std::integral_constant<int, KGE_LOSS_BCE>{});
+    default: return by_shard(std::integral_constant<int, KGE_LOSS_MARGIN>{});
   }
-  return launch_ring_variant<MODEL, BWD, 0>(a, gr, gloss, st);
 }
 
 // margin_step_fast_kernel (the register-resident form, KGE_TRAIN_RING=0) has the margin loss only; the
@@ -1296,87 +1298,52 @@ cudaError_t launch_corrupt_batch(const int64_t* h, const int64_t* t, const int64
   return cudaGetLastError();
 }
 
-cudaError_t launch_margin_step_shard_fwd(const MarginStepParams& a, cudaStream_t st);
-cudaError_t launch_margin_step_shard_bwd(const MarginStepParams& a, const TrainGrads& gr, const float* gloss,
-                                         cudaStream_t st);
+namespace {
+// f(std::integral_constant<int, MODEL>{}) for the models of the ring and register-resident forms
+// (fast_step_ok)
+template <class F>
+cudaError_t with_fast_model(int model, F&& f) {
+  switch (model) {
+    case KGE_TRANSE_L1: return f(std::integral_constant<int, KGE_TRANSE_L1>{});
+    case KGE_TRANSE_L2: return f(std::integral_constant<int, KGE_TRANSE_L2>{});
+    default: return f(std::integral_constant<int, KGE_DISTMULT>{});
+  }
+}
+
+// The ring kernel where it applies; else, unsharded with the margin loss, the register-resident form;
+// else the generic kernels.  An entity-sharded step (a.hrows) that holds no rows scores no negative.
+template <bool BWD>
+cudaError_t launch_margin_step(const MarginStepParams& a, const TrainGrads& gr, const float* gloss,
+                               cudaStream_t st) {
+  const bool shard = a.hrows != nullptr;
+  if (a.b <= 0 || (shard && a.n_rows <= 0)) return cudaSuccess;
+  const unsigned blocks = blocks_for_warps(a.b);
+  if (fast_step_ok(a) && ring_step_ok(a))
+    return with_fast_model(a.model, [&](auto m) { return launch_ring<decltype(m)::value, BWD>(a, gr, gloss, st); });
+  if (!shard && fast_step_ok(a) && a.loss_kind == KGE_LOSS_MARGIN) {
+    return with_fast_model(a.model, [&](auto m) {
+      margin_step_fast_kernel<decltype(m)::value, BWD><<<blocks, WARPS_PER_BLOCK * 32, 0, st>>>(a, gr, gloss);
+      return cudaGetLastError();
+    });
+  }
+  if constexpr (BWD) {
+    if (shard) margin_step_shard_bwd_kernel<<<blocks, WARPS_PER_BLOCK * 32, 0, st>>>(a, gr, gloss);
+    else margin_step_bwd_kernel<<<blocks, WARPS_PER_BLOCK * 32, 0, st>>>(a, gr, gloss);
+  } else {
+    if (shard) margin_step_shard_fwd_kernel<<<blocks, WARPS_PER_BLOCK * 32, 0, st>>>(a);
+    else margin_step_fwd_kernel<<<blocks, WARPS_PER_BLOCK * 32, 0, st>>>(a);
+  }
+  return cudaGetLastError();
+}
+}  // namespace
 
 cudaError_t launch_margin_step_fwd(const MarginStepParams& a, cudaStream_t st) {
-  if (a.hrows) return launch_margin_step_shard_fwd(a, st);
-  if (a.b <= 0) return cudaSuccess;
-  if (fast_step_ok(a) && ring_step_ok(a)) {
-    const TrainGrads none{nullptr, nullptr, nullptr, nullptr};
-    switch (a.model) {
-      case KGE_TRANSE_L1: return launch_ring<KGE_TRANSE_L1, false>(a, none, nullptr, st);
-      case KGE_TRANSE_L2: return launch_ring<KGE_TRANSE_L2, false>(a, none, nullptr, st);
-      default: return launch_ring<KGE_DISTMULT, false>(a, none, nullptr, st);
-    }
-  }
-  if (fast_step_ok(a) && a.loss_kind == KGE_LOSS_MARGIN) {
-    const TrainGrads none{nullptr, nullptr, nullptr, nullptr};
-    const unsigned blocks = blocks_for_warps(a.b);
-    switch (a.model) {
-      case KGE_TRANSE_L1: margin_step_fast_kernel<KGE_TRANSE_L1, false><<<blocks, WARPS_PER_BLOCK * 32, 0, st>>>(a, none, nullptr); break;
-      case KGE_TRANSE_L2: margin_step_fast_kernel<KGE_TRANSE_L2, false><<<blocks, WARPS_PER_BLOCK * 32, 0, st>>>(a, none, nullptr); break;
-      default: margin_step_fast_kernel<KGE_DISTMULT, false><<<blocks, WARPS_PER_BLOCK * 32, 0, st>>>(a, none, nullptr); break;
-    }
-    return cudaGetLastError();
-  }
-  margin_step_fwd_kernel<<<blocks_for_warps(a.b), WARPS_PER_BLOCK * 32, 0, st>>>(a);
-  return cudaGetLastError();
-}
-
-// Entity-sharded step: the ring kernel's SHARD form where it applies, else the generic sharded kernels
-// (the register-resident form has no sharded variant).
-cudaError_t launch_margin_step_shard_fwd(const MarginStepParams& a, cudaStream_t st) {
-  if (a.b <= 0 || a.n_rows <= 0) return cudaSuccess;   // nothing held: no negative is scored here
-  if (fast_step_ok(a) && ring_step_ok(a)) {
-    const TrainGrads none{nullptr, nullptr, nullptr, nullptr};
-    switch (a.model) {
-      case KGE_TRANSE_L1: return launch_ring<KGE_TRANSE_L1, false>(a, none, nullptr, st);
-      case KGE_TRANSE_L2: return launch_ring<KGE_TRANSE_L2, false>(a, none, nullptr, st);
-      default: return launch_ring<KGE_DISTMULT, false>(a, none, nullptr, st);
-    }
-  }
-  margin_step_shard_fwd_kernel<<<blocks_for_warps(a.b), WARPS_PER_BLOCK * 32, 0, st>>>(a);
-  return cudaGetLastError();
-}
-
-cudaError_t launch_margin_step_shard_bwd(const MarginStepParams& a, const TrainGrads& gr, const float* gloss,
-                                         cudaStream_t st) {
-  if (a.b <= 0 || a.n_rows <= 0) return cudaSuccess;
-  if (fast_step_ok(a) && ring_step_ok(a)) {
-    switch (a.model) {
-      case KGE_TRANSE_L1: return launch_ring<KGE_TRANSE_L1, true>(a, gr, gloss, st);
-      case KGE_TRANSE_L2: return launch_ring<KGE_TRANSE_L2, true>(a, gr, gloss, st);
-      default: return launch_ring<KGE_DISTMULT, true>(a, gr, gloss, st);
-    }
-  }
-  margin_step_shard_bwd_kernel<<<blocks_for_warps(a.b), WARPS_PER_BLOCK * 32, 0, st>>>(a, gr, gloss);
-  return cudaGetLastError();
+  return launch_margin_step<false>(a, TrainGrads{nullptr, nullptr, nullptr, nullptr}, nullptr, st);
 }
 
 cudaError_t launch_margin_step_bwd(const MarginStepParams& a, const TrainGrads& gr, const float* gloss,
                                    cudaStream_t st) {
-  if (a.hrows) return launch_margin_step_shard_bwd(a, gr, gloss, st);
-  if (a.b <= 0) return cudaSuccess;
-  if (fast_step_ok(a) && ring_step_ok(a)) {
-    switch (a.model) {
-      case KGE_TRANSE_L1: return launch_ring<KGE_TRANSE_L1, true>(a, gr, gloss, st);
-      case KGE_TRANSE_L2: return launch_ring<KGE_TRANSE_L2, true>(a, gr, gloss, st);
-      default: return launch_ring<KGE_DISTMULT, true>(a, gr, gloss, st);
-    }
-  }
-  if (fast_step_ok(a) && a.loss_kind == KGE_LOSS_MARGIN) {
-    const unsigned blocks = blocks_for_warps(a.b);
-    switch (a.model) {
-      case KGE_TRANSE_L1: margin_step_fast_kernel<KGE_TRANSE_L1, true><<<blocks, WARPS_PER_BLOCK * 32, 0, st>>>(a, gr, gloss); break;
-      case KGE_TRANSE_L2: margin_step_fast_kernel<KGE_TRANSE_L2, true><<<blocks, WARPS_PER_BLOCK * 32, 0, st>>>(a, gr, gloss); break;
-      default: margin_step_fast_kernel<KGE_DISTMULT, true><<<blocks, WARPS_PER_BLOCK * 32, 0, st>>>(a, gr, gloss); break;
-    }
-    return cudaGetLastError();
-  }
-  margin_step_bwd_kernel<<<blocks_for_warps(a.b), WARPS_PER_BLOCK * 32, 0, st>>>(a, gr, gloss);
-  return cudaGetLastError();
+  return launch_margin_step<true>(a, gr, gloss, st);
 }
 
 cudaError_t launch_margin_loss_fwd(const float* pos, const float* neg, int64_t n, float margin,
