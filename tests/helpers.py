@@ -205,7 +205,12 @@ def rescal_prep_emulated(side, vec, M):
         for k in range(d):
             y = y + M[:, k] * T(k)
         return y
-    bounds = [0, d] if d <= 384 else [0, (d + 1) // 2, d]
+    bounds = [0]                       # K-blocks of 384 while more than 768 terms remain ...
+    while d > 384 and d - bounds[-1] > 768:
+        bounds.append(bounds[-1] + 384)
+    if d > 384:                        # ... then the last 385..768 terms as two chains
+        bounds.append(bounds[-1] + (d - bounds[-1] + 1) // 2)
+    bounds.append(d)
     parts = []
     for a, b in zip(bounds[:-1], bounds[1:]):
         acc = np.zeros(d, np.float32)

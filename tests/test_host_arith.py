@@ -75,7 +75,7 @@ def _aten(kind, q, c):
 
 
 @pytest.mark.parametrize("kind", sorted(KINDS))
-@pytest.mark.parametrize("d", [1, 7, 8, 13, 50, 64, 200, 203, 520, 1001])
+@pytest.mark.parametrize("d", [1, 7, 8, 13, 50, 64, 200, 203, 520, 1001, 1024, 2049, 4095, 4096, 8191])
 def test_device_arithmetic_equals_aten(kind, d, host_lib):
     el, model, qw, cw = KINDS[kind]
     g = torch.Generator().manual_seed(1000 * el + d)
@@ -102,20 +102,27 @@ def test_device_arithmetic_equals_aten(kind, d, host_lib):
         assert same.all(), "%s d=%d mode=%d: %d of %d scores differ" % (kind, d, mode, int((~same).sum()), same.numel())
 
 
-@pytest.mark.parametrize("d", [1, 2, 7, 13, 16, 19, 20, 21, 31, 32, 33, 50, 64, 100, 129, 200, 203, 256, 300, 384, 385, 400, 512])
+#: the head side sums K-blocks of 384 while more than 768 terms remain, then two chains: dims at
+#: and around every block boundary up to the library's limit
+RESCAL_PREP_DIMS = [1, 2, 7, 13, 16, 19, 20, 21, 31, 32, 33, 50, 64, 100, 129, 200, 203, 256, 300, 384, 385,
+                    400, 512, 767, 768, 769, 770, 1000, 1151, 1152, 1153, 1535, 1536, 1537, 1919, 2048, 2049,
+                    3000, 4096, 8191]
+
+
+@pytest.mark.parametrize("d", RESCAL_PREP_DIMS)
 def test_rescal_query_preparation_equals_the_reference_matmul(d, host_lib):
     """`matmul(h.view(b, 1, d), M)` and `matmul(M, t.view(b, d, 1))` (bilinear.py:108, 113) against
     the device function the prep kernel is made of -- bit for bit.  This pins the oneMKL / ATen
     summation order the kernel replays (batches of >= 2 facts: a batch of one takes MKL's gemv path,
     whose order depends on memory alignment)."""
     g = torch.Generator().manual_seed(d)
-    b = 3
+    b = 3 if d <= 4096 else 2            # d = 8191: 2 x 268 MB of matrices
     v = torch.randn(b, d, generator=g)
     M = torch.randn(b, d, d, generator=g)
     v[1, : d // 2] = 0.0
     want_tail = torch.matmul(v.view(b, 1, d), M).view(b, d)
     want_head = torch.matmul(M, v.view(b, d, 1)).view(b, d)
-    vn, Mn = v.numpy().copy(), M.numpy().copy()
+    vn, Mn = v.numpy(), M.numpy()        # contiguous views: no second copy of the matrices
     P = ctypes.c_void_p
     for tail, want in ((1, want_tail), (0, want_head)):
         out = np.full((b, d), np.nan, dtype=np.float32)

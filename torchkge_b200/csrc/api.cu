@@ -459,6 +459,8 @@ int kge_tc_pack_table_cached(int model, const float* ent0, const float* ent1, in
   if (n_rows <= 0) return KGE_OK;
   if (!ent0 || !tc_packed || (kge::elem_cw(el) >= 2 && !ent1))
     return fail(KGE_ERR_ARG, "kge_tc_pack_table: null pointer");
+  // an image no scan could read (kge_rank_side rejects the same dims)
+  if (!get_schedule(model, dim)) return fail(KGE_ERR_UNSUPPORTED, "kge_tc_pack_table: unsupported dim");
   DeviceScope device_scope(ent0);
   const int k_total = tc_k_total(el, dim);
   const int n_kb = kge::tc::n_kblocks(k_total);

@@ -328,14 +328,16 @@ __device__ float pair_score_natural(int dim, const float* __restrict__ q0, const
 // rounded separately) below that (contraction * rows * cols < 400).  The summation ORDER below was
 // recovered by probing torch 2.11 / oneMKL 2024.2 (AVX-512 code path) with absorption tests
 // (2^25, 1, -2^25 at three positions of the contraction) and confirmed bit for bit on random data
-// for every d in 1..512 (tests/test_host_arith.py replays this very function on the host):
+// for every d in 1..512 and for d up to 8191 at and around every K-block boundary
+// (tests/test_host_arith.py replays this very function on the host):
 //   tail  q_j = sum_k h_k M[k][j], columns j < 16*floor(d/16) (full 16-lane vectors):
 //           per chunk of 8 k:  y = fma(h6,M6,y); y = fma(h4,M4,y); y += fma(h5,M5,h7*M7);
 //                              y += fma(h0,M0,h2*M2) + fma(h1,M1,h3*M3);   then a plain fma chain
 //           over the d % 8 leftover k;  remainder columns: one fma chain over all k
-//   head  q_j = sum_k M[j][k] t_k: one fma chain over k for d <= 384, two chains over the halves
-//           [0, ceil(d/2)) and [ceil(d/2), d) added at the end for 385 <= d <= 768 (beyond that
-//           MKL's K-blocking was not probed: tolerance parity only)
+//   head  q_j = sum_k M[j][k] t_k: one fma chain over k for d <= 384; beyond, one fma chain per
+//           K-block of 384 from k = 0 while more than 768 terms remain, then the last a..d-1
+//           (385..768 terms) as two chains [a, m) and [m, d), m = a + ceil((d - a)/2); the chains
+//           are added left to right (d = 1000: [0,384) [384,692) [692,1000); d <= 768: the halves)
 // `vec` = h (tail) or t (head); M row-major (d, d).  A batch of exactly ONE fact takes a different
 // MKL path in the reference (sgemv with alignment-dependent peeling, not reproducible): documented.
 __device__ __forceinline__ float rescal_query_component(bool tail, int d, int j, const float* __restrict__ vec,
@@ -367,11 +369,17 @@ __device__ __forceinline__ float rescal_query_component(bool tail, int d, int j,
     } else if (d <= 384) {
       for (int k = 0; k < d; ++k) acc = __fmaf_rn(row[k], vec[k], acc);
     } else {
-      const int half = (d + 1) / 2;
-      float a1 = 0.f;
-      for (int k = 0; k < half; ++k) acc = __fmaf_rn(row[k], vec[k], acc);
-      for (int k = half; k < d; ++k) a1 = __fmaf_rn(row[k], vec[k], a1);
-      acc = __fadd_rn(acc, a1);
+      int a = 0;
+      for (; d - a > 768; a += 384) {   // K-blocks of 384 while more than 768 terms remain
+        float c = 0.f;
+        for (int k = a; k < a + 384; ++k) c = __fmaf_rn(row[k], vec[k], c);
+        acc = a == 0 ? c : __fadd_rn(acc, c);
+      }
+      const int mid = a + (d - a + 1) / 2;   // the last 385..768 terms: two chains
+      float c0 = 0.f, c1 = 0.f;
+      for (int k = a; k < mid; ++k) c0 = __fmaf_rn(row[k], vec[k], c0);
+      for (int k = mid; k < d; ++k) c1 = __fmaf_rn(row[k], vec[k], c1);
+      acc = __fadd_rn(a == 0 ? c0 : __fadd_rn(acc, c0), c1);
     }
   }
   return acc;
