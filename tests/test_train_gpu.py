@@ -119,9 +119,11 @@ def test_gradients_match_torch_autograd_of_the_oracle(kind, cuda_device):
 @pytest.mark.parametrize("kind", ["transe_l1", "transe_l2", "distmult"])
 @pytest.mark.parametrize("d", [200, 256, 36])
 def test_fast_fused_step_matches_oracle_autograd(kind, d, cuda_device):
-    """The register-resident fused step (csrc/train.cu: margin_step_fast_kernel; dim % 4 == 0,
-    dim <= 256): head- and tail-corrupted negatives mixed, a negative equal to the positive, a few
-    pairs with BOTH ends replaced (generic path inside the fast kernel), un-normalised weights."""
+    """The fused step of the single-plane models at dim % 4 == 0, dim <= 256 -- at n_neg = 40 the ring
+    kernel (csrc/train.cu: margin_step_ring_kernel; the register-resident margin_step_fast_kernel and the
+    ring past 48 KB are tests/test_train_paths_gpu.py's): head- and tail-corrupted negatives mixed, a
+    negative equal to the positive, a few pairs with BOTH ends replaced (the generic path inside the
+    kernel), un-normalised weights."""
     n_ent, n_rel, b, n_neg = 900, 7, 96, 40
     model = helpers.make_model(kind, d, n_ent, n_rel, seed=11)
     with torch.no_grad():

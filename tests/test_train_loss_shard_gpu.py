@@ -11,73 +11,13 @@ import torch
 import torchkge_b200 as tk
 from tests import gloo, helpers
 from torchkge_b200 import _lib
-from torchkge_b200.engine import CudaEngine, EntityShard, _exchanged_rows
-from torchkge_b200.training import ShardedStep, _kernel_dim, _MarginStep, _param_tensors, _row_spec, _training_code
+from torchkge_b200.engine import CudaEngine, EntityShard
 
 pytestmark = pytest.mark.gpu
 DEV = "cuda:0"
 ALL_KINDS = ["transe_l1", "transe_l2", "distmult", "rescal", "complex", "rotate", "analogy", "toruse_l1",
              "toruse_l2"]
 KINDS = {"logistic": _lib.LOSS_LOGISTIC, "bce": _lib.LOSS_BCE}
-
-
-def _close_grad(a, b, rtol=1e-4):
-    """as tests/test_train_gpu.py: rtol plus an absolute floor of 1e-5 of the largest entry"""
-    b = b.detach().cpu().float()
-    torch.testing.assert_close(a.detach().cpu().float(), b, rtol=rtol, atol=1e-5 * float(b.abs().max()) + 1e-9)
-
-
-def _leaves(model):
-    code = _training_code(model)
-    ts = [None if x is None else x.detach().clone().contiguous().requires_grad_(True)
-          for x in _param_tensors(model, code)]
-    return code, _kernel_dim(model, code), ts
-
-
-def unsharded(model, h, t, r, probs, loss_kind, n_neg, seed, offset):
-    code, dim, ts = _leaves(model)
-    loss = _MarginStep.apply(code, dim, model.n_ent, 0.0, n_neg, h, t, r, None, None, probs, seed, offset, *ts,
-                             loss_kind)
-    loss.backward()
-    return loss.item(), [None if x is None else x.grad for x in ts]
-
-
-def emulated(model, h, t, r, probs, loss_kind, n_neg, seed, offset, world, eng):
-    """What `world` ranks compute, one rank range after the other on one device (the all-reduces are
-    sums here), then every rank's scatter into its own rows."""
-    code, dim, ts = _leaves(model)
-    tabs = [None if x is None else x.detach() for x in ts]
-    n_ent, b = model.n_ent, h.shape[0]
-    full = ShardedStep(code, dim, n_ent, 0, n_ent, n_neg, 0.0, seed, offset, loss_kind)
-    rows = _exchanged_rows(_row_spec(full, tabs), torch.cat([h, t]), EntityShard(n_ent), eng)
-    hrows, trows = rows[:b], rows[b:]
-    loss = torch.zeros((), dtype=torch.float32, device=DEV)
-    grad_rows = torch.zeros_like(rows)
-    grel = [None if x is None else torch.zeros_like(x) for x in tabs[2:]]
-    gent = [None if x is None else torch.zeros_like(x) for x in tabs[:2]]
-    parts = []
-    for rank in range(world):
-        sh = EntityShard(n_ent, rank, world, local_storage=True)
-        n = sh.hi - sh.lo
-        local = [None if x is None else x.narrow(-2, sh.lo, n) for x in tabs[:2]] + tabs[2:]
-        lg = [None if x is None else x.narrow(-2, sh.lo, n) for x in gent]
-        parts.append((sh, lg))
-        if n == 0:
-            continue
-        step = ShardedStep(code, dim, n_ent, sh.lo, n, n_neg, 0.0, seed, offset, loss_kind)
-        loss += eng.margin_step_fwd(step, local, h, t, r, probs, hrows, trows)
-        g_rows = torch.zeros_like(rows)
-        g_rel = [None if x is None else torch.zeros_like(x) for x in tabs[2:]]
-        gl = torch.ones((), dtype=torch.float32, device=DEV)
-        eng.margin_step_bwd(step, local, lg + g_rel, h, t, r, probs, gl, hrows, trows, g_rows[:b], g_rows[b:])
-        grad_rows += g_rows
-        for a, c in zip(grel, g_rel):
-            if a is not None:
-                a += c
-    for sh, lg in parts:
-        if sh.hi > sh.lo:
-            eng.scatter_rows_add(code, dim, lg[0], lg[1], sh.lo, torch.cat([h, t]), grad_rows)
-    return loss.item(), gent + grel
 
 
 def _batch(n_ent, n_rel, b, seed):
@@ -89,22 +29,12 @@ def _batch(n_ent, n_rel, b, seed):
     return h.to(DEV), t.to(DEV), r.to(DEV), probs.to(DEV)
 
 
-def _model(kind, d, n_ent, n_rel, seed):
-    model = helpers.make_model(kind, d, n_ent, n_rel, seed=seed)
-    if kind in ("transe_l1", "transe_l2", "distmult", "rescal"):
-        with torch.no_grad():
-            model.ent_emb.weight.mul_(1.0 + torch.rand(n_ent, 1))   # un-normalised rows
-    if kind.startswith("toruse"):
-        model.normalize_parameters()
-    return model.to(DEV)
-
-
 def _compare(got, want, rtol=1e-4):
     (gl, gg), (wl, wg) = got, want
     assert gl == pytest.approx(wl, rel=1e-5, abs=1e-6)
     for a, b in zip(gg, wg):
         if b is not None:
-            _close_grad(a, b, rtol)
+            helpers.close_grad(a, b, rtol)
 
 
 # ---------------------------------------------------------------- 1. emulated shards vs unsharded
@@ -117,12 +47,12 @@ CASES = [(k, d, (1, 33, 256)[i % 3]) for i, (k, d) in enumerate(RING + GENERIC)]
 @pytest.mark.parametrize("kind,d,n_neg", CASES, ids=["%s-d%d-neg%d" % c for c in CASES])
 def test_emulated_shards_equal_unsharded(kind, d, n_neg, loss):
     n_ent, n_rel, b = 700, 40, 160
-    model = _model(kind, d, n_ent, n_rel, seed=3)
+    model = helpers.train_model(kind, d, n_ent, n_rel, seed=3)
     h, t, r, probs = _batch(n_ent, n_rel, b, seed=d + n_neg)
-    want = unsharded(model, h, t, r, probs, KINDS[loss], n_neg, 99, 5)
+    want = helpers.unsharded(model, h, t, r, probs, 0.0, n_neg, 99, 5, loss_kind=KINDS[loss])
     eng = CudaEngine()
     for world in (1, 2, 3, 8):
-        _compare(emulated(model, h, t, r, probs, KINDS[loss], n_neg, 99, 5, world, eng), want)
+        _compare(helpers.emulated(model, h, t, r, probs, 0.0, n_neg, 99, 5, world, eng, loss_kind=KINDS[loss]), want)
 
 
 @pytest.mark.parametrize("loss", sorted(KINDS))
@@ -131,13 +61,13 @@ def test_emulated_shards_equal_unsharded(kind, d, n_neg, loss):
 def test_empty_shards_and_one_sided_draws(kind, d, loss):
     """17 entities over 8 ranks (one row per rank or none), Bernoulli probabilities 0 and 1."""
     n_ent, n_rel, b, n_neg = 17, 4, 64, 33
-    model = _model(kind, d, n_ent, n_rel, seed=13)
+    model = helpers.train_model(kind, d, n_ent, n_rel, seed=13)
     h, t, r, _ = _batch(n_ent, n_rel, b, seed=14)
     probs = torch.tensor([0.0, 1.0, 0.5, 0.25], device=DEV)
-    want = unsharded(model, h, t, r, probs, KINDS[loss], n_neg, 7, 3)
+    want = helpers.unsharded(model, h, t, r, probs, 0.0, n_neg, 7, 3, loss_kind=KINDS[loss])
     eng = CudaEngine()
     for world in (2, 3, 8):
-        _compare(emulated(model, h, t, r, probs, KINDS[loss], n_neg, 7, 3, world, eng), want)
+        _compare(helpers.emulated(model, h, t, r, probs, 0.0, n_neg, 7, 3, world, eng, loss_kind=KINDS[loss]), want)
 
 
 # ---------------------------------------------------------------- 2. public API, two processes

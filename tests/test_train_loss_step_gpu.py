@@ -12,12 +12,10 @@ import pytest
 import torch
 
 import torchkge_b200 as tk
-from oracle import kge_oracle as oracle
 from tests import helpers
 from torchkge_b200 import _lib
 from torchkge_b200.engine import _ptr, _stream
-from torchkge_b200.training import (_kernel_dim, _MarginStep, _param_tensors, _training_code, fused_loss_step,
-                                    fused_margin_step, loss_kind_of)
+from torchkge_b200.training import _MarginStep, fused_loss_step, fused_margin_step, loss_kind_of
 
 pytestmark = pytest.mark.gpu
 DEV = "cuda:0"
@@ -25,25 +23,6 @@ ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 ALL_KINDS = ["transe_l1", "transe_l2", "distmult", "rescal", "complex", "rotate", "analogy", "toruse_l1",
              "toruse_l2"]
 LOSSES = {"logistic": (tk.LogisticLoss, _lib.LOSS_LOGISTIC), "bce": (tk.BinaryCrossEntropyLoss, _lib.LOSS_BCE)}
-
-
-def _close_grad(a, b, rtol=1e-4):
-    """as tests/test_train_gpu.py: rtol plus an absolute floor of 1e-5 of the largest entry"""
-    b = b.detach().cpu().float()
-    torch.testing.assert_close(a.detach().cpu().float(), b, rtol=rtol, atol=1e-5 * float(b.abs().max()) + 1e-9)
-
-
-def torch_loss(loss, pos, neg):
-    """utils/losses.py:47-112 restated with torch's own modules (pos already repeated n_neg times).
-    "logistic_stable": the same loss through softplus -- SoftMarginLoss evaluates log(1 + exp(-y x)) as
-    written and overflows to inf beyond |x| ~ 88, where the package's LogisticLoss, fused or not, is finite."""
-    if loss == "logistic_stable":
-        return torch.nn.functional.softplus(-pos).sum() + torch.nn.functional.softplus(neg).sum()
-    if loss == "logistic":
-        crit = torch.nn.SoftMarginLoss(reduction="sum")
-        return crit(pos, torch.ones_like(pos)) + crit(neg, -torch.ones_like(neg))
-    crit = torch.nn.BCELoss(reduction="sum")
-    return crit(torch.sigmoid(pos), torch.ones_like(pos)) + crit(torch.sigmoid(neg), torch.zeros_like(neg))
 
 
 # ---------------------------------------------------------------- 1. reference golden values
@@ -59,101 +38,21 @@ def test_fused_step_matches_reference_golden(case, loss):
     assert got.item() == pytest.approx(float(z["loss_" + loss]), rel=1e-5)
     got.backward()
     for name, p in model.named_parameters():
-        _close_grad(p.grad, torch.from_numpy(z["g_%s:%s" % (loss, name)]))
+        helpers.close_grad(p.grad, torch.from_numpy(z["g_%s:%s" % (loss, name)]))
 
 
 # ---------------------------------------------------------------- 2. every training kind vs CPU autograd
-def _leaves(model):
-    """The model's tables in ModelSpec order as fresh leaves (RotatE: the (cos, sin) planes; Analogy:
-    stacked (3, n, dim) tables)."""
-    code = _training_code(model)
-    ts = [None if x is None else x.detach().clone().contiguous().requires_grad_(True)
-          for x in _param_tensors(model, code)]
-    return code, _kernel_dim(model, code), ts
-
-
-def _torus_scores(kind, ent, rel, h, t, r):
-    """translation.py:706-720 with dissimilarities.py:28-43 (torus L1 / L2)."""
-    x = (torch.frac(ent[h]) + torch.frac(rel[r])) - torch.frac(ent[t])
-    if kind == "toruse_l1":
-        ax = x.abs()
-        return -(2 * torch.minimum(ax, 1 - ax)).sum(dim=1)
-    x2 = x * x
-    return -(4 * torch.minimum(x2, 1 - x2)).sum(dim=1)
-
-
-def cpu_pos_neg(kind, leaves, h, t, r, nh, nt):
-    """oracle.forward_pos_neg over CPU copies of the kernel's leaves (TorusE restated above)."""
-    e0, e1, r0, r1 = leaves
-    if kind.startswith("toruse"):
-        n_neg = nh.shape[0] // h.shape[0]
-        return (_torus_scores(kind, e0, r0, h, t, r).repeat(n_neg),
-                _torus_scores(kind, e0, r0, nh, nt, r.repeat(n_neg)))
-    if kind in ("transe_l1", "transe_l2", "distmult"):
-        P = {"ent": e0, "rel": r0}
-    elif kind == "rescal":
-        P = {"ent": e0, "rel_mat": r0}
-    elif kind == "analogy":
-        P = {"sc_ent": e0[0], "re_ent": e0[1], "im_ent": e0[2], "sc_rel": r0[0], "re_rel": r0[1], "im_rel": r0[2]}
-    else:
-        P = {"re_ent": e0, "im_ent": e1, "re_rel": r0, "im_rel": r1}
-    return oracle.forward_pos_neg(kind, P, h, t, r, nh, nt)
-
-
-def check_against_cpu(model, kind, loss, h, t, r, nh, nt, rtol=2e-4, ref=None):
-    """fused step on the GPU (external negatives) vs torch autograd on the CPU (torch_loss(ref or loss)),
-    same leaf tables."""
-    code, dim, ts = _leaves(model)
-    got = _MarginStep.apply(code, dim, model.n_ent, 0.0, nh.shape[0] // h.shape[0], h.to(DEV), t.to(DEV),
-                            r.to(DEV), nh.to(DEV), nt.to(DEV), None, 0, 0, *ts, LOSSES[loss][1])
-    got.backward()
-    cpu = [None if x is None else x.detach().cpu().clone().requires_grad_(True) for x in ts]
-    pos, neg = cpu_pos_neg(kind, cpu, h.cpu(), t.cpu(), r.cpu(), nh.cpu(), nt.cpu())
-    want = torch_loss(ref or loss, pos, neg)
-    want.backward()
-    assert got.item() == pytest.approx(want.item(), rel=2e-5)
-    for a, b in zip(ts, cpu):
-        if a is not None:
-            _close_grad(a.grad, b.grad, rtol)
-    return ts, cpu
-
-
-def _model(kind, d, n_ent, n_rel, seed):
-    model = helpers.make_model(kind, d, n_ent, n_rel, seed=seed)
-    if kind in ("transe_l1", "transe_l2", "distmult", "rescal"):
-        with torch.no_grad():
-            model.ent_emb.weight.mul_(1.0 + torch.rand(n_ent, 1))   # un-normalised rows
-    if kind.startswith("toruse"):
-        model.normalize_parameters()
-    return model.to(DEV)
-
-
-def _negatives(h, t, n_ent, n_neg, gen):
-    """Head and tail corruption mixed, a negative equal to its positive, a few with both ends replaced."""
-    b = h.shape[0]
-    nh, nt = h.repeat(n_neg), t.repeat(n_neg)
-    which = torch.rand(b * n_neg, generator=gen) < 0.45
-    rnd = torch.randint(1, n_ent, (b * n_neg,), generator=gen)
-    nh = torch.where(which, rnd, nh)
-    nt = torch.where(~which, rnd, nt)
-    nt[0], nh[0] = t[0], h[0]
-    both = torch.arange(7, b * n_neg, 97)
-    nh[both] = (h.repeat(n_neg)[both] + 3) % n_ent
-    nt[both] = (t.repeat(n_neg)[both] + 5) % n_ent
-    return nh, nt
-
-
 @pytest.mark.parametrize("loss", sorted(LOSSES))
 @pytest.mark.parametrize("kind", ALL_KINDS)
 def test_every_kind_matches_cpu_autograd(kind, loss):
     n_ent, n_rel, b, n_neg = 300, 6, 64, 5
     d = 12 if kind == "rescal" else 40
-    model = _model(kind, d, n_ent, n_rel, seed=4)
+    model = helpers.train_model(kind, d, n_ent, n_rel, seed=4)
     gen = torch.Generator().manual_seed(6)
     h, t = torch.randint(0, n_ent, (b,), generator=gen), torch.randint(0, n_ent, (b,), generator=gen)
     r = torch.randint(0, n_rel, (b,), generator=gen)
-    nh, nt = _negatives(h, t, n_ent, n_neg, gen)
-    check_against_cpu(model, kind, loss, h, t, r, nh, nt)
+    nh, nt = helpers.negatives(h, t, n_ent, n_neg, gen)
+    helpers.check_against_cpu(model, kind, loss, h, t, r, nh, nt)
 
 
 # ---------------------------------------------------------------- 3. the ring kernel's shapes
@@ -168,13 +67,13 @@ def test_ring_shapes_match_cpu_autograd(kind, d, n_neg, source, loss):
     """External negatives (mixed sides, one equal to its positive, some with both ends replaced) and
     Philox draws (the ring's own draw loop; the CPU side gets kge_corrupt_batch's negatives)."""
     n_ent, n_rel, b = 900, 7, 96
-    model = _model(kind, d, n_ent, n_rel, seed=11)
+    model = helpers.train_model(kind, d, n_ent, n_rel, seed=11)
     gen = torch.Generator().manual_seed(d + n_neg)
     h, t = torch.randint(0, n_ent, (b,), generator=gen), torch.randint(0, n_ent, (b,), generator=gen)
     r = torch.randint(0, n_rel, (b,), generator=gen)
     if source == "external":
-        nh, nt = _negatives(h, t, n_ent, n_neg, gen)
-        check_against_cpu(model, kind, loss, h, t, r, nh, nt)
+        nh, nt = helpers.negatives(h, t, n_ent, n_neg, gen)
+        helpers.check_against_cpu(model, kind, loss, h, t, r, nh, nt)
         return
     probs = torch.rand(n_rel, generator=gen).to(DEV)
     hd, td, rd = h.to(DEV), t.to(DEV), r.to(DEV)
@@ -182,18 +81,18 @@ def test_ring_shapes_match_cpu_autograd(kind, d, n_neg, source, loss):
     nt = torch.empty_like(nh)
     _lib.check(_lib.load().kge_corrupt_batch(_ptr(hd), _ptr(td), _ptr(rd), b, n_neg, _ptr(probs), n_ent, 31, 2,
                                              _ptr(nh), _ptr(nt), _stream(hd.device)), "kge_corrupt_batch")
-    code, dim, ts = _leaves(model)
+    code, dim, ts = helpers.train_leaves(model)
     got = _MarginStep.apply(code, dim, n_ent, 0.0, n_neg, hd, td, rd, None, None, probs, 31, 2, *ts,
                             LOSSES[loss][1])
     got.backward()
     cpu = [None if x is None else x.detach().cpu().clone().requires_grad_(True) for x in ts]
-    pos, neg = cpu_pos_neg(kind, cpu, h, t, r, nh.cpu(), nt.cpu())
-    want = torch_loss(loss, pos, neg)
+    pos, neg = helpers.cpu_pos_neg(kind, cpu, h, t, r, nh.cpu(), nt.cpu())
+    want = helpers.torch_loss(loss, pos, neg)
     want.backward()
     assert got.item() == pytest.approx(want.item(), rel=2e-5)
     for a, c in zip(ts, cpu):
         if a is not None:
-            _close_grad(a.grad, c.grad, rtol=2e-4)
+            helpers.close_grad(a.grad, c.grad, rtol=2e-4)
 
 
 # ---------------------------------------------------------------- 4. saturated sigmoids
@@ -220,14 +119,14 @@ def test_saturated_scores(kind, d, loss):
     gen = torch.Generator().manual_seed(22)
     h, t = torch.randint(0, n_ent, (b,), generator=gen), torch.randint(0, n_ent, (b,), generator=gen)
     r = torch.randint(0, n_rel, (b,), generator=gen)
-    nh, nt = _negatives(h, t, n_ent, n_neg, gen)
+    nh, nt = helpers.negatives(h, t, n_ent, n_neg, gen)
     with torch.no_grad():
-        code, dim, ts = _leaves(model)
-        pos, neg = cpu_pos_neg(kind, [None if x is None else x.cpu() for x in ts], h, t, r, nh, nt)
+        code, dim, ts = helpers.train_leaves(model)
+        pos, neg = helpers.cpu_pos_neg(kind, [None if x is None else x.cpu() for x in ts], h, t, r, nh, nt)
     sat = r.repeat(n_neg) > 0
     assert (pos[sat].abs() > 100).all() and (neg[sat].abs() > 100).all()
     assert (pos[~sat].abs() < 20).all()
-    ts, cpu = check_against_cpu(model, kind, loss, h, t, r, nh, nt,
+    ts, cpu = helpers.check_against_cpu(model, kind, loss, h, t, r, nh, nt,
                                 ref="logistic_stable" if loss == "logistic" else None)
     for a, c in zip(ts, cpu):
         if a is not None:
@@ -258,7 +157,7 @@ def test_sampler_fused_step_equals_three_calls(loss):
     model.zero_grad()
     fused.backward()
     for n, p in model.named_parameters():
-        _close_grad(p.grad, g1[n])
+        helpers.close_grad(p.grad, g1[n])
 
 
 class MarginLoss(torch.nn.Module):
@@ -272,7 +171,7 @@ class MarginLoss(torch.nn.Module):
 @pytest.mark.parametrize("crit", ["package", "torchkge"])
 def test_margin_criterion_equals_fused_margin_step(crit):
     n_ent, n_rel, d, b = 500, 5, 200, 128
-    model = _model("distmult", d, n_ent, n_rel, seed=2)
+    model = helpers.train_model("distmult", d, n_ent, n_rel, seed=2)
     gen = torch.Generator().manual_seed(3)
     h, t = torch.randint(0, n_ent, (b,), generator=gen).to(DEV), torch.randint(0, n_ent, (b,), generator=gen).to(DEV)
     r = torch.randint(0, n_rel, (b,), generator=gen).to(DEV)
@@ -287,7 +186,7 @@ def test_margin_criterion_equals_fused_margin_step(crit):
     got.backward()
     assert got.item() == pytest.approx(want.item(), rel=1e-6)
     for n, p in model.named_parameters():
-        _close_grad(p.grad, g1[n])
+        helpers.close_grad(p.grad, g1[n])
 
 
 # ---------------------------------------------------------------- 6. ABI and argument errors

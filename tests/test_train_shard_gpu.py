@@ -14,78 +14,14 @@ import torchkge_b200 as tk
 from oracle import kge_oracle as oracle
 from tests import gloo, helpers
 from torchkge_b200 import _lib
-from torchkge_b200.engine import CudaEngine, EntityShard, _exchanged_rows, _ptr, _stream
-from torchkge_b200.training import (ShardedStep, _kernel_dim, _MarginStep, _param_tensors, _row_spec,
-                                    _training_code)
+from torchkge_b200.engine import CudaEngine, EntityShard, _ptr, _stream
+from torchkge_b200.training import _MarginStep
 
 pytestmark = pytest.mark.gpu
 DEV = "cuda:0"
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 ALL_KINDS = ["transe_l1", "transe_l2", "distmult", "rescal", "complex", "rotate", "analogy", "toruse_l1",
              "toruse_l2"]
-
-
-def _close_grad(a, b, rtol=1e-4):
-    """as tests/test_train_gpu.py: rtol plus an absolute floor of 1e-5 of the largest entry"""
-    b = b.detach().cpu().float()
-    torch.testing.assert_close(a.detach().cpu().float(), b, rtol=rtol, atol=1e-5 * float(b.abs().max()) + 1e-9)
-
-
-def _leaves(model):
-    """The model's tables in ModelSpec order as fresh leaves (RotatE: the (cos, sin) planes)."""
-    code = _training_code(model)
-    ts = [None if x is None else x.detach().clone().contiguous().requires_grad_(True)
-          for x in _param_tensors(model, code)]
-    return code, _kernel_dim(model, code), ts
-
-
-def unsharded(model, h, t, r, probs, margin, n_neg, seed, offset):
-    """(loss, [grad tables]) of the existing fused step on the whole table."""
-    code, dim, ts = _leaves(model)
-    loss = _MarginStep.apply(code, dim, model.n_ent, margin, n_neg, h, t, r, None, None, probs, seed, offset, *ts)
-    loss.backward()
-    return loss.item(), [None if x is None else x.grad for x in ts]
-
-
-def emulated(model, h, t, r, probs, margin, n_neg, seed, offset, world, eng):
-    """What `world` ranks compute, one rank range after the other on one device: the loss, the
-    relation gradients and grad_hrows / grad_trows summed over the ranks (the all-reduces), then
-    every rank's scatter into its own rows."""
-    code, dim, ts = _leaves(model)
-    tabs = [None if x is None else x.detach() for x in ts]
-    n_ent, b = model.n_ent, h.shape[0]
-    full = ShardedStep(code, dim, n_ent, 0, n_ent, n_neg, float(margin), seed, offset)
-    rows = _exchanged_rows(_row_spec(full, tabs), torch.cat([h, t]), EntityShard(n_ent), eng)
-    hrows, trows = rows[:b], rows[b:]
-    loss = torch.zeros((), dtype=torch.float32, device=DEV)
-    grad_rows = torch.zeros_like(rows)
-    grel = [None if x is None else torch.zeros_like(x) for x in tabs[2:]]
-    gent = [None if x is None else torch.zeros_like(x) for x in tabs[:2]]
-    parts = []
-    for rank in range(world):
-        sh = EntityShard(n_ent, rank, world, local_storage=True)
-        n = sh.hi - sh.lo
-        # every rank's entity rows and entity gradient are views of rows [lo, hi) of one table (a
-        # three-plane table keeps its planes equally spaced)
-        local = [None if x is None else x.narrow(-2, sh.lo, n) for x in tabs[:2]] + tabs[2:]
-        lg = [None if x is None else x.narrow(-2, sh.lo, n) for x in gent]
-        parts.append((sh, lg))
-        if n == 0:
-            continue
-        step = ShardedStep(code, dim, n_ent, sh.lo, n, n_neg, float(margin), seed, offset)
-        loss += eng.margin_step_fwd(step, local, h, t, r, probs, hrows, trows)
-        g_rows = torch.zeros_like(rows)
-        g_rel = [None if x is None else torch.zeros_like(x) for x in tabs[2:]]
-        gl = torch.ones((), dtype=torch.float32, device=DEV)
-        eng.margin_step_bwd(step, local, lg + g_rel, h, t, r, probs, gl, hrows, trows, g_rows[:b], g_rows[b:])
-        grad_rows += g_rows
-        for a, c in zip(grel, g_rel):
-            if a is not None:
-                a += c
-    for sh, lg in parts:          # after the all-reduce: every rank adds the rows it holds
-        if sh.hi > sh.lo:
-            eng.scatter_rows_add(code, dim, lg[0], lg[1], sh.lo, torch.cat([h, t]), grad_rows)
-    return loss.item(), gent + grel
 
 
 def _batch(n_ent, n_rel, b, seed):
@@ -97,22 +33,12 @@ def _batch(n_ent, n_rel, b, seed):
     return h.to(DEV), t.to(DEV), r.to(DEV), probs.to(DEV)
 
 
-def _model(kind, d, n_ent, n_rel, seed):
-    model = helpers.make_model(kind, d, n_ent, n_rel, seed=seed)
-    if kind in ("transe_l1", "transe_l2", "distmult", "rescal"):
-        with torch.no_grad():
-            model.ent_emb.weight.mul_(1.0 + torch.rand(n_ent, 1))   # un-normalised rows
-    if kind.startswith("toruse"):
-        model.normalize_parameters()
-    return model.to(DEV)
-
-
 def _compare(got, want, rtol=1e-4):
     (gl, gg), (wl, wg) = got, want
     assert gl == pytest.approx(wl, rel=1e-5, abs=1e-6)
     for a, b in zip(gg, wg):
         if b is not None:
-            _close_grad(a, b, rtol)
+            helpers.close_grad(a, b, rtol)
 
 
 # ---------------------------------------------------------------- 1. emulated shards vs unsharded
@@ -126,20 +52,20 @@ def test_emulated_shards_equal_unsharded(kind, d, n_neg):
     # 40 relations: a relation row sums ~b n_neg / 40 hinge terms, which keeps the atomics-order noise of
     # the relation gradients inside the rtol of the rule
     n_ent, n_rel, b = 700, 40, 160
-    model = _model(kind, d, n_ent, n_rel, seed=3)
+    model = helpers.train_model(kind, d, n_ent, n_rel, seed=3)
     h, t, r, probs = _batch(n_ent, n_rel, b, seed=d + n_neg)
     margin = 1.0 if kind not in ("transe_l1", "transe_l2") else 0.3
-    want = unsharded(model, h, t, r, probs, margin, n_neg, 99, 5)
+    want = helpers.unsharded(model, h, t, r, probs, margin, n_neg, 99, 5)
     eng = CudaEngine()
     for world in (1, 2, 3, 8):
-        _compare(emulated(model, h, t, r, probs, margin, n_neg, 99, 5, world, eng), want)
+        _compare(helpers.emulated(model, h, t, r, probs, margin, n_neg, 99, 5, world, eng), want)
 
 
 @pytest.mark.parametrize("kind,d", [("distmult", 200), ("transe_l2", 36), ("complex", 50), ("rotate", 64)])
 def test_emulated_shards_equal_oracle_autograd(kind, d):
     """Against the oracle's CPU autograd on the negatives kge_corrupt_batch draws at the same seed / offset."""
     n_ent, n_rel, b, n_neg, seed, offset = 500, 5, 96, 33, 4242, 17
-    model = _model(kind, d, n_ent, n_rel, seed=8)
+    model = helpers.train_model(kind, d, n_ent, n_rel, seed=8)
     h, t, r, probs = _batch(n_ent, n_rel, b, seed=9)
     nh = torch.empty(b * n_neg, dtype=torch.int64, device=DEV)
     nt = torch.empty_like(nh)
@@ -154,11 +80,11 @@ def test_emulated_shards_equal_oracle_autograd(kind, d):
     want = (ref.item(), [None if k is None else P[k].grad for k in keys])
     eng = CudaEngine()
     for world in (2, 3, 8):
-        got = emulated(model, h, t, r, probs, 1.0, n_neg, seed, offset, world, eng)
+        got = helpers.emulated(model, h, t, r, probs, 1.0, n_neg, seed, offset, world, eng)
         assert got[0] == pytest.approx(want[0], rel=2e-5)
         for a, c in zip(got[1], want[1]):
             if c is not None:
-                _close_grad(a, c, rtol=2e-4)
+                helpers.close_grad(a, c, rtol=2e-4)
 
 
 # ---------------------------------------------------------------- 2. hard cases
@@ -170,7 +96,7 @@ HARD = [("distmult", 200), ("transe_l1", 36), ("complex", 50), ("analogy", 64), 
 def test_hard_cases(kind, d, case):
     n_rel, b, n_neg = 4, 64, 33
     n_ent = {"empty_shards": 5, "tiny": 17}.get(case, 300)
-    model = _model(kind, d, n_ent, n_rel, seed=13)
+    model = helpers.train_model(kind, d, n_ent, n_rel, seed=13)
     h, t, r, _ = _batch(n_ent, n_rel, b, seed=14)
     probs = torch.tensor([0.0, 1.0, 0.5, 0.25], device=DEV)    # Bernoulli 0 and 1: one side only
     if case == "self_loops":
@@ -178,10 +104,10 @@ def test_hard_cases(kind, d, case):
     if case == "one_owner":                 # every positive held by rank 0 of 8 (rows [0, 38))
         h, t = h % 38, t % 38
     # tiny n_ent: most draws hit a shard's first or last row and many negatives equal their positive
-    want = unsharded(model, h, t, r, probs, 1.0, n_neg, 7, 3)
+    want = helpers.unsharded(model, h, t, r, probs, 1.0, n_neg, 7, 3)
     eng = CudaEngine()
     for world in (2, 3, 8):
-        _compare(emulated(model, h, t, r, probs, 1.0, n_neg, 7, 3, world, eng), want)
+        _compare(helpers.emulated(model, h, t, r, probs, 1.0, n_neg, 7, 3, world, eng), want)
 
 
 # ---------------------------------------------------------------- 3. kge_scatter_rows_add
@@ -255,9 +181,9 @@ def test_sharded_argument_errors():
 
 def test_legacy_calls_still_accept_their_arguments():
     """hrows == NULL: external negatives and every optional output, as before."""
-    model = _model("distmult", 36, 100, 3, seed=1)
+    model = helpers.train_model("distmult", 36, 100, 3, seed=1)
     h, t, r, probs = _batch(100, 3, 8, seed=1)
-    code, dim, ts = _leaves(model)
+    code, dim, ts = helpers.train_leaves(model)
     tabs = [None if x is None else x.detach() for x in ts]
     nh, nt = h.repeat(2), (t.repeat(2) + 1) % 100
     out = [torch.zeros(16, device=DEV), torch.zeros(8, device=DEV)]

@@ -501,7 +501,7 @@ __global__ void margin_step_bwd_kernel(MarginStepParams a, TrainGrads gr, const 
   const RowPtrs pp = make_rows(a.model, a.dim, a.tb, hi, ti, ri);
   const float pos = triple_score(a.model, a.dim, pp, lane, nullptr, nullptr);
   const float p_head = a.nh ? 0.f : a.probs[ri];
-  float gpos_sum = 0.f;
+  double gpos_sum = 0.0;   // thousands of non-integer dl/dpos terms (logistic, BCE): fp32 would drift
   for (int j = 0; j < a.n_neg; ++j) {
     const long long idx = (long long)j * a.b + w;
     long long nh, nt;
@@ -514,7 +514,7 @@ __global__ void margin_step_bwd_kernel(MarginStepParams a, TrainGrads gr, const 
     gpos_sum += gp;
     triple_backward(a.model, a.dim, pn, grad_rows(a.model, a.dim, gr, nh, nt, ri), g * gn, lane);
   }
-  triple_backward(a.model, a.dim, pp, grad_rows(a.model, a.dim, gr, hi, ti, ri), g * gpos_sum, lane);
+  triple_backward(a.model, a.dim, pp, grad_rows(a.model, a.dim, gr, hi, ti, ri), g * (float)gpos_sum, lane);
 }
 
 // Entity-sharded fused step (a.hrows set), one warp per positive.  Every rank runs the same draws;
@@ -579,7 +579,7 @@ __global__ void margin_step_shard_bwd_kernel(MarginStepParams a, TrainGrads gr, 
   const Planes<float> gh = buf_planes(a.grad_hrows, np, a.dim, w);
   const Planes<float> gt = buf_planes(a.grad_trows, np, a.dim, w);
   const Planes<float> grel = rel_planes(a.model, a.dim, gr.rel0, gr.rel1, ri);
-  float gpos_sum = 0.f;
+  double gpos_sum = 0.0;   // as in margin_step_bwd_kernel
   for (int j = 0; j < a.n_neg; ++j) {
     bool head;
     long long loc;
@@ -592,7 +592,7 @@ __global__ void margin_step_shard_bwd_kernel(MarginStepParams a, TrainGrads gr, 
     const Planes<float> ge = table_planes(gr.ent0, gr.ent1, np, (size_t)loc * a.dim);
     triple_backward(a.model, a.dim, pn, grads_of(head ? ge : gh, head ? gt : ge, grel), g * gn, lane);
   }
-  triple_backward(a.model, a.dim, pp, grads_of(gh, gt, grel), g * gpos_sum, lane);
+  triple_backward(a.model, a.dim, pp, grads_of(gh, gt, grel), g * (float)gpos_sum, lane);
 }
 
 // ------------------------------------------------------------------------------------------
@@ -1001,10 +1001,11 @@ margin_step_ring_kernel(MarginStepParams a, TrainGrads gr, const float* __restri
   Vec Vt, Vh;
 #pragma unroll
   for (int i = 0; i < FAST_NCH; ++i) Vt.c[i] = Vh.c[i] = make_float4(0.f, 0.f, 0.f, 0.f);
-  // per kind: the active hinges (margin) or the summed weights c_j
-  using Count = std::conditional_t<LOSS == KGE_LOSS_MARGIN, int, float>;
+  // per kind: the active hinges (margin) or the summed weights c_j.  The weights and dl/dpos are
+  // non-integers summed over up to thousands of negatives: in double, as fp32 would drift by ~n eps.
+  using Count = std::conditional_t<LOSS == KGE_LOSS_MARGIN, int, double>;
   Count n_t = 0, n_h = 0;
-  float gpos_sum = 0.f;   // LOSS != margin: sum of dl/dpos over the ring's negatives
+  double gpos_sum = 0.0;   // LOSS != margin: sum of dl/dpos over the ring's negatives
   unsigned phases = 0u;   // bit s = parity of the next completion of slot s (a skipped use does not advance it)
   for (int j = 0; j < n_loop; ++j) {
     const unsigned code = codes[j];
@@ -1107,11 +1108,11 @@ margin_step_ring_kernel(MarginStepParams a, TrainGrads gr, const float* __restri
   if constexpr (LOSS == KGE_LOSS_MARGIN) {
     if (n_t + n_h == 0) return;
   } else {
-    if (n_t == 0.f && n_h == 0.f && gpos_sum == 0.f) return;
+    if (n_t == 0.0 && n_h == 0.0 && gpos_sum == 0.0) return;
   }
   // fn: the positive's weight, -sum_j dl/dpos (the margin loss: the active count)
   const float fn_t = (float)n_t, fn_h = (float)n_h;
-  const float fn = LOSS == KGE_LOSS_MARGIN ? (float)(n_t + n_h) : -gpos_sum;
+  const float fn = LOSS == KGE_LOSS_MARGIN ? (float)(n_t + n_h) : (float)-gpos_sum;
   Vec Gh, Gt, Gr;
   if constexpr (MODEL == KGE_DISTMULT) {
     Gh = vec_map3(r, Vt, tn, [=](float rr, float vt, float tt) { return g * rr * (vt - fn * tt); });
