@@ -12,7 +12,7 @@ with CUDA events after warm-up; every figure is the median of --windows windows 
    another (the maximum over the ranks and the sum; collectives not run);
 4. the fused and three-call losses at the same seed and offset, each also against a float64 sum of the
    per-pair terms of the three-call scores (both are fp32 sums of 8.4M terms in atomics order);
-5. with --parent-lib (a libkge_b200.so built from the parent commit, ABI 10): the margin forward +
+5. with --parent-lib (a libkge_b200.so built from the parent commit, same ABI): the margin forward +
    backward of both libraries on the same arguments, alternating window by window.
 Records the GPU name, power limit and SM clock in the same run.
 """
@@ -219,8 +219,8 @@ def main():
         parent.kge_margin_step_bwd.argtypes = [ctypes.POINTER(_lib.MarginStepArgs), ctypes.POINTER(_lib.Grads),
                                                ctypes.c_void_p]
         parent.kge_last_error.restype = ctypes.c_char_p
-        assert parent.kge_abi_version() == 10, parent.kge_abi_version()
-        a, gr = built["margin"]          # ABI 10 reads the same fields, without the trailing loss_kind
+        assert parent.kge_abi_version() == lib.kge_abi_version(), parent.kge_abi_version()
+        a, gr = built["margin"]
         cmp_ = timed({"parent_fwd": fwd(parent, a), "this_fwd": fwd(lib, a),
                       "parent_fwd_bwd": fwd_bwd(parent, a, gr), "this_fwd_bwd": fwd_bwd(lib, a, gr)},
                      args.reps, max(args.windows, 7))

@@ -884,7 +884,8 @@ int kge_margin_loss_fwd(const float* pos, const float* neg, int64_t n, float mar
   if (n == 0) return KGE_OK;
   if (n < 0 || !pos || !neg || !loss) return fail(KGE_ERR_ARG, "kge_margin_loss_fwd: bad argument");
   DeviceScope device_scope(pos);
-  KGE_CUDA_TRY(kge::launch_margin_loss_fwd(pos, neg, n, margin, loss, static_cast<cudaStream_t>(stream)),
+  KGE_CUDA_TRY(kge::launch_pair_loss_fwd(KGE_LOSS_MARGIN, margin, pos, neg, n, loss,
+                                         static_cast<cudaStream_t>(stream)),
                "margin_loss_fwd");
   return KGE_OK;
 }
@@ -895,8 +896,8 @@ int kge_margin_loss_bwd(const float* pos, const float* neg, int64_t n, float mar
   if (n < 0 || !pos || !neg || !grad_loss || !grad_pos || !grad_neg)
     return fail(KGE_ERR_ARG, "kge_margin_loss_bwd: bad argument");
   DeviceScope device_scope(pos);
-  KGE_CUDA_TRY(kge::launch_margin_loss_bwd(pos, neg, n, margin, grad_loss, grad_pos, grad_neg,
-                                           static_cast<cudaStream_t>(stream)),
+  KGE_CUDA_TRY(kge::launch_pair_loss_bwd(KGE_LOSS_MARGIN, margin, pos, neg, n, grad_loss, grad_pos, grad_neg,
+                                         static_cast<cudaStream_t>(stream)),
                "margin_loss_bwd");
   return KGE_OK;
 }
@@ -906,7 +907,7 @@ int kge_pair_loss_fwd(int kind, const float* pos, const float* neg, int64_t n, f
   if (n == 0) return KGE_OK;
   if (n < 0 || !pos || !neg || !loss) return fail(KGE_ERR_ARG, "kge_pair_loss_fwd: bad argument");
   DeviceScope device_scope(pos);
-  KGE_CUDA_TRY(kge::launch_pair_loss_fwd(kind, pos, neg, n, loss, static_cast<cudaStream_t>(stream)),
+  KGE_CUDA_TRY(kge::launch_pair_loss_fwd(kind, 0.f, pos, neg, n, loss, static_cast<cudaStream_t>(stream)),
                "pair_loss_fwd");
   return KGE_OK;
 }
@@ -918,7 +919,7 @@ int kge_pair_loss_bwd(int kind, const float* pos, const float* neg, int64_t n, c
   if (n < 0 || !pos || !neg || !grad_loss || !grad_pos || !grad_neg)
     return fail(KGE_ERR_ARG, "kge_pair_loss_bwd: bad argument");
   DeviceScope device_scope(pos);
-  KGE_CUDA_TRY(kge::launch_pair_loss_bwd(kind, pos, neg, n, grad_loss, grad_pos, grad_neg,
+  KGE_CUDA_TRY(kge::launch_pair_loss_bwd(kind, 0.f, pos, neg, n, grad_loss, grad_pos, grad_neg,
                                          static_cast<cudaStream_t>(stream)),
                "pair_loss_bwd");
   return KGE_OK;

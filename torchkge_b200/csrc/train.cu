@@ -83,13 +83,18 @@ __device__ __forceinline__ void corrupt_one(uint64_t seed, uint64_t offset, uint
 
 // ------------------------------------------------------------------------------------------
 // Per-lane view of one triple.  Lane l owns embedding indices l, l+32, ...; `cnt` of them.
+// RowPtrs: the rows it is scored from.  GradRows: the destination rows of its gradient, plane by
+// plane, in the same layout.
 // ------------------------------------------------------------------------------------------
-struct RowPtrs {
-  const float* h0; const float* h1;  // head planes
-  const float* t0; const float* t1;  // tail planes
-  const float* r0; const float* r1;  // relation planes (RESCAL: r0 = matrix)
-  const float* h2; const float* t2; const float* r2;  // third planes (Analogy) or nullptr
+template <class T>
+struct Rows {
+  T* h0; T* h1;  // head planes
+  T* t0; T* t1;  // tail planes
+  T* r0; T* r1;  // relation planes (RESCAL: r0 = matrix)
+  T* h2; T* t2; T* r2;  // third planes (Analogy) or nullptr
 };
+using RowPtrs = Rows<const float>;
+using GradRows = Rows<float>;
 
 __device__ __forceinline__ float inv_norm_of(const float* row, int dim, int lane) {
   float s = 0.f;
@@ -164,58 +169,9 @@ __device__ float triple_score(int model, int dim, const RowPtrs& p, int lane, fl
   }
 }
 
-__device__ __forceinline__ RowPtrs make_rows(int model, int dim, const TrainTables& tb, long long h,
-                                             long long t, long long r) {
-  RowPtrs p;
-  p.h0 = tb.ent0 + (size_t)h * dim;
-  p.t0 = tb.ent0 + (size_t)t * dim;
-  p.h1 = tb.ent1 ? tb.ent1 + (size_t)h * dim : nullptr;
-  p.t1 = tb.ent1 ? tb.ent1 + (size_t)t * dim : nullptr;
-  const size_t rstride = model == KGE_RESCAL ? (size_t)dim * dim : (size_t)dim;
-  p.r0 = tb.rel0 + (size_t)r * rstride;
-  p.r1 = tb.rel1 ? tb.rel1 + (size_t)r * rstride : nullptr;
-  p.h2 = p.t2 = p.r2 = nullptr;
-  if (model == KGE_ANALOGY) {   // planes equally spaced in memory (include/kge_b200.h)
-    const float* e2 = tb.ent1 + (tb.ent1 - tb.ent0);
-    p.h2 = e2 + (size_t)h * dim;
-    p.t2 = e2 + (size_t)t * dim;
-    p.r2 = tb.rel1 + (tb.rel1 - tb.rel0) + (size_t)r * dim;
-  }
-  return p;
-}
-
-// Destination rows of one triple's gradient, plane by plane (same layout as RowPtrs).
-struct GradRows {
-  float* h0; float* h1;
-  float* t0; float* t1;
-  float* r0; float* r1;
-  float* h2; float* t2; float* r2;
-};
-
-// The rows of triple (h, t, r) in the dense gradient tables.
-__device__ __forceinline__ GradRows grad_rows(int model, int dim, const TrainGrads& gr, long long h,
-                                              long long t, long long r) {
-  GradRows d;
-  const size_t rstride = model == KGE_RESCAL ? (size_t)dim * dim : (size_t)dim;
-  d.h0 = gr.ent0 + (size_t)h * dim;
-  d.t0 = gr.ent0 + (size_t)t * dim;
-  d.r0 = gr.rel0 + (size_t)r * rstride;
-  d.h1 = d.t1 = d.r1 = d.h2 = d.t2 = d.r2 = nullptr;
-  if (model == KGE_COMPLEX || model == KGE_ROTATE || model == KGE_ANALOGY) {
-    d.h1 = gr.ent1 + (size_t)h * dim;
-    d.t1 = gr.ent1 + (size_t)t * dim;
-    d.r1 = gr.rel1 + (size_t)r * dim;
-  }
-  if (model == KGE_ANALOGY) {
-    float* ge2 = gr.ent1 + (gr.ent1 - gr.ent0);
-    d.h2 = ge2 + (size_t)h * dim;
-    d.t2 = ge2 + (size_t)t * dim;
-    d.r2 = gr.rel1 + (gr.rel1 - gr.rel0) + (size_t)r * dim;
-  }
-  return d;
-}
-
-// ---- entity-sharded rows: the replaced entity from the local table, the rest from [b][planes][dim]
+// ---- row pointers, built plane by plane: from a dense table, or (entity-sharded rows) the replaced
+// entity from the local table and the rest from [b][planes][dim] buffers.  Planes a model does not
+// have are nullptr; triple_score / triple_backward dereference only the ones it has.
 __device__ __forceinline__ int ent_planes(int model) {
   return model == KGE_ANALOGY ? 3 : (model == KGE_COMPLEX || model == KGE_ROTATE ? 2 : 1);
 }
@@ -223,8 +179,8 @@ __device__ __forceinline__ int ent_planes(int model) {
 template <class T>
 struct Planes { T* p0; T* p1; T* p2; };
 
-// plane pointers of the row at element offset `off` of a table with planes p0, p1 (a third plane at
-// p1 + (p1 - p0), include/kge_b200.h)
+// plane pointers of the row at element offset `off` of a table with planes p0, p1 (a third plane
+// follows at the same spacing, include/kge_b200.h)
 template <class T>
 __device__ __forceinline__ Planes<T> table_planes(T* p0, T* p1, int np, size_t off) {
   Planes<T> o;
@@ -248,22 +204,23 @@ __device__ __forceinline__ Planes<T> rel_planes(int model, int dim, T* r0, T* r1
   return table_planes(r0, r1, ent_planes(model), (size_t)r * rstride);
 }
 
-__device__ __forceinline__ RowPtrs rows_of(const Planes<const float>& h, const Planes<const float>& t,
-                                           const Planes<const float>& r) {
-  RowPtrs p;
+template <class T>
+__device__ __forceinline__ Rows<T> rows_of(const Planes<T>& h, const Planes<T>& t, const Planes<T>& r) {
+  Rows<T> p;
   p.h0 = h.p0; p.h1 = h.p1; p.h2 = h.p2;
   p.t0 = t.p0; p.t1 = t.p1; p.t2 = t.p2;
   p.r0 = r.p0; p.r1 = r.p1; p.r2 = r.p2;
   return p;
 }
 
-__device__ __forceinline__ GradRows grads_of(const Planes<float>& h, const Planes<float>& t,
-                                             const Planes<float>& r) {
-  GradRows d;
-  d.h0 = h.p0; d.h1 = h.p1; d.h2 = h.p2;
-  d.t0 = t.p0; d.t1 = t.p1; d.t2 = t.p2;
-  d.r0 = r.p0; d.r1 = r.p1; d.r2 = r.p2;
-  return d;
+// The rows of triple (h, t, r) in dense tables: RowPtrs from TrainTables, GradRows from TrainGrads.
+template <class Tables>
+__device__ __forceinline__ auto table_rows(int model, int dim, const Tables& tb, long long h, long long t,
+                                           long long r) {
+  const int np = ent_planes(model);
+  return rows_of(table_planes(tb.ent0, tb.ent1, np, (size_t)h * dim),
+                 table_planes(tb.ent0, tb.ent1, np, (size_t)t * dim),
+                 rel_planes(model, dim, tb.rel0, tb.rel1, r));
 }
 
 // Gradient of one triple's score, scaled by g, added into the rows `d` (atomics: rows repeat).
@@ -391,7 +348,7 @@ __global__ void score_triples_fwd_kernel(int model, int dim, TrainTables tb,
   const long long w = ((long long)blockIdx.x * blockDim.x + threadIdx.x) >> 5;
   const int lane = threadIdx.x & 31;
   if (w >= n) return;
-  const RowPtrs p = make_rows(model, dim, tb, h[w], t[w], r[w]);
+  const RowPtrs p = table_rows(model, dim, tb, h[w], t[w], r[w]);
   const float s = triple_score(model, dim, p, lane, nullptr, nullptr);
   if (lane == 0) out[w] = s;
 }
@@ -405,8 +362,8 @@ __global__ void score_triples_bwd_kernel(int model, int dim, TrainTables tb, Tra
   const int lane = threadIdx.x & 31;
   if (w >= n) return;
   const long long hi = h[w], ti = t[w], ri = r[w];
-  const RowPtrs p = make_rows(model, dim, tb, hi, ti, ri);
-  triple_backward(model, dim, p, grad_rows(model, dim, gr, hi, ti, ri), gout[w], lane);
+  const RowPtrs p = table_rows(model, dim, tb, hi, ti, ri);
+  triple_backward(model, dim, p, table_rows(model, dim, gr, hi, ti, ri), gout[w], lane);
 }
 
 __global__ void corrupt_batch_kernel(const int64_t* __restrict__ h, const int64_t* __restrict__ t,
@@ -468,7 +425,7 @@ __global__ void margin_step_fwd_kernel(MarginStepParams a) {
   const int lane = threadIdx.x & 31;
   if (w >= a.b) return;
   const long long hi = a.h[w], ti = a.t[w], ri = a.r[w];
-  const RowPtrs pp = make_rows(a.model, a.dim, a.tb, hi, ti, ri);
+  const RowPtrs pp = table_rows(a.model, a.dim, a.tb, hi, ti, ri);
   const float pos = triple_score(a.model, a.dim, pp, lane, nullptr, nullptr);
   if (lane == 0 && a.pos_out) a.pos_out[w] = pos;
   const float p_head = a.nh ? 0.f : a.probs[ri];
@@ -478,7 +435,7 @@ __global__ void margin_step_fwd_kernel(MarginStepParams a) {
     long long nh, nt;
     if (a.nh) { nh = a.nh[idx]; nt = a.nt[idx]; }
     else corrupt_one(a.seed, a.offset, (uint64_t)idx, p_head, a.n_ent, hi, ti, &nh, &nt);
-    const RowPtrs pn = make_rows(a.model, a.dim, a.tb, nh, nt, ri);
+    const RowPtrs pn = table_rows(a.model, a.dim, a.tb, nh, nt, ri);
     const float neg = triple_score(a.model, a.dim, pn, lane, nullptr, nullptr);
     if (lane == 0) {
       if (a.neg_out) a.neg_out[idx] = neg;
@@ -498,7 +455,7 @@ __global__ void margin_step_bwd_kernel(MarginStepParams a, TrainGrads gr, const 
   if (w >= a.b) return;
   const float g = *gloss;
   const long long hi = a.h[w], ti = a.t[w], ri = a.r[w];
-  const RowPtrs pp = make_rows(a.model, a.dim, a.tb, hi, ti, ri);
+  const RowPtrs pp = table_rows(a.model, a.dim, a.tb, hi, ti, ri);
   const float pos = triple_score(a.model, a.dim, pp, lane, nullptr, nullptr);
   const float p_head = a.nh ? 0.f : a.probs[ri];
   double gpos_sum = 0.0;   // thousands of non-integer dl/dpos terms (logistic, BCE): fp32 would drift
@@ -507,14 +464,14 @@ __global__ void margin_step_bwd_kernel(MarginStepParams a, TrainGrads gr, const 
     long long nh, nt;
     if (a.nh) { nh = a.nh[idx]; nt = a.nt[idx]; }
     else corrupt_one(a.seed, a.offset, (uint64_t)idx, p_head, a.n_ent, hi, ti, &nh, &nt);
-    const RowPtrs pn = make_rows(a.model, a.dim, a.tb, nh, nt, ri);
+    const RowPtrs pn = table_rows(a.model, a.dim, a.tb, nh, nt, ri);
     const float neg = triple_score(a.model, a.dim, pn, lane, nullptr, nullptr);
     float gp, gn;
     pair_loss_grads(a.loss_kind, a.margin, 1.f, pos, neg, &gp, &gn);
     gpos_sum += gp;
-    triple_backward(a.model, a.dim, pn, grad_rows(a.model, a.dim, gr, nh, nt, ri), g * gn, lane);
+    triple_backward(a.model, a.dim, pn, table_rows(a.model, a.dim, gr, nh, nt, ri), g * gn, lane);
   }
-  triple_backward(a.model, a.dim, pp, grad_rows(a.model, a.dim, gr, hi, ti, ri), g * (float)gpos_sum, lane);
+  triple_backward(a.model, a.dim, pp, table_rows(a.model, a.dim, gr, hi, ti, ri), g * (float)gpos_sum, lane);
 }
 
 // Entity-sharded fused step (a.hrows set), one warp per positive.  Every rank runs the same draws;
@@ -590,9 +547,9 @@ __global__ void margin_step_shard_bwd_kernel(MarginStepParams a, TrainGrads gr, 
     pair_loss_grads(a.loss_kind, a.margin, 1.f, pos, neg, &gp, &gn);
     gpos_sum += gp;
     const Planes<float> ge = table_planes(gr.ent0, gr.ent1, np, (size_t)loc * a.dim);
-    triple_backward(a.model, a.dim, pn, grads_of(head ? ge : gh, head ? gt : ge, grel), g * gn, lane);
+    triple_backward(a.model, a.dim, pn, rows_of(head ? ge : gh, head ? gt : ge, grel), g * gn, lane);
   }
-  triple_backward(a.model, a.dim, pp, grads_of(gh, gt, grel), g * (float)gpos_sum, lane);
+  triple_backward(a.model, a.dim, pp, rows_of(gh, gt, grel), g * (float)gpos_sum, lane);
 }
 
 // ------------------------------------------------------------------------------------------
@@ -611,9 +568,14 @@ __global__ void margin_step_shard_bwd_kernel(MarginStepParams a, TrainGrads gr, 
 // relation are linear in  V = sum over active negatives of en  (TransE-L1: of sign(P - en)),
 // which stays in registers, so the positive's three rows are written once per positive instead of
 // once per negative (the relation rows are shared by thousands of triples: 256x fewer atomics on
-// the hottest addresses).  Philox draws are made 32 negatives at a time, one per lane.
+// the hottest addresses).
 // Algorithmic traffic per positive: forward (n_neg + 3) * 4 dim bytes, backward the same rows
 // again (recomputed, not stored) plus one RMW of each (SURVEY.md section 8d).
+//
+// That arithmetic is stated once, in fast_positive / fast_negative / fast_negative_backward /
+// fast_positive_backward below (both_replaced_pair is the one case outside the closed form).  Two
+// kernels run it, margin_step_fast_kernel and margin_step_ring_kernel: they differ only in how a
+// negative's identity and row reach the warp, and that is all their bodies contain.
 // ------------------------------------------------------------------------------------------
 constexpr int FAST_NCH = 2;         // float4 chunks per lane
 constexpr int FAST_MAX_DIM = 4 * 32 * FAST_NCH;
@@ -683,50 +645,247 @@ __device__ __forceinline__ void warp_sum2(float& a, float& b) {
 }
 __device__ __forceinline__ float sgn(float x) { return x > 0.f ? 1.f : (x < 0.f ? -1.f : 0.f); }
 
+// The positive, as its negatives see it.
+struct FastPos {
+  Vec r, hn, tn;       // the relation's row; the normalised head and tail
+  float inv_h, inv_t;  // 1 / max(|h|, eps), 1 / max(|t|, eps)
+  float sA, sB;        // |A|^2, |Bv|^2 (TransE-L2)
+  float pos;           // its score
+};
+// A and Bv are an object of their own: a negative picks one of them by address (head ? Bv : A), and the
+// compiler keeps the whole object addressed that way in local memory.  As members of FastPos they take
+// the positive's other rows there with them (192 stack bytes instead of these 64).
+struct FastAB { Vec A, Bv; };
+
+// hrow / trow / rrow: the positive's three rows in global memory, read here and nowhere else.
+template <int MODEL>
+__device__ __forceinline__ void fast_positive(const float* hrow, const float* trow, const float* rrow, int dim,
+                                              int lane, FastPos& p, FastAB& ab) {
+  const Vec h = vec_load(hrow, dim, lane);
+  const Vec t = vec_load(trow, dim, lane);
+  p.r = vec_load(rrow, dim, lane);
+  float sh = vec_dot(h, h), stt = vec_dot(t, t);
+  warp_sum2(sh, stt);
+  p.inv_h = 1.0f / fmaxf(sqrtf(sh), NORM_EPS);
+  p.inv_t = 1.0f / fmaxf(sqrtf(stt), NORM_EPS);
+  p.hn = vec_scale(h, p.inv_h);
+  p.tn = vec_scale(t, p.inv_t);
+  if constexpr (MODEL == KGE_DISTMULT) {
+    ab.A = vec_map(p.hn, p.r, [](float x, float y) { return x * y; });
+    ab.Bv = vec_map(p.r, p.tn, [](float x, float y) { return x * y; });
+  } else {
+    ab.A = vec_map(p.hn, p.r, [](float x, float y) { return x + y; });
+    ab.Bv = vec_map(p.tn, p.r, [](float x, float y) { return x - y; });
+  }
+  p.sA = p.sB = 0.f;
+  if constexpr (MODEL == KGE_DISTMULT) {
+    p.pos = warp_sum(vec_dot(ab.A, p.tn));
+  } else if constexpr (MODEL == KGE_TRANSE_L2) {
+    p.sA = vec_dot(ab.A, ab.A); p.sB = vec_dot(ab.Bv, ab.Bv);
+    warp_sum2(p.sA, p.sB);
+    const Vec x = vec_map(ab.A, p.tn, [](float a_, float q) { return a_ - q; });
+    p.pos = -warp_sum(vec_dot(x, x));
+  } else {
+    p.pos = -warp_sum(vec_l1_diff(ab.A, p.tn));
+  }
+}
+
+// One negative, scored from its corrupted entity's row ev (head: the head is the replaced end).
+struct FastNeg {
+  float neg, inv_e;  // its score; 1 / max(|e|, eps)
+  float en_dot_G;    // en . (d neg / d en), needed by the normalisation Jacobian
+  Vec en;            // the normalised row: TransE-L1 scores with it, the others need it in the backward only
+};
+
+template <int MODEL, bool BWD>
+__device__ __forceinline__ void fast_negative(const FastPos& p, const FastAB& ab, const Vec& ev, bool head,
+                                              FastNeg& n) {
+  const Vec& P = head ? ab.Bv : ab.A;
+  float se = vec_dot(ev, ev), sp = vec_dot(ev, P);
+  warp_sum2(se, sp);
+  n.inv_e = 1.0f / fmaxf(sqrtf(se), NORM_EPS);
+  n.en_dot_G = 0.f;
+  if constexpr (MODEL == KGE_DISTMULT) {
+    n.neg = sp * n.inv_e;
+    n.en_dot_G = n.neg;
+  } else if constexpr (MODEL == KGE_TRANSE_L2) {
+    const float sP = head ? p.sB : p.sA;
+    const float ee = n.inv_e * n.inv_e * se, pe = n.inv_e * sp;
+    n.neg = -(sP - 2.f * pe + ee);
+    n.en_dot_G = 2.f * (pe - ee);
+  } else {
+    n.en = vec_scale(ev, n.inv_e);
+    float l1 = vec_l1_diff(P, n.en), eg = 0.f;
+    if (BWD) {
+      const Vec sg = vec_map(P, n.en, [](float a_, float q) { return sgn(a_ - q); });
+      eg = vec_dot(n.en, sg);
+    }
+    warp_sum2(l1, eg);
+    n.neg = -l1;
+    n.en_dot_G = eg;
+  }
+}
+
+// Lane 0 keeps the loss term of the pair (pos, neg); the forward writes the negative's score out.
+template <bool BWD, int LOSS>
+__device__ __forceinline__ void pair_forward(const MarginStepParams& a, long long idx, int lane, float pos,
+                                             float neg, float& loss) {
+  const float term = pair_loss_term(LOSS, a.margin, pos, neg);
+  if (lane == 0) {
+    if (!BWD && a.neg_out) a.neg_out[idx] = neg;
+    loss += term;
+  }
+}
+
+// What the backward sums over one positive's negatives.  The closed form is linear in the negatives, so
+// a loss other than the margin only turns the counts into weights: negative j enters V, its kind's sum
+// and its own scatter with weight c_j = dl/dneg_j, and the positive with -sum_j dl/dpos instead of the
+// active count.  For the margin loss c_j = 1 on every active hinge and the weights drop out at compile
+// time.  The weights and dl/dpos are non-integers summed over up to thousands of negatives: in double, as
+// fp32 would drift by ~n eps.
+template <int LOSS>
+struct FastAcc {
+  using Count = std::conditional_t<LOSS == KGE_LOSS_MARGIN, int, double>;
+  Vec Vt, Vh;              // V over the tail- / head-corrupted negatives
+  Count n_t = 0, n_h = 0;  // per kind: the active hinges (margin) or the summed weights c_j
+  double gpos_sum = 0.0;   // LOSS != margin: sum of dl/dpos
+  __device__ __forceinline__ FastAcc() {
+#pragma unroll
+    for (int i = 0; i < FAST_NCH; ++i) Vt.c[i] = Vh.c[i] = make_float4(0.f, 0.f, 0.f, 0.f);
+  }
+};
+
+// Backward of one negative: its row's gradient, g c_j (G - en (en . G)) * inv_e with G = d neg / d en,
+// goes to dst at once; c_j V and c_j go into acc.
+template <int MODEL, int LOSS>
+__device__ __forceinline__ void fast_negative_backward(const FastPos& p, const FastAB& ab, const Vec& ev, bool head,
+                                                       const FastNeg& n, float margin, float g, float* dst,
+                                                       int dim, int lane, FastAcc<LOSS>& acc) {
+  float gp, cj;   // dl/dpos and dl/dneg of this pair (g = 1)
+  pair_loss_grads(LOSS, margin, 1.f, p.pos, n.neg, &gp, &cj);
+  if constexpr (LOSS != KGE_LOSS_MARGIN) acc.gpos_sum += gp;
+  if (cj == 0.f) return;
+  const float wj = LOSS == KGE_LOSS_MARGIN ? 1.f : cj;
+  const Vec& P = head ? ab.Bv : ab.A;
+  Vec en;
+  if constexpr (MODEL == KGE_TRANSE_L1) en = n.en;
+  else en = vec_scale(ev, n.inv_e);
+  const float en_dot_G = n.en_dot_G;
+  Vec ge, V;
+  const float c = LOSS == KGE_LOSS_MARGIN ? g * n.inv_e : g * wj * n.inv_e;
+  if constexpr (MODEL == KGE_DISTMULT) {
+    ge = vec_map(P, en, [=](float a_, float q) { return c * (a_ - q * en_dot_G); });
+    V = LOSS == KGE_LOSS_MARGIN ? en : vec_scale(en, wj);
+  } else if constexpr (MODEL == KGE_TRANSE_L2) {
+    ge = vec_map(P, en, [=](float a_, float q) { return c * (2.f * (a_ - q) - q * en_dot_G); });
+    V = LOSS == KGE_LOSS_MARGIN ? en : vec_scale(en, wj);
+  } else {
+    V = vec_map(P, en, [](float a_, float q) { return sgn(a_ - q); });
+    ge = vec_map(V, en, [=](float s_, float q) { return c * (s_ - q * en_dot_G); });
+    if constexpr (LOSS != KGE_LOSS_MARGIN) V = vec_scale(V, wj);
+  }
+  vec_atomic_add(dst, dim, lane, ge);
+  using Count = typename FastAcc<LOSS>::Count;
+  const Count inc = LOSS == KGE_LOSS_MARGIN ? Count(1) : Count(wj);
+  if (head) { acc.Vh = vec_map(acc.Vh, V, [](float x, float y) { return x + y; }); acc.n_h += inc; }
+  else { acc.Vt = vec_map(acc.Vt, V, [](float x, float y) { return x + y; }); acc.n_t += inc; }
+}
+
+// Backward of the positive, once: gradients with respect to hn, tn, r (+g c_j per negative, -g fn for
+// the positive), through the normalisation, added into the three destination rows.
+template <int MODEL, int LOSS>
+__device__ __forceinline__ void fast_positive_backward(const FastPos& p, const FastAB& ab, const FastAcc<LOSS>& acc,
+                                                       float g, float* dst_h, float* dst_t, float* dst_r,
+                                                       int dim, int lane) {
+  if constexpr (LOSS == KGE_LOSS_MARGIN) {
+    if (acc.n_t + acc.n_h == 0) return;
+  } else {
+    if (acc.n_t == 0.0 && acc.n_h == 0.0 && acc.gpos_sum == 0.0) return;
+  }
+  // fn: the positive's weight, -sum_j dl/dpos (the margin loss: the active count)
+  const float fn_t = (float)acc.n_t, fn_h = (float)acc.n_h;
+  const float fn = LOSS == KGE_LOSS_MARGIN ? (float)(acc.n_t + acc.n_h) : (float)-acc.gpos_sum;
+  const Vec& Vt = acc.Vt;
+  const Vec& Vh = acc.Vh;
+  Vec Gh, Gt, Gr;
+  if constexpr (MODEL == KGE_DISTMULT) {
+    // neg_t = sum A en, A = hn r ;  neg_h = sum en Bv, Bv = r tn ;  pos = sum hn r tn
+    Gh = vec_map3(p.r, Vt, p.tn, [=](float rr, float vt, float tt) { return g * rr * (vt - fn * tt); });
+    Gt = vec_map3(p.r, Vh, p.hn, [=](float rr, float vh, float hh) { return g * rr * (vh - fn * hh); });
+    const Vec tmp = vec_map3(p.hn, Vt, p.tn, [=](float hh, float vt, float tt) { return hh * (vt - fn * tt); });
+    Gr = vec_map3(tmp, p.tn, Vh, [=](float x, float tt, float vh) { return g * (x + tt * vh); });
+  } else if constexpr (MODEL == KGE_TRANSE_L2) {
+    // neg_t = -|A - en|^2 ; neg_h = -|en - Bv|^2 ; pos = -|x|^2, x = A - tn
+    const Vec x = vec_map(ab.A, p.tn, [](float a_, float q) { return a_ - q; });
+    const Vec dt = vec_map3(ab.A, Vt, x, [=](float aa, float vt, float xx) {  // sum_t (A - en) - n x
+      return fn_t * aa - vt - fn * xx; });
+    const Vec dh = vec_map(Vh, ab.Bv, [=](float vh, float bb) { return vh - fn_h * bb; });  // sum_h (en - Bv)
+    Gh = vec_scale(dt, -2.f * g);
+    Gt = vec_map3(dh, x, x, [=](float d, float xx, float) { return 2.f * g * (d - fn * xx); });
+    Gr = vec_map(dt, dh, [=](float a_, float q) { return -2.f * g * (a_ + q); });
+  } else {
+    // neg_t = -|A - en|_1 (V = sign(A - en)) ; neg_h = -|Bv - en|_1 (V = sign(Bv - en)) ; pos = -|x|_1
+    const Vec sx = vec_map(ab.A, p.tn, [](float a_, float q) { return sgn(a_ - q); });
+    Gh = vec_map(Vt, sx, [=](float vt, float s_) { return g * (fn * s_ - vt); });
+    Gt = vec_map(Vh, sx, [=](float vh, float s_) { return g * (-vh - fn * s_); });
+    Gr = vec_map3(Vt, Vh, sx, [=](float vt, float vh, float s_) { return g * (vh - vt + fn * s_); });
+  }
+  float ph = vec_dot(p.hn, Gh), pt = vec_dot(p.tn, Gt);
+  warp_sum2(ph, pt);
+  const float inv_h = p.inv_h, inv_t = p.inv_t;
+  const Vec gh = vec_map(Gh, p.hn, [=](float gg, float q) { return (gg - q * ph) * inv_h; });
+  const Vec gt = vec_map(Gt, p.tn, [=](float gg, float q) { return (gg - q * pt) * inv_t; });
+  vec_atomic_add(dst_h, dim, lane, gh);
+  vec_atomic_add(dst_t, dim, lane, gt);
+  vec_atomic_add(dst_r, dim, lane, Gr);
+}
+
+// A negative with both ends replaced (possible with caller-supplied negatives only) is outside the
+// closed form: the generic score, and in the backward the generic gradients of the negative and of
+// the positive for this pair alone.
+template <int MODEL, bool BWD, int LOSS>
+__device__ __forceinline__ void both_replaced_pair(const MarginStepParams& a, const TrainGrads& gr, long long hi,
+                                                   long long ti, long long ri, long long nh, long long nt,
+                                                   long long idx, float pos, float g, int lane, float& loss) {
+  const RowPtrs pn = table_rows(MODEL, a.dim, a.tb, nh, nt, ri);
+  const float neg = triple_score(MODEL, a.dim, pn, lane, nullptr, nullptr);
+  pair_forward<BWD, LOSS>(a, idx, lane, pos, neg, loss);
+  if constexpr (BWD) {
+    float gp, gn;   // g = 1; the margin loss: -1 and 1 on an active hinge
+    pair_loss_grads(LOSS, a.margin, 1.f, pos, neg, &gp, &gn);
+    if (gn != 0.f || gp != 0.f) {
+      triple_backward(MODEL, a.dim, pn, table_rows(MODEL, a.dim, gr, nh, nt, ri),
+                      LOSS == KGE_LOSS_MARGIN ? g : g * gn, lane);
+      const RowPtrs pp = table_rows(MODEL, a.dim, a.tb, hi, ti, ri);
+      triple_backward(MODEL, a.dim, pp, table_rows(MODEL, a.dim, gr, hi, ti, ri),
+                      LOSS == KGE_LOSS_MARGIN ? -g : g * gp, lane);
+    }
+  }
+}
+
+// Register-resident form: no shared memory.  Philox draws are made 32 negatives at a time, one per
+// lane, and handed round by shuffle; PF rows at a time are loaded into registers and then reduced.
+// Margin loss only (launch_margin_step): the other losses take the ring or the generic kernels.
 template <int MODEL, bool BWD>
 __global__ void __launch_bounds__(WARPS_PER_BLOCK * 32, 4)
 margin_step_fast_kernel(MarginStepParams a, TrainGrads gr, const float* __restrict__ gloss) {
   constexpr int PF = BWD ? 2 : 4;  // negatives whose rows are in flight together, per warp
+  constexpr int LOSS = KGE_LOSS_MARGIN;
   const long long w = ((long long)blockIdx.x * blockDim.x + threadIdx.x) >> 5;
   const int lane = threadIdx.x & 31;
   if (w >= a.b) return;
   const int dim = a.dim;
   const float* __restrict__ ent = a.tb.ent0;
   const long long hi = a.h[w], ti = a.t[w], ri = a.r[w];
-  const Vec h = vec_load(ent + (size_t)hi * dim, dim, lane);
-  const Vec t = vec_load(ent + (size_t)ti * dim, dim, lane);
-  const Vec r = vec_load(a.tb.rel0 + (size_t)ri * dim, dim, lane);
-  float sh = vec_dot(h, h), stt = vec_dot(t, t);
-  warp_sum2(sh, stt);
-  const float inv_h = 1.0f / fmaxf(sqrtf(sh), NORM_EPS), inv_t = 1.0f / fmaxf(sqrtf(stt), NORM_EPS);
-  const Vec hn = vec_scale(h, inv_h), tn = vec_scale(t, inv_t);
-  Vec A, Bv;
-  if constexpr (MODEL == KGE_DISTMULT) {
-    A = vec_map(hn, r, [](float x, float y) { return x * y; });
-    Bv = vec_map(r, tn, [](float x, float y) { return x * y; });
-  } else {
-    A = vec_map(hn, r, [](float x, float y) { return x + y; });
-    Bv = vec_map(tn, r, [](float x, float y) { return x - y; });
-  }
-  float sA = 0.f, sB = 0.f, pos;
-  if constexpr (MODEL == KGE_DISTMULT) {
-    pos = warp_sum(vec_dot(A, tn));
-  } else if constexpr (MODEL == KGE_TRANSE_L2) {
-    sA = vec_dot(A, A); sB = vec_dot(Bv, Bv);
-    warp_sum2(sA, sB);
-    const Vec x = vec_map(A, tn, [](float p, float q) { return p - q; });
-    pos = -warp_sum(vec_dot(x, x));
-  } else {
-    pos = -warp_sum(vec_l1_diff(A, tn));
-  }
-  if (lane == 0 && a.pos_out && !BWD) a.pos_out[w] = pos;
+  FastPos pp;
+  FastAB ab;
+  fast_positive<MODEL>(ent + (size_t)hi * dim, ent + (size_t)ti * dim, a.tb.rel0 + (size_t)ri * dim, dim, lane, pp,
+                       ab);
+  if (lane == 0 && a.pos_out && !BWD) a.pos_out[w] = pp.pos;
   const float p_head = a.nh ? 0.f : a.probs[ri];
   const float g = BWD ? *gloss : 0.f;
   float loss = 0.f;
-  Vec Vt, Vh;  // sums over the active tail- / head-corrupted negatives (BWD only)
-#pragma unroll
-  for (int i = 0; i < FAST_NCH; ++i) Vt.c[i] = Vh.c[i] = make_float4(0.f, 0.f, 0.f, 0.f);
-  int n_t = 0, n_h = 0;  // active negatives per kind
+  FastAcc<LOSS> acc;
   for (int j0 = 0; j0 < a.n_neg; j0 += 32) {
     // this lane's draw for negative j0 + lane
     long long my_nh = hi, my_nt = ti;
@@ -740,131 +899,40 @@ margin_step_fast_kernel(MarginStepParams a, TrainGrads gr, const float* __restri
     // PF negatives at a time: their rows are requested together (memory-level parallelism:
     // PF x 4 dim bytes in flight per warp), then reduced one after the other
     for (int jj0 = 0; jj0 < jn; jj0 += PF) {
-     long long nhs[PF], nts[PF];
-     Vec evs[PF];
+      long long nhs[PF], nts[PF];
+      Vec evs[PF];
 #pragma unroll
-     for (int u = 0; u < PF; ++u) {
-       const int jj = min(jj0 + u, 31);
-       nhs[u] = __shfl_sync(0xffffffffu, my_nh, jj);
-       nts[u] = __shfl_sync(0xffffffffu, my_nt, jj);
-       const bool both = nhs[u] != hi && nts[u] != ti;
-       const long long e_ = nhs[u] != hi ? nhs[u] : nts[u];
-       if (jj0 + u < jn && !both) evs[u] = vec_load(ent + (size_t)e_ * dim, dim, lane);
-     }
+      for (int u = 0; u < PF; ++u) {
+        const int jj = min(jj0 + u, 31);
+        nhs[u] = __shfl_sync(0xffffffffu, my_nh, jj);
+        nts[u] = __shfl_sync(0xffffffffu, my_nt, jj);
+        const bool both = nhs[u] != hi && nts[u] != ti;
+        const long long e_ = nhs[u] != hi ? nhs[u] : nts[u];
+        if (jj0 + u < jn && !both) evs[u] = vec_load(ent + (size_t)e_ * dim, dim, lane);
+      }
 #pragma unroll
-     for (int u = 0; u < PF; ++u) {
-      if (jj0 + u >= jn) break;
-      const int jj = jj0 + u;
-      const long long nh = nhs[u], nt = nts[u];
-      const long long idx = (long long)(j0 + jj) * a.b + w;
-      if (nh != hi && nt != ti) {
-        // both ends replaced (possible with caller-supplied negatives only): generic path
-        const RowPtrs pn = make_rows(MODEL, dim, a.tb, nh, nt, ri);
-        const float neg = triple_score(MODEL, dim, pn, lane, nullptr, nullptr);
-        const float v = a.margin - pos + neg;
-        if (lane == 0) {
-          if (!BWD && a.neg_out) a.neg_out[idx] = neg;
-          loss += fmaxf(0.f, v);
+      for (int u = 0; u < PF; ++u) {
+        if (jj0 + u >= jn) break;
+        const long long nh = nhs[u], nt = nts[u];
+        const long long idx = (long long)(j0 + jj0 + u) * a.b + w;
+        if (nh != hi && nt != ti) {
+          both_replaced_pair<MODEL, BWD, LOSS>(a, gr, hi, ti, ri, nh, nt, idx, pp.pos, g, lane, loss);
+          continue;
         }
-        if (BWD && v > 0.f) {
-          triple_backward(MODEL, dim, pn, grad_rows(MODEL, dim, gr, nh, nt, ri), g, lane);
-          const RowPtrs pp = make_rows(MODEL, dim, a.tb, hi, ti, ri);
-          triple_backward(MODEL, dim, pp, grad_rows(MODEL, dim, gr, hi, ti, ri), -g, lane);
-        }
-        continue;
+        const bool head = nh != hi;            // warp-uniform
+        FastNeg n;
+        fast_negative<MODEL, BWD>(pp, ab, evs[u], head, n);
+        pair_forward<BWD, LOSS>(a, idx, lane, pp.pos, n.neg, loss);
+        if constexpr (BWD)
+          fast_negative_backward<MODEL, LOSS>(pp, ab, evs[u], head, n, a.margin, g,
+                                              gr.ent0 + (size_t)(head ? nh : nt) * dim, dim, lane, acc);
       }
-      const bool head = nh != hi;            // warp-uniform
-      const long long e = head ? nh : nt;
-      const Vec ev = evs[u];
-      const Vec& P = head ? Bv : A;
-      float se = vec_dot(ev, ev), sp = vec_dot(ev, P);
-      warp_sum2(se, sp);
-      const float inv_e = 1.0f / fmaxf(sqrtf(se), NORM_EPS);
-      float neg, en_dot_G = 0.f;  // en . (d neg / d en), needed by the normalisation Jacobian
-      Vec en;
-      if constexpr (MODEL == KGE_DISTMULT) {
-        neg = sp * inv_e;
-        en_dot_G = neg;
-      } else if constexpr (MODEL == KGE_TRANSE_L2) {
-        const float sP = head ? sB : sA;
-        const float ee = inv_e * inv_e * se, pe = inv_e * sp;
-        neg = -(sP - 2.f * pe + ee);
-        en_dot_G = 2.f * (pe - ee);
-      } else {
-        en = vec_scale(ev, inv_e);
-        float l1 = vec_l1_diff(P, en), eg = 0.f;
-        if (BWD) {
-          const Vec sg = vec_map(P, en, [](float p, float q) { return sgn(p - q); });
-          eg = vec_dot(en, sg);
-        }
-        warp_sum2(l1, eg);
-        neg = -l1;
-        en_dot_G = eg;
-      }
-      const float v = a.margin - pos + neg;
-      if (lane == 0) {
-        if (!BWD && a.neg_out) a.neg_out[idx] = neg;
-        loss += fmaxf(0.f, v);
-      }
-      if (BWD && v > 0.f) {  // same sub-gradient as torch: zero at the kink
-        if constexpr (MODEL != KGE_TRANSE_L1) en = vec_scale(ev, inv_e);
-        // G = d neg / d en ; d neg / d e = (G - en (en . G)) * inv_e
-        Vec ge, V;
-        const float c = g * inv_e;
-        if constexpr (MODEL == KGE_DISTMULT) {
-          ge = vec_map(P, en, [=](float p, float q) { return c * (p - q * en_dot_G); });
-          V = en;
-        } else if constexpr (MODEL == KGE_TRANSE_L2) {
-          ge = vec_map(P, en, [=](float p, float q) { return c * (2.f * (p - q) - q * en_dot_G); });
-          V = en;
-        } else {
-          V = vec_map(P, en, [](float p, float q) { return sgn(p - q); });
-          ge = vec_map(V, en, [=](float s_, float q) { return c * (s_ - q * en_dot_G); });
-        }
-        vec_atomic_add(gr.ent0 + (size_t)e * dim, dim, lane, ge);
-        if (head) { Vh = vec_map(Vh, V, [](float x, float y) { return x + y; }); ++n_h; }
-        else { Vt = vec_map(Vt, V, [](float x, float y) { return x + y; }); ++n_t; }
-      }
-     }
     }
   }
-  if (!BWD) {
-    if (lane == 0) atomicAdd(a.loss, loss);
-    return;
-  }
-  if (n_t + n_h == 0) return;
-  // Gradients with respect to hn, tn, r: +g per active negative, -g * (n_t + n_h) for the positive.
-  const float fn_t = (float)n_t, fn_h = (float)n_h, fn = (float)(n_t + n_h);
-  Vec Gh, Gt, Gr;
-  if constexpr (MODEL == KGE_DISTMULT) {
-    // neg_t = sum A en, A = hn r ;  neg_h = sum en Bv, Bv = r tn ;  pos = sum hn r tn
-    Gh = vec_map3(r, Vt, tn, [=](float rr, float vt, float tt) { return g * rr * (vt - fn * tt); });
-    Gt = vec_map3(r, Vh, hn, [=](float rr, float vh, float hh) { return g * rr * (vh - fn * hh); });
-    const Vec tmp = vec_map3(hn, Vt, tn, [=](float hh, float vt, float tt) { return hh * (vt - fn * tt); });
-    Gr = vec_map3(tmp, tn, Vh, [=](float x, float tt, float vh) { return g * (x + tt * vh); });
-  } else if constexpr (MODEL == KGE_TRANSE_L2) {
-    // neg_t = -|A - en|^2 ; neg_h = -|en - Bv|^2 ; pos = -|x|^2, x = A - tn
-    const Vec x = vec_map(A, tn, [](float p, float q) { return p - q; });
-    const Vec dt = vec_map3(A, Vt, x, [=](float aa, float vt, float xx) {  // sum_t (A - en) - n x
-      return fn_t * aa - vt - fn * xx; });
-    const Vec dh = vec_map(Vh, Bv, [=](float vh, float bb) { return vh - fn_h * bb; });  // sum_h (en - Bv)
-    Gh = vec_scale(dt, -2.f * g);
-    Gt = vec_map3(dh, x, x, [=](float d, float xx, float) { return 2.f * g * (d - fn * xx); });
-    Gr = vec_map(dt, dh, [=](float p, float q) { return -2.f * g * (p + q); });
-  } else {
-    // neg_t = -|A - en|_1 (V = sign(A - en)) ; neg_h = -|Bv - en|_1 (V = sign(Bv - en)) ; pos = -|x|_1
-    const Vec sx = vec_map(A, tn, [](float p, float q) { return sgn(p - q); });
-    Gh = vec_map(Vt, sx, [=](float vt, float s_) { return g * (fn * s_ - vt); });
-    Gt = vec_map(Vh, sx, [=](float vh, float s_) { return g * (-vh - fn * s_); });
-    Gr = vec_map3(Vt, Vh, sx, [=](float vt, float vh, float s_) { return g * (vh - vt + fn * s_); });
-  }
-  float ph = vec_dot(hn, Gh), pt = vec_dot(tn, Gt);
-  warp_sum2(ph, pt);
-  const Vec gh = vec_map(Gh, hn, [=](float gg, float q) { return (gg - q * ph) * inv_h; });
-  const Vec gt = vec_map(Gt, tn, [=](float gg, float q) { return (gg - q * pt) * inv_t; });
-  vec_atomic_add(gr.ent0 + (size_t)hi * dim, dim, lane, gh);
-  vec_atomic_add(gr.ent0 + (size_t)ti * dim, dim, lane, gt);
-  vec_atomic_add(gr.rel0 + (size_t)ri * dim, dim, lane, Gr);
+  if constexpr (BWD)
+    fast_positive_backward<MODEL, LOSS>(pp, ab, acc, g, gr.ent0 + (size_t)hi * dim, gr.ent0 + (size_t)ti * dim,
+                                        gr.rel0 + (size_t)ri * dim, dim, lane);
+  else if (lane == 0) atomicAdd(a.loss, loss);
 }
 
 // ------------------------------------------------------------------------------------------
@@ -875,7 +943,7 @@ margin_step_fast_kernel(MarginStepParams a, TrainGrads gr, const float* __restri
 // with 16 resident warps per SM (ncu: warps active 24 %).  Here a warp keeps RING rows in flight
 // at all times (8 x 800 B = 6.4 KB), independently of its register budget, the Philox draws of all
 // negatives are made up front into shared memory, and row j + RING is requested the moment row j
-// has been consumed.  Arithmetic per negative is exactly that of margin_step_fast_kernel.
+// has been consumed.  The arithmetic per negative is the closed form stated above.
 // Shared memory per warp: RING * row_bytes + 4 * n_neg (codes) + RING barriers.
 // ------------------------------------------------------------------------------------------
 constexpr int RING = 8;
@@ -897,9 +965,7 @@ __device__ __forceinline__ Vec vec_load_smem(const float* row, int dim, int lane
 // trows, the draw loop keeps only the negatives whose replaced entity this rank holds (ballot +
 // prefix, local row numbers in `codes`), so the ring streams owned rows only, and the positive's
 // gradients go to grad_hrows / grad_trows[w].
-// LOSS: KGE_LOSS_*.  The backward's closed form is linear in the negatives, so a loss other than the
-// margin only turns the counts into weights: negative j enters V, its kind's sum and its own scatter
-// with weight c_j = dl/dneg_j, and the positive with -sum_j dl/dpos instead of the active count.
+// LOSS: KGE_LOSS_*; it turns the backward's counts into weights (FastAcc).
 template <int MODEL, bool BWD, int MINB = 0, bool SHARD = false, int LOSS = KGE_LOSS_MARGIN>
 __global__ void __launch_bounds__(WARPS_PER_BLOCK * 32, MINB == 0 ? 1 : MINB)
 margin_step_ring_kernel(MarginStepParams a, TrainGrads gr, const float* __restrict__ gloss) {
@@ -969,68 +1035,21 @@ margin_step_ring_kernel(MarginStepParams a, TrainGrads gr, const float* __restri
     for (int j = 0; j < first; ++j) request(j);
   }
   // ---- the positive (its three rows come straight from global memory, once) ----
-  const Vec h = vec_load(SHARD ? a.hrows + (size_t)w * dim : ent + (size_t)hi * dim, dim, lane);
-  const Vec t = vec_load(SHARD ? a.trows + (size_t)w * dim : ent + (size_t)ti * dim, dim, lane);
-  const Vec r = vec_load(a.tb.rel0 + (size_t)ri * dim, dim, lane);
-  float sh = vec_dot(h, h), stt = vec_dot(t, t);
-  warp_sum2(sh, stt);
-  const float inv_h = 1.0f / fmaxf(sqrtf(sh), NORM_EPS), inv_t = 1.0f / fmaxf(sqrtf(stt), NORM_EPS);
-  const Vec hn = vec_scale(h, inv_h), tn = vec_scale(t, inv_t);
-  Vec A, Bv;
-  if constexpr (MODEL == KGE_DISTMULT) {
-    A = vec_map(hn, r, [](float x, float y) { return x * y; });
-    Bv = vec_map(r, tn, [](float x, float y) { return x * y; });
-  } else {
-    A = vec_map(hn, r, [](float x, float y) { return x + y; });
-    Bv = vec_map(tn, r, [](float x, float y) { return x - y; });
-  }
-  float sA = 0.f, sB = 0.f, pos;
-  if constexpr (MODEL == KGE_DISTMULT) {
-    pos = warp_sum(vec_dot(A, tn));
-  } else if constexpr (MODEL == KGE_TRANSE_L2) {
-    sA = vec_dot(A, A); sB = vec_dot(Bv, Bv);
-    warp_sum2(sA, sB);
-    const Vec x = vec_map(A, tn, [](float p, float q) { return p - q; });
-    pos = -warp_sum(vec_dot(x, x));
-  } else {
-    pos = -warp_sum(vec_l1_diff(A, tn));
-  }
-  if (lane == 0 && a.pos_out && !BWD) a.pos_out[w] = pos;
+  FastPos pp;
+  FastAB ab;
+  fast_positive<MODEL>(SHARD ? a.hrows + (size_t)w * dim : ent + (size_t)hi * dim,
+                       SHARD ? a.trows + (size_t)w * dim : ent + (size_t)ti * dim,
+                       a.tb.rel0 + (size_t)ri * dim, dim, lane, pp, ab);
+  if (lane == 0 && a.pos_out && !BWD) a.pos_out[w] = pp.pos;
   const float g = BWD ? *gloss : 0.f;
   float loss = 0.f;
-  Vec Vt, Vh;
-#pragma unroll
-  for (int i = 0; i < FAST_NCH; ++i) Vt.c[i] = Vh.c[i] = make_float4(0.f, 0.f, 0.f, 0.f);
-  // per kind: the active hinges (margin) or the summed weights c_j.  The weights and dl/dpos are
-  // non-integers summed over up to thousands of negatives: in double, as fp32 would drift by ~n eps.
-  using Count = std::conditional_t<LOSS == KGE_LOSS_MARGIN, int, double>;
-  Count n_t = 0, n_h = 0;
-  double gpos_sum = 0.0;   // LOSS != margin: sum of dl/dpos over the ring's negatives
+  FastAcc<LOSS> acc;
   unsigned phases = 0u;   // bit s = parity of the next completion of slot s (a skipped use does not advance it)
   for (int j = 0; j < n_loop; ++j) {
     const unsigned code = codes[j];
     const long long idx = (long long)j * a.b + w;   // (unsharded: the negative's index in nh / nt / neg_out)
-    if (!SHARD && code == CODE_BOTH) {
-      // both ends replaced (possible with caller-supplied negatives only): generic path, no ring slot
-      const long long nh = a.nh[idx], nt = a.nt[idx];
-      const RowPtrs pn = make_rows(MODEL, dim, a.tb, nh, nt, ri);
-      const float neg = triple_score(MODEL, dim, pn, lane, nullptr, nullptr);
-      const float term = pair_loss_term(LOSS, a.margin, pos, neg);
-      if (lane == 0) {
-        if (!BWD && a.neg_out) a.neg_out[idx] = neg;
-        loss += term;
-      }
-      if constexpr (BWD) {
-        float gp, gn;   // g = 1; the margin loss: -1 and 1 on an active hinge
-        pair_loss_grads(LOSS, a.margin, 1.f, pos, neg, &gp, &gn);
-        if (gn != 0.f || gp != 0.f) {
-          triple_backward(MODEL, dim, pn, grad_rows(MODEL, dim, gr, nh, nt, ri),
-                          LOSS == KGE_LOSS_MARGIN ? g : g * gn, lane);
-          const RowPtrs pp = make_rows(MODEL, dim, a.tb, hi, ti, ri);
-          triple_backward(MODEL, dim, pp, grad_rows(MODEL, dim, gr, hi, ti, ri),
-                          LOSS == KGE_LOSS_MARGIN ? -g : g * gp, lane);
-        }
-      }
+    if (!SHARD && code == CODE_BOTH) {   // no ring slot
+      both_replaced_pair<MODEL, BWD, LOSS>(a, gr, hi, ti, ri, a.nh[idx], a.nt[idx], idx, pp.pos, g, lane, loss);
       if (lane == 0 && j + RING < n_loop) request(j + RING);
       continue;
     }
@@ -1045,100 +1064,18 @@ margin_step_ring_kernel(MarginStepParams a, TrainGrads gr, const float* __restri
     }
     const bool head = (code & 0x80000000u) != 0u;   // warp-uniform
     const long long e = (long long)(code & 0x7FFFFFFFu);
-    const Vec& P = head ? Bv : A;
-    float se = vec_dot(ev, ev), sp = vec_dot(ev, P);
-    warp_sum2(se, sp);
-    const float inv_e = 1.0f / fmaxf(sqrtf(se), NORM_EPS);
-    float neg, en_dot_G = 0.f;
-    Vec en;
-    if constexpr (MODEL == KGE_DISTMULT) {
-      neg = sp * inv_e;
-      en_dot_G = neg;
-    } else if constexpr (MODEL == KGE_TRANSE_L2) {
-      const float sP = head ? sB : sA;
-      const float ee = inv_e * inv_e * se, pe = inv_e * sp;
-      neg = -(sP - 2.f * pe + ee);
-      en_dot_G = 2.f * (pe - ee);
-    } else {
-      en = vec_scale(ev, inv_e);
-      float l1 = vec_l1_diff(P, en), eg = 0.f;
-      if (BWD) {
-        const Vec sg = vec_map(P, en, [](float p, float q) { return sgn(p - q); });
-        eg = vec_dot(en, sg);
-      }
-      warp_sum2(l1, eg);
-      neg = -l1;
-      en_dot_G = eg;
-    }
-    const float term = pair_loss_term(LOSS, a.margin, pos, neg);
-    if (lane == 0) {
-      if (!BWD && a.neg_out) a.neg_out[idx] = neg;
-      loss += term;
-    }
-    float gp = 0.f, cj = 0.f;   // dl/dpos and dl/dneg of this pair (g = 1)
-    if constexpr (BWD) pair_loss_grads(LOSS, a.margin, 1.f, pos, neg, &gp, &cj);
-    if constexpr (LOSS != KGE_LOSS_MARGIN) gpos_sum += gp;
-    if (BWD && cj != 0.f) {
-      // c_j = 1 on every active hinge of the margin loss: the weights drop out
-      const float wj = LOSS == KGE_LOSS_MARGIN ? 1.f : cj;
-      if constexpr (MODEL != KGE_TRANSE_L1) en = vec_scale(ev, inv_e);
-      Vec ge, V;
-      const float c = LOSS == KGE_LOSS_MARGIN ? g * inv_e : g * wj * inv_e;
-      if constexpr (MODEL == KGE_DISTMULT) {
-        ge = vec_map(P, en, [=](float p, float q) { return c * (p - q * en_dot_G); });
-        V = LOSS == KGE_LOSS_MARGIN ? en : vec_scale(en, wj);
-      } else if constexpr (MODEL == KGE_TRANSE_L2) {
-        ge = vec_map(P, en, [=](float p, float q) { return c * (2.f * (p - q) - q * en_dot_G); });
-        V = LOSS == KGE_LOSS_MARGIN ? en : vec_scale(en, wj);
-      } else {
-        V = vec_map(P, en, [](float p, float q) { return sgn(p - q); });
-        ge = vec_map(V, en, [=](float s_, float q) { return c * (s_ - q * en_dot_G); });
-        if constexpr (LOSS != KGE_LOSS_MARGIN) V = vec_scale(V, wj);
-      }
-      vec_atomic_add(gr.ent0 + (size_t)e * dim, dim, lane, ge);
-      const Count inc = LOSS == KGE_LOSS_MARGIN ? Count(1) : Count(wj);
-      if (head) { Vh = vec_map(Vh, V, [](float x, float y) { return x + y; }); n_h += inc; }
-      else { Vt = vec_map(Vt, V, [](float x, float y) { return x + y; }); n_t += inc; }
-    }
+    FastNeg n;
+    fast_negative<MODEL, BWD>(pp, ab, ev, head, n);
+    pair_forward<BWD, LOSS>(a, idx, lane, pp.pos, n.neg, loss);
+    if constexpr (BWD)
+      fast_negative_backward<MODEL, LOSS>(pp, ab, ev, head, n, a.margin, g, gr.ent0 + (size_t)e * dim, dim, lane, acc);
   }
-  if (!BWD) {
-    if (lane == 0) atomicAdd(a.loss, loss);
-    return;
-  }
-  if constexpr (LOSS == KGE_LOSS_MARGIN) {
-    if (n_t + n_h == 0) return;
-  } else {
-    if (n_t == 0.0 && n_h == 0.0 && gpos_sum == 0.0) return;
-  }
-  // fn: the positive's weight, -sum_j dl/dpos (the margin loss: the active count)
-  const float fn_t = (float)n_t, fn_h = (float)n_h;
-  const float fn = LOSS == KGE_LOSS_MARGIN ? (float)(n_t + n_h) : (float)-gpos_sum;
-  Vec Gh, Gt, Gr;
-  if constexpr (MODEL == KGE_DISTMULT) {
-    Gh = vec_map3(r, Vt, tn, [=](float rr, float vt, float tt) { return g * rr * (vt - fn * tt); });
-    Gt = vec_map3(r, Vh, hn, [=](float rr, float vh, float hh) { return g * rr * (vh - fn * hh); });
-    const Vec tmp = vec_map3(hn, Vt, tn, [=](float hh, float vt, float tt) { return hh * (vt - fn * tt); });
-    Gr = vec_map3(tmp, tn, Vh, [=](float x, float tt, float vh) { return g * (x + tt * vh); });
-  } else if constexpr (MODEL == KGE_TRANSE_L2) {
-    const Vec x = vec_map(A, tn, [](float p, float q) { return p - q; });
-    const Vec dt = vec_map3(A, Vt, x, [=](float aa, float vt, float xx) { return fn_t * aa - vt - fn * xx; });
-    const Vec dh = vec_map(Vh, Bv, [=](float vh, float bb) { return vh - fn_h * bb; });
-    Gh = vec_scale(dt, -2.f * g);
-    Gt = vec_map3(dh, x, x, [=](float d, float xx, float) { return 2.f * g * (d - fn * xx); });
-    Gr = vec_map(dt, dh, [=](float p, float q) { return -2.f * g * (p + q); });
-  } else {
-    const Vec sx = vec_map(A, tn, [](float p, float q) { return sgn(p - q); });
-    Gh = vec_map(Vt, sx, [=](float vt, float s_) { return g * (fn * s_ - vt); });
-    Gt = vec_map(Vh, sx, [=](float vh, float s_) { return g * (-vh - fn * s_); });
-    Gr = vec_map3(Vt, Vh, sx, [=](float vt, float vh, float s_) { return g * (vh - vt + fn * s_); });
-  }
-  float ph = vec_dot(hn, Gh), pt = vec_dot(tn, Gt);
-  warp_sum2(ph, pt);
-  const Vec gh = vec_map(Gh, hn, [=](float gg, float q) { return (gg - q * ph) * inv_h; });
-  const Vec gt = vec_map(Gt, tn, [=](float gg, float q) { return (gg - q * pt) * inv_t; });
-  vec_atomic_add(SHARD ? a.grad_hrows + (size_t)w * dim : gr.ent0 + (size_t)hi * dim, dim, lane, gh);
-  vec_atomic_add(SHARD ? a.grad_trows + (size_t)w * dim : gr.ent0 + (size_t)ti * dim, dim, lane, gt);
-  vec_atomic_add(gr.rel0 + (size_t)ri * dim, dim, lane, Gr);
+  if constexpr (BWD)
+    fast_positive_backward<MODEL, LOSS>(pp, ab, acc, g,
+                                        SHARD ? a.grad_hrows + (size_t)w * dim : gr.ent0 + (size_t)hi * dim,
+                                        SHARD ? a.grad_trows + (size_t)w * dim : gr.ent0 + (size_t)ti * dim,
+                                        gr.rel0 + (size_t)ri * dim, dim, lane);
+  else if (lane == 0) atomicAdd(a.loss, loss);
 }
 
 __host__ inline size_t ring_smem_bytes(const MarginStepParams& a) {
@@ -1198,44 +1135,24 @@ __host__ inline bool fast_step_ok(const MarginStepParams& a) {
          a.dim % 4 == 0 && a.dim <= FAST_MAX_DIM;
 }
 
-__global__ void margin_loss_fwd_kernel(const float* __restrict__ pos, const float* __restrict__ neg,
-                                       long long n, float margin, float* __restrict__ loss) {
+// MarginLoss, LogisticLoss, BinaryCrossEntropyLoss (utils/losses.py:12-112), sum-reduced: pair_loss_term /
+// pair_loss_grads element by element.  `margin` is read by the margin loss only.
+__global__ void pair_loss_fwd_kernel(int kind, float margin, const float* __restrict__ pos,
+                                     const float* __restrict__ neg, long long n, float* __restrict__ loss) {
   float s = 0.f;
   for (long long i = (long long)blockIdx.x * blockDim.x + threadIdx.x; i < n;
        i += (long long)gridDim.x * blockDim.x)
-    s += fmaxf(0.f, margin - pos[i] + neg[i]);
+    s += pair_loss_term(kind, margin, pos[i], neg[i]);
   s = warp_sum(s);
   if ((threadIdx.x & 31) == 0 && s != 0.f) atomicAdd(loss, s);
 }
 
-__global__ void margin_loss_bwd_kernel(const float* __restrict__ pos, const float* __restrict__ neg,
-                                       long long n, float margin, const float* __restrict__ gloss,
-                                       float* __restrict__ gpos, float* __restrict__ gneg) {
-  const long long i = (long long)blockIdx.x * blockDim.x + threadIdx.x;
-  if (i >= n) return;
-  const float g = (margin - pos[i] + neg[i] > 0.f) ? *gloss : 0.f;
-  gpos[i] = -g;
-  gneg[i] = g;
-}
-
-// LogisticLoss / BinaryCrossEntropyLoss (utils/losses.py:47-112), sum-reduced: pair_loss_term /
-// pair_loss_grads element by element.
-__global__ void pair_loss_fwd_kernel(int kind, const float* __restrict__ pos, const float* __restrict__ neg,
-                                     long long n, float* __restrict__ loss) {
-  float s = 0.f;
-  for (long long i = (long long)blockIdx.x * blockDim.x + threadIdx.x; i < n;
-       i += (long long)gridDim.x * blockDim.x)
-    s += pair_loss_term(kind, 0.f, pos[i], neg[i]);
-  s = warp_sum(s);
-  if ((threadIdx.x & 31) == 0 && s != 0.f) atomicAdd(loss, s);
-}
-
-__global__ void pair_loss_bwd_kernel(int kind, const float* __restrict__ pos, const float* __restrict__ neg,
-                                     long long n, const float* __restrict__ gloss,
+__global__ void pair_loss_bwd_kernel(int kind, float margin, const float* __restrict__ pos,
+                                     const float* __restrict__ neg, long long n, const float* __restrict__ gloss,
                                      float* __restrict__ gpos, float* __restrict__ gneg) {
   const long long i = (long long)blockIdx.x * blockDim.x + threadIdx.x;
   if (i >= n) return;
-  pair_loss_grads(kind, 0.f, *gloss, pos[i], neg[i], gpos + i, gneg + i);
+  pair_loss_grads(kind, margin, *gloss, pos[i], neg[i], gpos + i, gneg + i);
 }
 
 inline unsigned blocks_for_warps(long long warps) {
@@ -1255,7 +1172,8 @@ __global__ void scatter_rows_add_kernel(float* __restrict__ grad0, float* __rest
   const int pl = (int)(w - i * planes);
   const long long row = idx[i] - ent_lo;
   if (row < 0 || row >= n_rows) return;
-  float* dst = (pl == 0 ? grad0 : (pl == 1 ? grad1 : grad1 + (grad1 - grad0))) + (size_t)row * dim;
+  const Planes<float> p = table_planes(grad0, grad1, planes, (size_t)row * dim);
+  float* dst = pl == 0 ? p.p0 : (pl == 1 ? p.p1 : p.p2);
   const float* src = rows + (size_t)w * dim;
   for (int k = lane; k < dim; k += 32) atomicAdd(dst + k, src[k]);
 }
@@ -1347,34 +1265,18 @@ cudaError_t launch_margin_step_bwd(const MarginStepParams& a, const TrainGrads& 
   return launch_margin_step<true>(a, gr, gloss, st);
 }
 
-cudaError_t launch_margin_loss_fwd(const float* pos, const float* neg, int64_t n, float margin,
-                                   float* loss, cudaStream_t st) {
+cudaError_t launch_pair_loss_fwd(int kind, float margin, const float* pos, const float* neg, int64_t n,
+                                 float* loss, cudaStream_t st) {
   if (n <= 0) return cudaSuccess;
   const unsigned blocks = (unsigned)((n + 255) / 256 < 1184 ? (n + 255) / 256 : 1184);
-  margin_loss_fwd_kernel<<<blocks, 256, 0, st>>>(pos, neg, n, margin, loss);
+  pair_loss_fwd_kernel<<<blocks, 256, 0, st>>>(kind, margin, pos, neg, n, loss);
   return cudaGetLastError();
 }
 
-cudaError_t launch_pair_loss_fwd(int kind, const float* pos, const float* neg, int64_t n, float* loss,
-                                 cudaStream_t st) {
-  if (n <= 0) return cudaSuccess;
-  const unsigned blocks = (unsigned)((n + 255) / 256 < 1184 ? (n + 255) / 256 : 1184);
-  pair_loss_fwd_kernel<<<blocks, 256, 0, st>>>(kind, pos, neg, n, loss);
-  return cudaGetLastError();
-}
-
-cudaError_t launch_pair_loss_bwd(int kind, const float* pos, const float* neg, int64_t n,
+cudaError_t launch_pair_loss_bwd(int kind, float margin, const float* pos, const float* neg, int64_t n,
                                  const float* gloss, float* gpos, float* gneg, cudaStream_t st) {
   if (n <= 0) return cudaSuccess;
-  pair_loss_bwd_kernel<<<(unsigned)((n + 255) / 256), 256, 0, st>>>(kind, pos, neg, n, gloss, gpos, gneg);
-  return cudaGetLastError();
-}
-
-cudaError_t launch_margin_loss_bwd(const float* pos, const float* neg, int64_t n, float margin,
-                                   const float* gloss, float* gpos, float* gneg, cudaStream_t st) {
-  if (n <= 0) return cudaSuccess;
-  margin_loss_bwd_kernel<<<(unsigned)((n + 255) / 256), 256, 0, st>>>(pos, neg, n, margin, gloss,
-                                                                      gpos, gneg);
+  pair_loss_bwd_kernel<<<(unsigned)((n + 255) / 256), 256, 0, st>>>(kind, margin, pos, neg, n, gloss, gpos, gneg);
   return cudaGetLastError();
 }
 

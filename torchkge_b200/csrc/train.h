@@ -66,13 +66,11 @@ cudaError_t launch_margin_step_bwd(const MarginStepParams& a, const TrainGrads& 
                                    cudaStream_t st);
 cudaError_t launch_scatter_rows_add(float* grad0, float* grad1, int planes, int64_t ent_lo, int64_t n_rows,
                                     int dim, const int64_t* idx, int64_t n, const float* rows, cudaStream_t st);
-cudaError_t launch_margin_loss_fwd(const float* pos, const float* neg, int64_t n, float margin,
-                                   float* loss, cudaStream_t st);
-cudaError_t launch_pair_loss_fwd(int kind, const float* pos, const float* neg, int64_t n, float* loss,
-                                 cudaStream_t st);
-cudaError_t launch_pair_loss_bwd(int kind, const float* pos, const float* neg, int64_t n,
+// MarginLoss / LogisticLoss / BinaryCrossEntropyLoss on score arrays (kind: KGE_LOSS_*; margin is used by
+// the margin loss only)
+cudaError_t launch_pair_loss_fwd(int kind, float margin, const float* pos, const float* neg, int64_t n,
+                                 float* loss, cudaStream_t st);
+cudaError_t launch_pair_loss_bwd(int kind, float margin, const float* pos, const float* neg, int64_t n,
                                  const float* gloss, float* gpos, float* gneg, cudaStream_t st);
-cudaError_t launch_margin_loss_bwd(const float* pos, const float* neg, int64_t n, float margin,
-                                   const float* gloss, float* gpos, float* gneg, cudaStream_t st);
 
 }  // namespace kge
