@@ -438,6 +438,38 @@ int kge_margin_step_bwd(const kge_margin_step_args_t* a, const kge_grads_t* g,
 int kge_scatter_rows_add(int model, float* grad0, float* grad1, int64_t ent_lo, int64_t n_rows, int dim,
                          const int64_t* idx, int64_t n, const float* rows, void* stream);
 
+/* ---- relation-corrupting negatives (BernoulliRelationNegativeSampler, sampling.py:507-553) ----------
+ * kge_corrupt_batch_rel: nh / nt / nr of length b*n_neg in n_neg blocks of the batch.  Negative j of fact
+ * i keeps its entities and replaces its relation, uniform on [1, n_rel), with probability 1 - rel_share;
+ * otherwise it replaces the head with probability bern_probs[r[i]], else the tail, uniform on [1, n_ent),
+ * and keeps its relation.  Exactly one position changes; true triples are not rejected.  Philox4x32-10
+ * as kge_corrupt_batch (key = seed, counter = (j*b+i, offset)): words x, y decide and draw the entity as
+ * there, word z decides entity (below rel_share) or relation, word w draws the relation -- so
+ * rel_share = 1 gives kge_corrupt_batch's nh / nt.  0 <= rel_share <= 1; n_rel >= 2 unless rel_share = 1.
+ *
+ * kge_rel_step_fwd / _bwd: the fused step of kge_margin_step_fwd / _bwd with these negatives drawn in the
+ * kernel at (seed, offset), exactly as kge_corrupt_batch_rel draws them, or taken from base.nh / base.nt
+ * / nr (all three or none; any positions may change).  nr_out (optional, unsharded only) receives the
+ * relations of the negatives next to base.nh_out / base.nt_out.  A negative scores (nh, nt, nr); its
+ * gradient goes to those rows.  Entity-sharded (base.hrows != NULL): an entity negative is scored by the
+ * rank holding its replaced entity as in kge_margin_step_fwd, a relation negative by the rank holding the
+ * positive's HEAD, from hrows / trows, its entity gradients into grad_hrows / grad_trows and its relation
+ * gradient into g->rel0 / rel1 -- the buffers the caller already sums over the ranks.  The argument rules
+ * are those of kge_margin_step_fwd / _bwd, plus: n_rel >= 1, n_rel >= 2 unless rel_share >= 1,
+ * rel_share in [0, 1], nr non-NULL exactly when base.nh is, and nr / nr_out NULL when sharded. */
+int kge_corrupt_batch_rel(const int64_t* h, const int64_t* t, const int64_t* r, int64_t b, int32_t n_neg,
+                          const float* bern_probs, int64_t n_ent, int64_t n_rel, float rel_share, uint64_t seed,
+                          uint64_t offset, int64_t* nh, int64_t* nt, int64_t* nr, void* stream);
+typedef struct {
+  kge_margin_step_args_t base;
+  int64_t n_rel;                        /* relations in the table: the relation draw is uniform on [1, n_rel) */
+  float rel_share;                      /* probability that a negative replaces an entity */
+  const int64_t* nr;                    /* external negatives' relations (with base.nh / base.nt), or NULL */
+  int64_t* nr_out;                      /* optional: relations of the negatives (b*n_neg) */
+} kge_rel_step_args_t;
+int kge_rel_step_fwd(const kge_rel_step_args_t* a);
+int kge_rel_step_bwd(const kge_rel_step_args_t* a, const kge_grads_t* g, const float* grad_loss);
+
 /* ---- measurement hook ------------------------------------------------------------------
  * When enabled, the dominant kernels of kge_rank_side / kge_score_all are bracketed by CUDA
  * events recorded on the launch stream: kind 0 = scalar dense scan, 1 = tensor-core scan,

@@ -13,7 +13,7 @@ from .evaluation import (LinkPredictionEvaluator, RelationPredictionEvaluator,  
                          TripletClassificationEvaluator)
 from .inference import EntityInference, RelationInference  # noqa: F401
 from .losses import BinaryCrossEntropyLoss, LogisticLoss, MarginLoss  # noqa: F401
-from .sampling import (BernoulliNegativeSampler, PositionalNegativeSampler,  # noqa: F401
-                       UniformNegativeSampler)
+from .sampling import (BernoulliNegativeSampler, BernoulliRelationNegativeSampler,  # noqa: F401
+                       PositionalNegativeSampler, UniformNegativeSampler)
 
 __version__ = "0.1.0"

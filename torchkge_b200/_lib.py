@@ -96,6 +96,14 @@ class MarginStepArgs(ctypes.Structure):
     ]
 
 
+class RelStepArgs(ctypes.Structure):
+    """kge_rel_step_args_t"""
+    _fields_ = [
+        ("base", MarginStepArgs), ("n_rel", _c.c_int64), ("rel_share", _c.c_float),
+        ("nr", _p), ("nr_out", _p),
+    ]
+
+
 # name -> (restype, argtypes); every symbol include/kge_b200.h declares
 SIGNATURES = {
     "kge_abi_version": (_c.c_int, []),
@@ -141,6 +149,10 @@ SIGNATURES = {
     "kge_margin_step_bwd": (_c.c_int, [_c.POINTER(MarginStepArgs), _c.POINTER(Grads), _p]),
     "kge_scatter_rows_add": (_c.c_int, [_c.c_int, _p, _p, _c.c_int64, _c.c_int64, _c.c_int, _p, _c.c_int64,
                                         _p, _p]),
+    "kge_corrupt_batch_rel": (_c.c_int, [_p, _p, _p, _c.c_int64, _c.c_int32, _p, _c.c_int64, _c.c_int64,
+                                         _c.c_float, _c.c_uint64, _c.c_uint64, _p, _p, _p, _p]),
+    "kge_rel_step_fwd": (_c.c_int, [_c.POINTER(RelStepArgs)]),
+    "kge_rel_step_bwd": (_c.c_int, [_c.POINTER(RelStepArgs), _c.POINTER(Grads), _p]),
     "kge_scan_timing_enable": (_c.c_int, [_c.c_int]),
     "kge_scan_timing_read": (_c.c_int, [_c.c_int, _c.POINTER(_c.c_int64), _c.POINTER(_c.c_double)]),
 }

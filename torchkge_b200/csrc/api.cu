@@ -803,7 +803,17 @@ kge::MarginStepParams to_step(const kge_margin_step_args_t* a) {
   p.ent_lo = a->ent_lo; p.n_rows = a->n_rows; p.hrows = a->hrows; p.trows = a->trows;
   p.grad_hrows = a->grad_hrows; p.grad_trows = a->grad_trows;
   p.loss_kind = a->loss_kind;
+  p.n_rel = 0; p.rel_share = 1.f; p.nr = nullptr; p.nr_out = nullptr;   // the entity step
   return p;
+}
+kge::MarginStepParams to_rel_step(const kge_rel_step_args_t* a) {
+  kge::MarginStepParams p = to_step(&a->base);
+  p.n_rel = a->n_rel; p.rel_share = a->rel_share; p.nr = a->nr; p.nr_out = a->nr_out;
+  return p;
+}
+// n_rel >= 2 unless every negative replaces an entity; a NaN rel_share fails the range test
+bool rel_draw_ok(int64_t n_rel, float rel_share) {
+  return rel_share >= 0.f && rel_share <= 1.f && n_rel >= 1 && (n_rel >= 2 || rel_share >= 1.f);
 }
 // A shard that holds no rows (n_rows = 0) may pass no entity planes.
 bool step_tables_ok(const kge_margin_step_args_t* a) {
@@ -837,6 +847,12 @@ bool step_ok(const kge_margin_step_args_t* a) {
 }
 bool shard_grads_ok(const kge_margin_step_args_t* a) {
   return !a->hrows || (a->grad_hrows && a->grad_trows);
+}
+bool rel_step_ok(const kge_rel_step_args_t* a) {
+  if (!a || !step_ok(&a->base) || !rel_draw_ok(a->n_rel, a->rel_share)) return false;
+  if ((a->nr == nullptr) != (a->base.nh == nullptr)) return false;
+  if (a->base.hrows && a->nr_out) return false;   // sharded: no per-negative outputs
+  return true;
 }
 }  // namespace
 
@@ -941,6 +957,39 @@ int kge_margin_step_bwd(const kge_margin_step_args_t* a, const kge_grads_t* g,
   KGE_CUDA_TRY(kge::launch_margin_step_bwd(to_step(a), to_grads(g), grad_loss,
                                            static_cast<cudaStream_t>(a->stream)),
                "margin_step_bwd");
+  return KGE_OK;
+}
+
+int kge_corrupt_batch_rel(const int64_t* h, const int64_t* t, const int64_t* r, int64_t b, int32_t n_neg,
+                          const float* bern_probs, int64_t n_ent, int64_t n_rel, float rel_share, uint64_t seed,
+                          uint64_t offset, int64_t* nh, int64_t* nt, int64_t* nr, void* stream) {
+  if (b < 0 || n_neg < 1 || n_ent < 1 || !rel_draw_ok(n_rel, rel_share))
+    return fail(KGE_ERR_ARG, "kge_corrupt_batch_rel: bad argument");
+  if (b == 0) return KGE_OK;
+  if (!h || !t || !r || !bern_probs || !nh || !nt || !nr)
+    return fail(KGE_ERR_ARG, "kge_corrupt_batch_rel: null pointer");
+  DeviceScope device_scope(h);
+  KGE_CUDA_TRY(kge::launch_corrupt_batch_rel(h, t, r, b, n_neg, bern_probs, n_ent, n_rel, rel_share, seed, offset,
+                                             nh, nt, nr, static_cast<cudaStream_t>(stream)),
+               "corrupt_batch_rel");
+  return KGE_OK;
+}
+
+int kge_rel_step_fwd(const kge_rel_step_args_t* a) {
+  if (!rel_step_ok(a)) return fail(KGE_ERR_ARG, "kge_rel_step_fwd: bad argument");
+  DeviceScope device_scope(a->base.tb.ent0);
+  KGE_CUDA_TRY(kge::launch_margin_step_fwd(to_rel_step(a), static_cast<cudaStream_t>(a->base.stream)),
+               "rel_step_fwd");
+  return KGE_OK;
+}
+
+int kge_rel_step_bwd(const kge_rel_step_args_t* a, const kge_grads_t* g, const float* grad_loss) {
+  if (!rel_step_ok(a) || !step_grads_ok(&a->base, g) || !grad_loss || !shard_grads_ok(&a->base))
+    return fail(KGE_ERR_ARG, "kge_rel_step_bwd: bad argument");
+  DeviceScope device_scope(a->base.tb.ent0);
+  KGE_CUDA_TRY(kge::launch_margin_step_bwd(to_rel_step(a), to_grads(g), grad_loss,
+                                           static_cast<cudaStream_t>(a->base.stream)),
+               "rel_step_bwd");
   return KGE_OK;
 }
 

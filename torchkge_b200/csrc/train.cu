@@ -81,6 +81,43 @@ __device__ __forceinline__ void corrupt_one(uint64_t seed, uint64_t offset, uint
   *nt = head ? t : e;
 }
 
+// The draw of one relation-corrupting negative (BernoulliRelationNegativeSampler, sampling.py:507-553).
+// Words x and y are those of draw_one: Bernoulli(p_r) decides head vs tail, the entity is uniform on
+// [1, n_ent).  Word z decides entity (u < rel_share) vs relation; word w picks the relation, uniform on
+// [1, n_rel).  Since u < 1 always, rel_share = 1 gives draw_one's draws.  Returns the kind.
+constexpr int NEG_TAIL = 0, NEG_HEAD = 1, NEG_REL = 2;
+
+__device__ __forceinline__ int draw_rel(uint64_t seed, uint64_t offset, uint64_t idx, float p, float rel_share,
+                                        long long n_ent, long long n_rel, long long* e_out) {
+  const uint4 rnd = philox4x32(seed, offset, idx);
+  const float u_ent = (rnd.z >> 8) * (1.0f / 16777216.0f);
+  if (!(u_ent < rel_share)) {
+    const long long span = n_rel - 1;
+    long long r = 1;
+    if (span > 0) r = 1 + (long long)(((unsigned long long)rnd.w * (unsigned long long)span) >> 32);
+    *e_out = r;
+    return NEG_REL;
+  }
+  const float u = (rnd.x >> 8) * (1.0f / 16777216.0f);
+  const long long span = n_ent - 1;
+  long long e = 1;
+  if (span > 0) e = 1 + (long long)(((unsigned long long)rnd.y * (unsigned long long)span) >> 32);
+  *e_out = e;
+  return u < p ? NEG_HEAD : NEG_TAIL;
+}
+
+// One corrupted triple (nh, nt, nr) of the positive (h, t, r).
+__device__ __forceinline__ void corrupt_one_rel(uint64_t seed, uint64_t offset, uint64_t idx, float p,
+                                                float rel_share, long long n_ent, long long n_rel, long long h,
+                                                long long t, long long r, long long* nh, long long* nt,
+                                                long long* nr) {
+  long long e;
+  const int kind = draw_rel(seed, offset, idx, p, rel_share, n_ent, n_rel, &e);
+  *nh = kind == NEG_HEAD ? e : h;
+  *nt = kind == NEG_TAIL ? e : t;
+  *nr = kind == NEG_REL ? e : r;
+}
+
 // ------------------------------------------------------------------------------------------
 // Per-lane view of one triple.  Lane l owns embedding indices l, l+32, ...; `cnt` of them.
 // RowPtrs: the rows it is scored from.  GradRows: the destination rows of its gradient, plane by
@@ -379,6 +416,34 @@ __global__ void corrupt_batch_kernel(const int64_t* __restrict__ h, const int64_
   nh[gid] = a; nt[gid] = c;
 }
 
+__global__ void corrupt_batch_rel_kernel(const int64_t* __restrict__ h, const int64_t* __restrict__ t,
+                                         const int64_t* __restrict__ r, long long b, int n_neg,
+                                         const float* __restrict__ probs, long long n_ent, long long n_rel,
+                                         float rel_share, uint64_t seed, uint64_t offset, int64_t* __restrict__ nh,
+                                         int64_t* __restrict__ nt, int64_t* __restrict__ nr) {
+  const long long gid = (long long)blockIdx.x * blockDim.x + threadIdx.x;
+  if (gid >= b * n_neg) return;
+  const long long i = gid % b;
+  long long a, c, q;
+  corrupt_one_rel(seed, offset, (uint64_t)gid, probs[r[i]], rel_share, n_ent, n_rel, h[i], t[i], r[i], &a, &c, &q);
+  nh[gid] = a; nt[gid] = c; nr[gid] = q;
+}
+
+// Negative idx of the positive (hi, ti, ri) in the generic kernels: the caller's (nh, nt[, nr]), else a
+// Philox draw -- draw_rel in a relation-corrupting step (a.n_rel > 0), draw_one otherwise.
+__device__ __forceinline__ void step_negative(const MarginStepParams& a, long long idx, float p_head, long long hi,
+                                              long long ti, long long ri, long long* nh, long long* nt,
+                                              long long* nr) {
+  if (a.nh) {
+    *nh = a.nh[idx]; *nt = a.nt[idx]; *nr = a.nr ? a.nr[idx] : ri;
+  } else if (a.n_rel > 0) {
+    corrupt_one_rel(a.seed, a.offset, (uint64_t)idx, p_head, a.rel_share, a.n_ent, a.n_rel, hi, ti, ri, nh, nt, nr);
+  } else {
+    corrupt_one(a.seed, a.offset, (uint64_t)idx, p_head, a.n_ent, hi, ti, nh, nt);
+    *nr = ri;
+  }
+}
+
 // ---- per-pair loss terms: the one statement of each loss, used by pair_loss_fwd / _bwd_kernel and
 // by every fused step (kind: KGE_LOSS_*, a runtime value or a template constant).
 //   margin  : max(0, margin - pos + neg)                    (MarginRankingLoss, target +1, sum)
@@ -432,14 +497,14 @@ __global__ void margin_step_fwd_kernel(MarginStepParams a) {
   float loss = 0.f;
   for (int j = 0; j < a.n_neg; ++j) {
     const long long idx = (long long)j * a.b + w;
-    long long nh, nt;
-    if (a.nh) { nh = a.nh[idx]; nt = a.nt[idx]; }
-    else corrupt_one(a.seed, a.offset, (uint64_t)idx, p_head, a.n_ent, hi, ti, &nh, &nt);
-    const RowPtrs pn = table_rows(a.model, a.dim, a.tb, nh, nt, ri);
+    long long nh, nt, nr;
+    step_negative(a, idx, p_head, hi, ti, ri, &nh, &nt, &nr);
+    const RowPtrs pn = table_rows(a.model, a.dim, a.tb, nh, nt, nr);
     const float neg = triple_score(a.model, a.dim, pn, lane, nullptr, nullptr);
     if (lane == 0) {
       if (a.neg_out) a.neg_out[idx] = neg;
       if (a.nh_out) { a.nh_out[idx] = nh; a.nt_out[idx] = nt; }
+      if (a.nr_out) a.nr_out[idx] = nr;
       loss += pair_loss_term(a.loss_kind, a.margin, pos, neg);
     }
   }
@@ -461,15 +526,14 @@ __global__ void margin_step_bwd_kernel(MarginStepParams a, TrainGrads gr, const 
   double gpos_sum = 0.0;   // thousands of non-integer dl/dpos terms (logistic, BCE): fp32 would drift
   for (int j = 0; j < a.n_neg; ++j) {
     const long long idx = (long long)j * a.b + w;
-    long long nh, nt;
-    if (a.nh) { nh = a.nh[idx]; nt = a.nt[idx]; }
-    else corrupt_one(a.seed, a.offset, (uint64_t)idx, p_head, a.n_ent, hi, ti, &nh, &nt);
-    const RowPtrs pn = table_rows(a.model, a.dim, a.tb, nh, nt, ri);
+    long long nh, nt, nr;
+    step_negative(a, idx, p_head, hi, ti, ri, &nh, &nt, &nr);
+    const RowPtrs pn = table_rows(a.model, a.dim, a.tb, nh, nt, nr);
     const float neg = triple_score(a.model, a.dim, pn, lane, nullptr, nullptr);
     float gp, gn;
     pair_loss_grads(a.loss_kind, a.margin, 1.f, pos, neg, &gp, &gn);
     gpos_sum += gp;
-    triple_backward(a.model, a.dim, pn, table_rows(a.model, a.dim, gr, nh, nt, ri), g * gn, lane);
+    triple_backward(a.model, a.dim, pn, table_rows(a.model, a.dim, gr, nh, nt, nr), g * gn, lane);
   }
   triple_backward(a.model, a.dim, pp, table_rows(a.model, a.dim, gr, hi, ti, ri), g * (float)gpos_sum, lane);
 }
@@ -501,6 +565,31 @@ __device__ __forceinline__ bool owned_draw(const MarginStepParams& a, long long 
   return (unsigned long long)*loc < (unsigned long long)a.n_rows;
 }
 
+// Negative idx of positive w in a sharded step: its kind (NEG_*), its relation nr and, if this rank scores
+// it, true with loc = the local row of its replaced entity.  A relation-corrupting negative (a.n_rel > 0)
+// is scored by the rank that holds the positive's head: its h / t rows are hrows / trows[w], so its
+// entity gradients land in grad_hrows / grad_trows, which the ranks sum like every other.
+__device__ __forceinline__ bool owned_negative(const MarginStepParams& a, long long w, long long idx, float p_head,
+                                               long long ri, int* kind, long long* loc, long long* nr) {
+  *nr = ri;
+  if (a.n_rel == 0) {
+    bool head;
+    const bool own = owned_draw(a, idx, p_head, &head, loc);
+    *kind = head ? NEG_HEAD : NEG_TAIL;
+    return own;
+  }
+  long long e;
+  *kind = draw_rel(a.seed, a.offset, (uint64_t)idx, p_head, a.rel_share, a.n_ent, a.n_rel, &e);
+  if (*kind == NEG_REL) *nr = e;
+  *loc = (*kind == NEG_REL ? a.h[w] : e) - a.ent_lo;
+  return (unsigned long long)*loc < (unsigned long long)a.n_rows;
+}
+
+__device__ __forceinline__ RowPtrs shard_kind_rows(const MarginStepParams& a, long long w, long long nr, int kind,
+                                                   long long loc) {
+  return kind == NEG_REL ? shard_pos_rows(a, w, nr) : shard_neg_rows(a, w, nr, kind == NEG_HEAD, loc);
+}
+
 __global__ void margin_step_shard_fwd_kernel(MarginStepParams a) {
   const long long w = ((long long)blockIdx.x * blockDim.x + threadIdx.x) >> 5;
   const int lane = threadIdx.x & 31;
@@ -510,10 +599,10 @@ __global__ void margin_step_shard_fwd_kernel(MarginStepParams a) {
   const float p_head = a.probs[ri];
   float loss = 0.f;
   for (int j = 0; j < a.n_neg; ++j) {
-    bool head;
-    long long loc;
-    if (!owned_draw(a, (long long)j * a.b + w, p_head, &head, &loc)) continue;
-    const float neg = triple_score(a.model, a.dim, shard_neg_rows(a, w, ri, head, loc), lane, nullptr, nullptr);
+    int kind;
+    long long loc, nr;
+    if (!owned_negative(a, w, (long long)j * a.b + w, p_head, ri, &kind, &loc, &nr)) continue;
+    const float neg = triple_score(a.model, a.dim, shard_kind_rows(a, w, nr, kind, loc), lane, nullptr, nullptr);
     if (lane == 0) loss += pair_loss_term(a.loss_kind, a.margin, pos, neg);
   }
   if (lane == 0) atomicAdd(a.loss, loss);
@@ -538,14 +627,20 @@ __global__ void margin_step_shard_bwd_kernel(MarginStepParams a, TrainGrads gr, 
   const Planes<float> grel = rel_planes(a.model, a.dim, gr.rel0, gr.rel1, ri);
   double gpos_sum = 0.0;   // as in margin_step_bwd_kernel
   for (int j = 0; j < a.n_neg; ++j) {
-    bool head;
-    long long loc;
-    if (!owned_draw(a, (long long)j * a.b + w, p_head, &head, &loc)) continue;
-    const RowPtrs pn = shard_neg_rows(a, w, ri, head, loc);
+    int kind;
+    long long loc, nr;
+    if (!owned_negative(a, w, (long long)j * a.b + w, p_head, ri, &kind, &loc, &nr)) continue;
+    const RowPtrs pn = shard_kind_rows(a, w, nr, kind, loc);
     const float neg = triple_score(a.model, a.dim, pn, lane, nullptr, nullptr);
     float gp, gn;
     pair_loss_grads(a.loss_kind, a.margin, 1.f, pos, neg, &gp, &gn);
     gpos_sum += gp;
+    if (kind == NEG_REL) {
+      triple_backward(a.model, a.dim, pn, rows_of(gh, gt, rel_planes(a.model, a.dim, gr.rel0, gr.rel1, nr)), g * gn,
+                      lane);
+      continue;
+    }
+    const bool head = kind == NEG_HEAD;
     const Planes<float> ge = table_planes(gr.ent0, gr.ent1, np, (size_t)loc * a.dim);
     triple_backward(a.model, a.dim, pn, rows_of(head ? ge : gh, head ? gt : ge, grel), g * gn, lane);
   }
@@ -573,7 +668,8 @@ __global__ void margin_step_shard_bwd_kernel(MarginStepParams a, TrainGrads gr, 
 // again (recomputed, not stored) plus one RMW of each (SURVEY.md section 8d).
 //
 // That arithmetic is stated once, in fast_positive / fast_negative / fast_negative_backward /
-// fast_positive_backward below (both_replaced_pair is the one case outside the closed form).  Two
+// fast_positive_backward below, with the relation kind in fast_rel_negative / fast_rel_negative_backward
+// (both_replaced_pair is the one case outside the closed form).  Two
 // kernels run it, margin_step_fast_kernel and margin_step_ring_kernel: they differ only in how a
 // negative's identity and row reach the warp, and that is all their bodies contain.
 // ------------------------------------------------------------------------------------------
@@ -791,20 +887,106 @@ __device__ __forceinline__ void fast_negative_backward(const FastPos& p, const F
   else { acc.Vt = vec_map(acc.Vt, V, [](float x, float y) { return x + y; }); acc.n_t += inc; }
 }
 
-// Backward of the positive, once: gradients with respect to hn, tn, r (+g c_j per negative, -g fn for
-// the positive), through the normalisation, added into the three destination rows.
+// The relation kind (BernoulliRelationNegativeSampler): a negative (h, t, r') keeps the positive's entities,
+// so it is scored from its relation row r' against C, a function of the positive's hn and tn alone:
+//     DistMult: neg = C . r',  C = hn * tn        TransE: neg = -|C + r'|,  C = hn - tn
+// (TransE-L2 expands |C + r'|^2 = |C|^2 + 2 C.r' + |r'|^2).  C costs a few lane-local flops, so it is formed
+// where it is used rather than held next to A and Bv.  The relation row is not normalised.
+template <int MODEL>
+__device__ __forceinline__ Vec rel_C(const FastPos& p) {
+  if constexpr (MODEL == KGE_DISTMULT) return vec_map(p.hn, p.tn, [](float x, float y) { return x * y; });
+  else return vec_map(p.hn, p.tn, [](float x, float y) { return x - y; });
+}
+
+// What the backward sums over the relation negatives: W = sum_j c_j r'_j (TransE-L1: of c_j sign(C + r'_j))
+// and their summed weights.  The positive's hn / tn gradients from them are linear in W (and n_r).
+template <int LOSS>
+struct FastRelAcc {
+  using Count = typename FastAcc<LOSS>::Count;
+  Vec W;
+  Count n_r = 0;
+  float sC = 0.f;          // |C|^2 (TransE-L2), set with the positive
+  __device__ __forceinline__ FastRelAcc() {
+#pragma unroll
+    for (int i = 0; i < FAST_NCH; ++i) W.c[i] = make_float4(0.f, 0.f, 0.f, 0.f);
+  }
+};
+
 template <int MODEL, int LOSS>
+__device__ __forceinline__ void fast_rel_positive(const FastPos& p, FastRelAcc<LOSS>& rl) {
+  if constexpr (MODEL == KGE_TRANSE_L2) {
+    const Vec C = rel_C<MODEL>(p);
+    rl.sC = warp_sum(vec_dot(C, C));
+  }
+}
+
+// One relation negative, scored from its relation row rv.
+template <int MODEL, int LOSS>
+__device__ __forceinline__ void fast_rel_negative(const FastPos& p, const FastRelAcc<LOSS>& rl, const Vec& rv,
+                                                  FastNeg& n) {
+  const Vec C = rel_C<MODEL>(p);
+  n.inv_e = 1.f;
+  n.en_dot_G = 0.f;
+  if constexpr (MODEL == KGE_DISTMULT) {
+    n.neg = warp_sum(vec_dot(C, rv));
+  } else if constexpr (MODEL == KGE_TRANSE_L2) {
+    float se = vec_dot(rv, rv), sp = vec_dot(rv, C);
+    warp_sum2(se, sp);
+    n.neg = -(rl.sC + 2.f * sp + se);
+  } else {
+    n.neg = -warp_sum(vec_l1_diff(C, vec_scale(rv, -1.f)));
+  }
+}
+
+// Backward of one relation negative: g c_j d neg / d r' goes to its relation row dst at once; c_j r'_j
+// (TransE-L1: c_j sign(C + r'_j)) and c_j go into rl, dl/dpos into acc.
+template <int MODEL, int LOSS>
+__device__ __forceinline__ void fast_rel_negative_backward(const FastPos& p, const Vec& rv, const FastNeg& n,
+                                                           float margin, float g, float* dst, int dim, int lane,
+                                                           FastAcc<LOSS>& acc, FastRelAcc<LOSS>& rl) {
+  float gp, cj;
+  pair_loss_grads(LOSS, margin, 1.f, p.pos, n.neg, &gp, &cj);
+  if constexpr (LOSS != KGE_LOSS_MARGIN) acc.gpos_sum += gp;
+  if (cj == 0.f) return;
+  const float wj = LOSS == KGE_LOSS_MARGIN ? 1.f : cj;
+  const float c = g * wj;
+  const Vec C = rel_C<MODEL>(p);
+  Vec gr, V;
+  if constexpr (MODEL == KGE_DISTMULT) {
+    gr = vec_scale(C, c);
+    V = LOSS == KGE_LOSS_MARGIN ? rv : vec_scale(rv, wj);
+  } else if constexpr (MODEL == KGE_TRANSE_L2) {
+    gr = vec_map(C, rv, [=](float a_, float q) { return -2.f * c * (a_ + q); });
+    V = LOSS == KGE_LOSS_MARGIN ? rv : vec_scale(rv, wj);
+  } else {
+    const Vec sg = vec_map(C, rv, [](float a_, float q) { return sgn(a_ + q); });
+    gr = vec_scale(sg, -c);
+    V = LOSS == KGE_LOSS_MARGIN ? sg : vec_scale(sg, wj);
+  }
+  vec_atomic_add(dst, dim, lane, gr);
+  using Count = typename FastAcc<LOSS>::Count;
+  rl.W = vec_map(rl.W, V, [](float x, float y) { return x + y; });
+  rl.n_r += LOSS == KGE_LOSS_MARGIN ? Count(1) : Count(wj);
+}
+
+// Backward of the positive, once: gradients with respect to hn, tn, r (+g c_j per negative, -g fn for
+// the positive), through the normalisation, added into the three destination rows.  REL: the relation
+// negatives' hn / tn terms too, from rl.
+template <int MODEL, int LOSS, bool REL = false>
 __device__ __forceinline__ void fast_positive_backward(const FastPos& p, const FastAB& ab, const FastAcc<LOSS>& acc,
                                                        float g, float* dst_h, float* dst_t, float* dst_r,
-                                                       int dim, int lane) {
+                                                       int dim, int lane, const FastRelAcc<LOSS>* rl = nullptr) {
+  using Count = typename FastAcc<LOSS>::Count;
+  Count n_r = 0;
+  if constexpr (REL) n_r = rl->n_r;
   if constexpr (LOSS == KGE_LOSS_MARGIN) {
-    if (acc.n_t + acc.n_h == 0) return;
+    if (acc.n_t + acc.n_h + n_r == 0) return;
   } else {
-    if (acc.n_t == 0.0 && acc.n_h == 0.0 && acc.gpos_sum == 0.0) return;
+    if (acc.n_t == 0.0 && acc.n_h == 0.0 && n_r == 0.0 && acc.gpos_sum == 0.0) return;
   }
   // fn: the positive's weight, -sum_j dl/dpos (the margin loss: the active count)
   const float fn_t = (float)acc.n_t, fn_h = (float)acc.n_h;
-  const float fn = LOSS == KGE_LOSS_MARGIN ? (float)(acc.n_t + acc.n_h) : (float)-acc.gpos_sum;
+  const float fn = LOSS == KGE_LOSS_MARGIN ? (float)(acc.n_t + acc.n_h + n_r) : (float)-acc.gpos_sum;
   const Vec& Vt = acc.Vt;
   const Vec& Vh = acc.Vh;
   Vec Gh, Gt, Gr;
@@ -830,6 +1012,27 @@ __device__ __forceinline__ void fast_positive_backward(const FastPos& p, const F
     Gt = vec_map(Vh, sx, [=](float vh, float s_) { return g * (-vh - fn * s_); });
     Gr = vec_map3(Vt, Vh, sx, [=](float vt, float vh, float s_) { return g * (vh - vt + fn * s_); });
   }
+  if constexpr (REL) {
+    // relation negatives: d neg / d hn = tn r' (DistMult), -2 (C + r') (TransE-L2), -sign(C + r') (L1);
+    // d neg / d tn the same with hn for tn (DistMult) or the opposite sign (TransE)
+    const Vec& W = rl->W;
+    Vec Q;
+    if constexpr (MODEL == KGE_DISTMULT) {
+      Q = W;
+    } else if constexpr (MODEL == KGE_TRANSE_L2) {
+      const float fr = (float)n_r;
+      Q = vec_map(rel_C<MODEL>(p), W, [=](float cc, float w_) { return -2.f * (fr * cc + w_); });
+    } else {
+      Q = vec_scale(W, -1.f);
+    }
+    if constexpr (MODEL == KGE_DISTMULT) {
+      Gh = vec_map3(Gh, p.tn, Q, [=](float a_, float tt, float q) { return a_ + g * tt * q; });
+      Gt = vec_map3(Gt, p.hn, Q, [=](float a_, float hh, float q) { return a_ + g * hh * q; });
+    } else {
+      Gh = vec_map(Gh, Q, [=](float a_, float q) { return a_ + g * q; });
+      Gt = vec_map(Gt, Q, [=](float a_, float q) { return a_ - g * q; });
+    }
+  }
   float ph = vec_dot(p.hn, Gh), pt = vec_dot(p.tn, Gt);
   warp_sum2(ph, pt);
   const float inv_h = p.inv_h, inv_t = p.inv_t;
@@ -840,21 +1043,22 @@ __device__ __forceinline__ void fast_positive_backward(const FastPos& p, const F
   vec_atomic_add(dst_r, dim, lane, Gr);
 }
 
-// A negative with both ends replaced (possible with caller-supplied negatives only) is outside the
-// closed form: the generic score, and in the backward the generic gradients of the negative and of
+// A negative with more than one position replaced (possible with caller-supplied negatives only) is outside
+// the closed form: the generic score, and in the backward the generic gradients of the negative and of
 // the positive for this pair alone.
 template <int MODEL, bool BWD, int LOSS>
 __device__ __forceinline__ void both_replaced_pair(const MarginStepParams& a, const TrainGrads& gr, long long hi,
                                                    long long ti, long long ri, long long nh, long long nt,
-                                                   long long idx, float pos, float g, int lane, float& loss) {
-  const RowPtrs pn = table_rows(MODEL, a.dim, a.tb, nh, nt, ri);
+                                                   long long idx, float pos, float g, int lane, float& loss,
+                                                   long long nr) {
+  const RowPtrs pn = table_rows(MODEL, a.dim, a.tb, nh, nt, nr);
   const float neg = triple_score(MODEL, a.dim, pn, lane, nullptr, nullptr);
   pair_forward<BWD, LOSS>(a, idx, lane, pos, neg, loss);
   if constexpr (BWD) {
     float gp, gn;   // g = 1; the margin loss: -1 and 1 on an active hinge
     pair_loss_grads(LOSS, a.margin, 1.f, pos, neg, &gp, &gn);
     if (gn != 0.f || gp != 0.f) {
-      triple_backward(MODEL, a.dim, pn, table_rows(MODEL, a.dim, gr, nh, nt, ri),
+      triple_backward(MODEL, a.dim, pn, table_rows(MODEL, a.dim, gr, nh, nt, nr),
                       LOSS == KGE_LOSS_MARGIN ? g : g * gn, lane);
       const RowPtrs pp = table_rows(MODEL, a.dim, a.tb, hi, ti, ri);
       triple_backward(MODEL, a.dim, pp, table_rows(MODEL, a.dim, gr, hi, ti, ri),
@@ -916,7 +1120,7 @@ margin_step_fast_kernel(MarginStepParams a, TrainGrads gr, const float* __restri
         const long long nh = nhs[u], nt = nts[u];
         const long long idx = (long long)(j0 + jj0 + u) * a.b + w;
         if (nh != hi && nt != ti) {
-          both_replaced_pair<MODEL, BWD, LOSS>(a, gr, hi, ti, ri, nh, nt, idx, pp.pos, g, lane, loss);
+          both_replaced_pair<MODEL, BWD, LOSS>(a, gr, hi, ti, ri, nh, nt, idx, pp.pos, g, lane, loss, ri);
           continue;
         }
         const bool head = nh != hi;            // warp-uniform
@@ -966,9 +1170,13 @@ __device__ __forceinline__ Vec vec_load_smem(const float* row, int dim, int lane
 // prefix, local row numbers in `codes`), so the ring streams owned rows only, and the positive's
 // gradients go to grad_hrows / grad_trows[w].
 // LOSS: KGE_LOSS_*; it turns the backward's counts into weights (FastAcc).
-template <int MODEL, bool BWD, int MINB = 0, bool SHARD = false, int LOSS = KGE_LOSS_MARGIN>
-__global__ void __launch_bounds__(WARPS_PER_BLOCK * 32, MINB == 0 ? 1 : MINB)
-margin_step_ring_kernel(MarginStepParams a, TrainGrads gr, const float* __restrict__ gloss) {
+// REL: the relation-corrupting step (a.n_rel > 0, margin_step_ring_rel_kernel).  A relation negative's
+// code carries CODE_REL and its relation; its row streams through the same ring from the relation table.
+// SHARD: the rank holding the positive's head scores it.  Codes then hold 30-bit row numbers.
+constexpr unsigned CODE_REL = 0x40000000u;
+
+template <int MODEL, bool BWD, bool SHARD, int LOSS, bool REL>
+__device__ __forceinline__ void ring_step(const MarginStepParams& a, const TrainGrads& gr, const float* gloss) {
   extern __shared__ __align__(128) unsigned char ring_smem[];
   const int warp_in_block = threadIdx.x >> 5, lane = threadIdx.x & 31;
   const long long w = (long long)blockIdx.x * WARPS_PER_BLOCK + warp_in_block;
@@ -989,20 +1197,35 @@ margin_step_ring_kernel(MarginStepParams a, TrainGrads gr, const float* __restri
   const float* __restrict__ ent = a.tb.ent0;
   const long long hi = a.h[w], ti = a.t[w], ri = a.r[w];
   const float p_head = a.nh ? 0.f : a.probs[ri];
-  // ---- all corruptions of this positive, up front: code = entity | head flag ----
+  constexpr unsigned ROW_MASK = REL ? 0x3FFFFFFFu : 0x7FFFFFFFu;
+  // ---- all corruptions of this positive, up front: code = entity | head flag (REL: or relation | CODE_REL) ----
   int n_loop = a.n_neg;            // SHARD: the owned negatives, compacted to the front of `codes`
   if constexpr (SHARD) {
     n_loop = 0;
+    const bool own_head = (unsigned long long)(hi - a.ent_lo) < (unsigned long long)a.n_rows;
     for (int j0 = 0; j0 < a.n_neg; j0 += 32) {
       const int j = j0 + lane;
       bool own = false;
       unsigned code = 0u;
       if (j < a.n_neg) {
+        const uint64_t idx = (uint64_t)((long long)j * a.b + w);
         long long e;
-        const bool head = draw_one(a.seed, a.offset, (uint64_t)((long long)j * a.b + w), p_head, a.n_ent, &e);
-        const unsigned long long loc = (unsigned long long)(e - a.ent_lo);
-        own = loc < (unsigned long long)a.n_rows;      // n_rows < 2^31 (ring_step_ok)
-        code = (unsigned)loc | (head ? 0x80000000u : 0u);
+        if constexpr (REL) {
+          const int kind = draw_rel(a.seed, a.offset, idx, p_head, a.rel_share, a.n_ent, a.n_rel, &e);
+          if (kind == NEG_REL) {
+            own = own_head;
+            code = (unsigned)e | CODE_REL;
+          } else {
+            const unsigned long long loc = (unsigned long long)(e - a.ent_lo);
+            own = loc < (unsigned long long)a.n_rows;
+            code = (unsigned)loc | (kind == NEG_HEAD ? 0x80000000u : 0u);
+          }
+        } else {
+          const bool head = draw_one(a.seed, a.offset, idx, p_head, a.n_ent, &e);
+          const unsigned long long loc = (unsigned long long)(e - a.ent_lo);
+          own = loc < (unsigned long long)a.n_rows;      // n_rows < 2^31 (ring_step_ok)
+          code = (unsigned)loc | (head ? 0x80000000u : 0u);
+        }
       }
       const unsigned ball = __ballot_sync(0xffffffffu, own);
       if (own) codes[n_loop + __popc(ball & ((1u << lane) - 1u))] = code;
@@ -1014,11 +1237,23 @@ margin_step_ring_kernel(MarginStepParams a, TrainGrads gr, const float* __restri
       if (j < a.n_neg) {
         const long long idx = (long long)j * a.b + w;
         long long nh = hi, nt = ti;
-        if (a.nh) { nh = a.nh[idx]; nt = a.nt[idx]; }
-        else corrupt_one(a.seed, a.offset, (uint64_t)idx, p_head, a.n_ent, hi, ti, &nh, &nt);
-        if (!BWD && a.nh_out) { a.nh_out[idx] = nh; a.nt_out[idx] = nt; }
-        const bool head = nh != hi;
-        codes[j] = (nh != hi && nt != ti) ? CODE_BOTH : ((unsigned)(head ? nh : nt) | (head ? 0x80000000u : 0u));
+        if constexpr (REL) {
+          long long nr = ri;
+          step_negative(a, idx, p_head, hi, ti, ri, &nh, &nt, &nr);
+          if (!BWD && a.nh_out) { a.nh_out[idx] = nh; a.nt_out[idx] = nt; }
+          if (!BWD && a.nr_out) a.nr_out[idx] = nr;
+          const int changed = (nh != hi) + (nt != ti) + (nr != ri);
+          const bool head = nh != hi;
+          codes[j] = changed > 1 ? CODE_BOTH
+                     : nr != ri ? ((unsigned)nr | CODE_REL)
+                                : ((unsigned)(head ? nh : nt) | (head ? 0x80000000u : 0u));
+        } else {
+          if (a.nh) { nh = a.nh[idx]; nt = a.nt[idx]; }
+          else corrupt_one(a.seed, a.offset, (uint64_t)idx, p_head, a.n_ent, hi, ti, &nh, &nt);
+          if (!BWD && a.nh_out) { a.nh_out[idx] = nh; a.nt_out[idx] = nt; }
+          const bool head = nh != hi;
+          codes[j] = (nh != hi && nt != ti) ? CODE_BOTH : ((unsigned)(head ? nh : nt) | (head ? 0x80000000u : 0u));
+        }
       }
     }
   }
@@ -1027,8 +1262,9 @@ margin_step_ring_kernel(MarginStepParams a, TrainGrads gr, const float* __restri
     const unsigned code = codes[j];
     if (!SHARD && code == CODE_BOTH) return;
     const int slot = j % RING;
+    const float* src = REL && (code & CODE_REL) ? a.tb.rel0 : ent;
     ptx::mbar_arrive_expect_tx(&bars[slot], row_bytes);
-    ptx::bulk_g2s(ring + (size_t)slot * dim, ent + (size_t)(code & 0x7FFFFFFFu) * dim, row_bytes, &bars[slot]);
+    ptx::bulk_g2s(ring + (size_t)slot * dim, src + (size_t)(code & ROW_MASK) * dim, row_bytes, &bars[slot]);
   };
   if (lane == 0) {
     const int first = n_loop < RING ? n_loop : RING;
@@ -1044,12 +1280,15 @@ margin_step_ring_kernel(MarginStepParams a, TrainGrads gr, const float* __restri
   const float g = BWD ? *gloss : 0.f;
   float loss = 0.f;
   FastAcc<LOSS> acc;
+  FastRelAcc<LOSS> rl;
+  if constexpr (REL) fast_rel_positive<MODEL, LOSS>(pp, rl);
   unsigned phases = 0u;   // bit s = parity of the next completion of slot s (a skipped use does not advance it)
   for (int j = 0; j < n_loop; ++j) {
     const unsigned code = codes[j];
     const long long idx = (long long)j * a.b + w;   // (unsharded: the negative's index in nh / nt / neg_out)
     if (!SHARD && code == CODE_BOTH) {   // no ring slot
-      both_replaced_pair<MODEL, BWD, LOSS>(a, gr, hi, ti, ri, a.nh[idx], a.nt[idx], idx, pp.pos, g, lane, loss);
+      both_replaced_pair<MODEL, BWD, LOSS>(a, gr, hi, ti, ri, a.nh[idx], a.nt[idx], idx, pp.pos, g, lane, loss,
+                                           REL ? a.nr[idx] : ri);
       if (lane == 0 && j + RING < n_loop) request(j + RING);
       continue;
     }
@@ -1062,20 +1301,39 @@ margin_step_ring_kernel(MarginStepParams a, TrainGrads gr, const float* __restri
       ptx::fence_proxy_async();          // generic-proxy reads above, async-proxy write below
       request(j + RING);
     }
-    const bool head = (code & 0x80000000u) != 0u;   // warp-uniform
-    const long long e = (long long)(code & 0x7FFFFFFFu);
+    const long long e = (long long)(code & ROW_MASK);
     FastNeg n;
+    if (REL && (code & CODE_REL)) {      // warp-uniform
+      fast_rel_negative<MODEL, LOSS>(pp, rl, ev, n);
+      pair_forward<BWD, LOSS>(a, idx, lane, pp.pos, n.neg, loss);
+      if constexpr (BWD)
+        fast_rel_negative_backward<MODEL, LOSS>(pp, ev, n, a.margin, g, gr.rel0 + (size_t)e * dim, dim, lane, acc, rl);
+      continue;
+    }
+    const bool head = (code & 0x80000000u) != 0u;   // warp-uniform
     fast_negative<MODEL, BWD>(pp, ab, ev, head, n);
     pair_forward<BWD, LOSS>(a, idx, lane, pp.pos, n.neg, loss);
     if constexpr (BWD)
       fast_negative_backward<MODEL, LOSS>(pp, ab, ev, head, n, a.margin, g, gr.ent0 + (size_t)e * dim, dim, lane, acc);
   }
   if constexpr (BWD)
-    fast_positive_backward<MODEL, LOSS>(pp, ab, acc, g,
-                                        SHARD ? a.grad_hrows + (size_t)w * dim : gr.ent0 + (size_t)hi * dim,
-                                        SHARD ? a.grad_trows + (size_t)w * dim : gr.ent0 + (size_t)ti * dim,
-                                        gr.rel0 + (size_t)ri * dim, dim, lane);
+    fast_positive_backward<MODEL, LOSS, REL>(pp, ab, acc, g,
+                                             SHARD ? a.grad_hrows + (size_t)w * dim : gr.ent0 + (size_t)hi * dim,
+                                             SHARD ? a.grad_trows + (size_t)w * dim : gr.ent0 + (size_t)ti * dim,
+                                             gr.rel0 + (size_t)ri * dim, dim, lane, &rl);
   else if (lane == 0) atomicAdd(a.loss, loss);
+}
+
+template <int MODEL, bool BWD, int MINB = 0, bool SHARD = false, int LOSS = KGE_LOSS_MARGIN>
+__global__ void __launch_bounds__(WARPS_PER_BLOCK * 32, MINB == 0 ? 1 : MINB)
+margin_step_ring_kernel(MarginStepParams a, TrainGrads gr, const float* __restrict__ gloss) {
+  ring_step<MODEL, BWD, SHARD, LOSS, false>(a, gr, gloss);
+}
+
+template <int MODEL, bool BWD, bool SHARD, int LOSS>
+__global__ void __launch_bounds__(WARPS_PER_BLOCK * 32, 1)
+margin_step_ring_rel_kernel(MarginStepParams a, TrainGrads gr, const float* __restrict__ gloss) {
+  ring_step<MODEL, BWD, SHARD, LOSS, true>(a, gr, gloss);
 }
 
 __host__ inline size_t ring_smem_bytes(const MarginStepParams& a) {
@@ -1090,22 +1348,39 @@ __host__ inline bool ring_step_ok(const MarginStepParams& a) {
   return enabled && a.n_neg <= 8192 && rows < 0x7FFFFFFFll && ring_smem_bytes(a) <= 96 * 1024;
 }
 
-template <int MODEL, bool BWD, int MINB, bool SHARD = false, int LOSS = KGE_LOSS_MARGIN>
+// REL: margin_step_ring_rel_kernel (MINB is 0 there)
+template <int MODEL, bool BWD, int MINB, bool SHARD = false, int LOSS = KGE_LOSS_MARGIN, bool REL = false>
 cudaError_t launch_ring_variant(const MarginStepParams& a, const TrainGrads& gr, const float* gloss, cudaStream_t st) {
+  void (*kernel)(MarginStepParams, TrainGrads, const float*) =
+      REL ? margin_step_ring_rel_kernel<MODEL, BWD, SHARD, LOSS> : margin_step_ring_kernel<MODEL, BWD, MINB, SHARD, LOSS>;
   const size_t smem = ring_smem_bytes(a);
   static bool configured[64] = {};
   int dev = 0;
   cudaError_t e = cudaGetDevice(&dev);
   if (e != cudaSuccess) return e;
   if (smem > 48 * 1024 && (dev < 0 || dev >= 64 || !configured[dev])) {
-    e = cudaFuncSetAttribute(margin_step_ring_kernel<MODEL, BWD, MINB, SHARD, LOSS>,
-                             cudaFuncAttributeMaxDynamicSharedMemorySize, 96 * 1024);
+    e = cudaFuncSetAttribute(kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, 96 * 1024);
     if (e != cudaSuccess) return e;
     if (dev >= 0 && dev < 64) configured[dev] = true;
   }
   const unsigned blocks = (unsigned)((a.b + WARPS_PER_BLOCK - 1) / WARPS_PER_BLOCK);
-  margin_step_ring_kernel<MODEL, BWD, MINB, SHARD, LOSS><<<blocks, WARPS_PER_BLOCK * 32, smem, st>>>(a, gr, gloss);
+  kernel<<<blocks, WARPS_PER_BLOCK * 32, smem, st>>>(a, gr, gloss);
   return cudaGetLastError();
+}
+
+// The relation-corrupting ring step, one kernel per (loss kind, sharded)
+template <int MODEL, bool BWD>
+cudaError_t launch_ring_rel(const MarginStepParams& a, const TrainGrads& gr, const float* gloss, cudaStream_t st) {
+  auto by_shard = [&](auto loss) -> cudaError_t {
+    constexpr int LOSS = decltype(loss)::value;
+    if (a.hrows) return launch_ring_variant<MODEL, BWD, 0, true, LOSS, true>(a, gr, gloss, st);
+    return launch_ring_variant<MODEL, BWD, 0, false, LOSS, true>(a, gr, gloss, st);
+  };
+  switch (a.loss_kind) {
+    case KGE_LOSS_LOGISTIC: return by_shard(std::integral_constant<int, KGE_LOSS_LOGISTIC>{});
+    case KGE_LOSS_BCE: return by_shard(std::integral_constant<int, KGE_LOSS_BCE>{});
+    default: return by_shard(std::integral_constant<int, KGE_LOSS_MARGIN>{});
+  }
 }
 
 // One ring kernel per (loss kind, sharded).  KGE_TRAIN_BWD_BLOCKS=5 holds the backward kernel to 96
@@ -1217,6 +1492,17 @@ cudaError_t launch_corrupt_batch(const int64_t* h, const int64_t* t, const int64
   return cudaGetLastError();
 }
 
+cudaError_t launch_corrupt_batch_rel(const int64_t* h, const int64_t* t, const int64_t* r, int64_t b,
+                                     int n_neg, const float* probs, int64_t n_ent, int64_t n_rel, float rel_share,
+                                     uint64_t seed, uint64_t offset, int64_t* nh, int64_t* nt, int64_t* nr,
+                                     cudaStream_t st) {
+  const long long n = (long long)b * n_neg;
+  if (n <= 0) return cudaSuccess;
+  corrupt_batch_rel_kernel<<<(unsigned)((n + 255) / 256), 256, 0, st>>>(h, t, r, b, n_neg, probs, n_ent, n_rel,
+                                                                         rel_share, seed, offset, nh, nt, nr);
+  return cudaGetLastError();
+}
+
 namespace {
 // f(std::integral_constant<int, MODEL>{}) for the models of the ring and register-resident forms
 // (fast_step_ok)
@@ -1233,7 +1519,41 @@ cudaError_t with_fast_model(int model, F&& f) {
 // else the generic kernels.  An entity-sharded step (a.hrows) that holds no rows scores no negative.
 template <bool BWD>
 cudaError_t launch_margin_step(const MarginStepParams& a, const TrainGrads& gr, const float* gloss,
+                               cudaStream_t st);
+
+// A relation-corrupting step.  At rel_share >= 1 its draws are the entity step's (draw_rel), so without
+// caller negatives or an nr_out to fill it is that step, on whichever kernel that one takes.  Otherwise:
+// TransE-L1 / L2 and DistMult take the ring kernel's relation kind (margin_step_ring_rel_kernel) where
+// the ring applies (its codes then hold 30-bit row numbers); everything else, and KGE_TRAIN_RING=0, the
+// generic kernels, which score a negative from its own (nh, nt, nr).  The register-resident form has no
+// relation kind.
+template <bool BWD>
+cudaError_t launch_rel_step(const MarginStepParams& a, const TrainGrads& gr, const float* gloss, cudaStream_t st) {
+  if (a.rel_share >= 1.f && !a.nh && !a.nr_out) {
+    MarginStepParams e = a;
+    e.n_rel = 0;
+    return launch_margin_step<BWD>(e, gr, gloss, st);
+  }
+  const bool shard = a.hrows != nullptr;
+  if (a.b <= 0 || (shard && a.n_rows <= 0)) return cudaSuccess;
+  const long long rows = shard ? a.n_rows : a.n_ent;
+  if (fast_step_ok(a) && ring_step_ok(a) && rows < 0x3FFFFFFFll && a.n_rel < 0x3FFFFFFFll)
+    return with_fast_model(a.model, [&](auto m) { return launch_ring_rel<decltype(m)::value, BWD>(a, gr, gloss, st); });
+  const unsigned blocks = blocks_for_warps(a.b);
+  if constexpr (BWD) {
+    if (shard) margin_step_shard_bwd_kernel<<<blocks, WARPS_PER_BLOCK * 32, 0, st>>>(a, gr, gloss);
+    else margin_step_bwd_kernel<<<blocks, WARPS_PER_BLOCK * 32, 0, st>>>(a, gr, gloss);
+  } else {
+    if (shard) margin_step_shard_fwd_kernel<<<blocks, WARPS_PER_BLOCK * 32, 0, st>>>(a);
+    else margin_step_fwd_kernel<<<blocks, WARPS_PER_BLOCK * 32, 0, st>>>(a);
+  }
+  return cudaGetLastError();
+}
+
+template <bool BWD>
+cudaError_t launch_margin_step(const MarginStepParams& a, const TrainGrads& gr, const float* gloss,
                                cudaStream_t st) {
+  if (a.n_rel > 0) return launch_rel_step<BWD>(a, gr, gloss, st);
   const bool shard = a.hrows != nullptr;
   if (a.b <= 0 || (shard && a.n_rows <= 0)) return cudaSuccess;
   const unsigned blocks = blocks_for_warps(a.b);

@@ -50,6 +50,13 @@ struct MarginStepParams {
   float* grad_hrows;   // [b][planes][dim], +=
   float* grad_trows;
   int loss_kind;       // KGE_LOSS_MARGIN / _LOGISTIC / _BCE; margin is used by the margin loss only
+  // Relation-corrupting step (n_rel > 0, BernoulliRelationNegativeSampler): a negative replaces the
+  // relation with probability 1 - rel_share (draw_rel), else the head or the tail.  External negatives
+  // then come with nr; nr_out receives the relations of the negatives.  n_rel == 0: the entity step.
+  long long n_rel;
+  float rel_share;
+  const int64_t* nr;
+  int64_t* nr_out;
 };
 
 cudaError_t launch_score_triples_fwd(int model, int dim, const TrainTables& tb, const int64_t* h,
@@ -61,6 +68,11 @@ cudaError_t launch_score_triples_bwd(int model, int dim, const TrainTables& tb, 
 cudaError_t launch_corrupt_batch(const int64_t* h, const int64_t* t, const int64_t* r, int64_t b,
                                  int n_neg, const float* probs, int64_t n_ent, uint64_t seed,
                                  uint64_t offset, int64_t* nh, int64_t* nt, cudaStream_t st);
+// BernoulliRelationNegativeSampler.corrupt_batch: draw_rel per negative, (nh, nt, nr) out
+cudaError_t launch_corrupt_batch_rel(const int64_t* h, const int64_t* t, const int64_t* r, int64_t b,
+                                     int n_neg, const float* probs, int64_t n_ent, int64_t n_rel, float rel_share,
+                                     uint64_t seed, uint64_t offset, int64_t* nh, int64_t* nt, int64_t* nr,
+                                     cudaStream_t st);
 cudaError_t launch_margin_step_fwd(const MarginStepParams& a, cudaStream_t st);
 cudaError_t launch_margin_step_bwd(const MarginStepParams& a, const TrainGrads& gr, const float* gloss,
                                    cudaStream_t st);

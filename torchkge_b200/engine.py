@@ -465,17 +465,27 @@ class CudaEngine:
         a.ent_lo, a.n_rows = step.ent_lo, step.n_rows
         a.hrows, a.trows = _ptr(hrows), _ptr(trows)
         a.loss_kind = step.loss_kind
-        return a
+        if getattr(step, "n_rel", 0) == 0:
+            return a
+        ra = _lib.RelStepArgs()           # relation-corrupting step: kge_rel_step_* around the same arguments
+        ra.base, ra.n_rel, ra.rel_share = a, step.n_rel, step.rel_share
+        return ra
+
+    def _step_call(self, a, which, *rest):
+        name = ("kge_rel_step_" if isinstance(a, _lib.RelStepArgs) else "kge_margin_step_") + which
+        _lib.check(getattr(self.lib, name)(ctypes.byref(a), *rest), name)
 
     def margin_step_fwd(self, step, tables, h, t, r, probs, hrows, trows):
         """Sum of the loss terms (step.loss_kind: the hinge, logistic or BCE term of each pair) of the
         negatives this shard scores (float32 scalar tensor): the negatives whose replaced entity lies in
         [step.ent_lo, step.ent_lo + step.n_rows).  ``tables``:
         (ent0, ent1, rel0, rel1) with this shard's entity rows (a three-plane table as one stacked
-        (3, n, dim) tensor in ent0 / rel0); hrows / trows: (b, planes, dim) rows of every positive."""
+        (3, n, dim) tensor in ent0 / rel0); hrows / trows: (b, planes, dim) rows of every positive.
+        step.n_rel > 0: the relation-corrupting step (kge_rel_step_fwd), whose relation negatives this shard
+        scores when it holds the positive's head."""
         loss = torch.zeros((), dtype=torch.float32, device=h.device)
         a = self._shard_step_args(step, tables, h, t, r, probs, loss, hrows, trows)
-        _lib.check(self.lib.kge_margin_step_fwd(ctypes.byref(a)), "kge_margin_step_fwd")
+        self._step_call(a, "fwd")
         self.launches += 1
         return loss
 
@@ -484,12 +494,12 @@ class CudaEngine:
         and grad_hrows / grad_trows (b, planes, dim)."""
         dummy = torch.zeros((), dtype=torch.float32, device=h.device)   # the loss is not recomputed
         a = self._shard_step_args(step, tables, h, t, r, probs, dummy, hrows, trows)
-        a.grad_hrows, a.grad_trows = _ptr(grad_hrows), _ptr(grad_trows)
+        base = a.base if isinstance(a, _lib.RelStepArgs) else a
+        base.grad_hrows, base.grad_trows = _ptr(grad_hrows), _ptr(grad_trows)
         g = _lib.Grads()
         g.ent0, g.ent1 = _plane_ptrs(grads[0], grads[1])
         g.rel0, g.rel1 = _plane_ptrs(grads[2], grads[3])
-        _lib.check(self.lib.kge_margin_step_bwd(ctypes.byref(a), ctypes.byref(g), _ptr(gloss)),
-                   "kge_margin_step_bwd")
+        self._step_call(a, "bwd", ctypes.byref(g), _ptr(gloss))
         self.launches += 1
 
     def scatter_rows_add(self, code, dim, grad0, grad1, ent_lo, idx, rows):

@@ -146,23 +146,111 @@ class BernoulliNegativeSampler(NegativeSampler):
         shard: ``EntityShard(local_storage=True)`` for a model holding only its entity rows (see
         ``training.fused_margin_step``); every rank uses a sampler with the same seed and call count,
         built on the whole graph, and passes the same batch."""
-        if (margin is None) == (criterion is None):
-            raise ValueError("fused_step takes exactly one of margin and criterion")
-        if criterion is not None:
-            loss_kind_of(criterion)       # an unsupported criterion raises before the call count moves
-        if n_neg is None:
-            n_neg = self.n_neg
-        if shard is not None and getattr(shard, "n_ent", self.n_ent) != self.n_ent:
-            raise ValueError("the sampler draws on %d entities, the shard partitions %d"
-                             % (self.n_ent, shard.n_ent))
-        self.bern_probs = self.bern_probs.to(heads.device)
-        if criterion is not None:
-            return fused_loss_step(model, heads, tails, relations, criterion, n_neg=n_neg,
-                                   bern_probs=self.bern_probs, seed=self.seed,
-                                   offset=self._next_offset(), shard=shard)
-        return fused_margin_step(model, heads, tails, relations, margin, n_neg=n_neg,
-                                 bern_probs=self.bern_probs, seed=self.seed,
-                                 offset=self._next_offset(), shard=shard)
+        return _sampler_fused_step(self, model, heads, tails, relations, margin, n_neg, criterion, shard)
+
+
+def _sampler_fused_step(sampler, model, heads, tails, relations, margin, n_neg, criterion, shard, rel_share=None):
+    """fused_step of the Bernoulli samplers: their argument checks, then the fused step at the sampler's
+    next call count (rel_share: the relation-corrupting step)."""
+    if (margin is None) == (criterion is None):
+        raise ValueError("fused_step takes exactly one of margin and criterion")
+    if criterion is not None:
+        loss_kind_of(criterion)       # an unsupported criterion raises before the call count moves
+    if n_neg is None:
+        n_neg = sampler.n_neg
+    if shard is not None and getattr(shard, "n_ent", sampler.n_ent) != sampler.n_ent:
+        raise ValueError("the sampler draws on %d entities, the shard partitions %d"
+                         % (sampler.n_ent, shard.n_ent))
+    sampler.bern_probs = sampler.bern_probs.to(heads.device)
+    if criterion is not None:
+        return fused_loss_step(model, heads, tails, relations, criterion, n_neg=n_neg,
+                               bern_probs=sampler.bern_probs, seed=sampler.seed,
+                               offset=sampler._next_offset(), shard=shard, rel_share=rel_share)
+    return fused_margin_step(model, heads, tails, relations, margin, n_neg=n_neg,
+                             bern_probs=sampler.bern_probs, seed=sampler.seed,
+                             offset=sampler._next_offset(), shard=shard, rel_share=rel_share)
+
+
+class BernoulliRelationNegativeSampler(NegativeSampler):
+    """Bernoulli sampler that also corrupts relations, torchkge/sampling.py:507-553: with probability
+    ``rel_share`` a negative replaces an entity -- the head with probability ``bern_probs[r]``, else the
+    tail, uniform on [1, n_ent) -- and otherwise its relation, uniform on [1, n_rel).  Exactly one
+    position changes; entity 0 and relation 0 are never drawn and true triples are not rejected, as in the
+    reference.  Use with ``model(h, t, r, nh, nt, nr)``.
+
+    Draws come from the counter-based generator of ``BernoulliNegativeSampler`` (kge_corrupt_batch_rel):
+    with the same seed and call count, ``rel_share = 1`` gives that sampler's negatives.
+
+    Attributes
+    ----------
+    bern_probs: torch.FloatTensor (n_rel,) -- probability of corrupting the HEAD of an entity negative
+        (0.5 for relations absent from ``kg``).
+    rel_share: float -- probability that a negative replaces an entity rather than the relation.
+    seed: int -- key of the counter-based generator (extension; defaults to torch's seed).
+    """
+
+    def __init__(self, kg, kg_val=None, kg_test=None, n_neg=1, rel_share=.33, seed=None):
+        super().__init__(kg, kg_val, kg_test, n_neg)
+        self.n_rel = kg.n_rel
+        rel_share = float(rel_share)
+        if not 0.0 <= rel_share <= 1.0:
+            raise ValueError("rel_share must lie in [0, 1], got %r" % (rel_share,))
+        if self.n_rel < 2 and rel_share < 1.0:
+            raise ValueError("relation corruption draws from [1, n_rel) and needs n_rel >= 2 (n_rel = %d)"
+                             % self.n_rel)
+        self.rel_share = rel_share
+        self.bern_probs = self.evaluate_probabilities()
+        self.seed = int(torch.initial_seed() if seed is None else seed) & 0xFFFFFFFFFFFFFFFF
+        self._calls = 0
+
+    evaluate_probabilities = BernoulliNegativeSampler.evaluate_probabilities
+    _next_offset = BernoulliNegativeSampler._next_offset
+
+    def corrupt_batch(self, heads, tails, relations, n_neg=None):
+        """(neg_heads, neg_tails, neg_rels), int64, on ``heads.device``: ONE negative per fact, as in the
+        reference (``n_neg`` is ignored: ``Model.forward`` cannot pair blocks of relations with an
+        unrepeated positive)."""
+        dev = heads.device
+        assert dev == tails.device
+        if not heads.is_cuda:
+            raise _lib.KgeLibraryError("corrupt_batch needs CUDA index tensors; there is no CPU path")
+        b = heads.shape[0]
+        self.bern_probs = self.bern_probs.to(dev)
+        h, t, r = (x.to(dev).long().contiguous() for x in (heads, tails, relations))
+        nh, nt, nr = (torch.empty(b, dtype=torch.int64, device=dev) for _ in range(3))
+        _lib.check(_lib.load().kge_corrupt_batch_rel(_ptr(h), _ptr(t), _ptr(r), b, 1, _ptr(self.bern_probs),
+                                                     self.n_ent, self.n_rel, self.rel_share, self.seed,
+                                                     self._next_offset(), _ptr(nh), _ptr(nt), _ptr(nr),
+                                                     _stream(dev)), "kge_corrupt_batch_rel")
+        return nh, nt, nr
+
+    def corrupt_kg(self, batch_size, use_cuda, which='main'):
+        """Corrupt a whole graph (one negative per fact): (neg_heads, neg_tails, neg_rels), CPU tensors.
+        The reference inherits a two-value version that fails for this sampler."""
+        assert which in ['main', 'train', 'test', 'val']
+        kg = {'val': self.kg_val, 'test': self.kg_test}.get(which, self.kg)
+        assert kg is not None and kg.n_facts > 0
+        if not use_cuda:
+            raise _lib.KgeLibraryError("corrupt_kg(use_cuda=False): negative sampling runs on CUDA "
+                                       "only in this package")
+        out = ([], [], [])
+        for lo in range(0, kg.n_facts, batch_size):
+            sl = slice(lo, lo + batch_size)
+            for acc, x in zip(out, self.corrupt_batch(kg.head_idx[sl].cuda(), kg.tail_idx[sl].cuda(),
+                                                      kg.relations[sl].cuda())):
+                acc.append(x)
+        return tuple(torch.cat(x).long().cpu() for x in out)
+
+    def fused_step(self, model, heads, tails, relations, margin=None, n_neg=None, *, criterion=None,
+                   shard=None):
+        """Extension: corruption + ``model(h, t, r, nh, nt, nr)`` + the loss in ONE kernel; returns the
+        differentiable scalar loss.  Arguments and errors as in ``BernoulliNegativeSampler.fused_step``.
+
+        n_neg (extension) >= 1 negatives per fact, drawn as n_neg blocks of the batch; block 0 is exactly
+        what ``corrupt_batch`` draws at the same call count.  With ``shard``, the rank holding a positive's
+        head scores its relation negatives."""
+        return _sampler_fused_step(self, model, heads, tails, relations, margin, n_neg, criterion, shard,
+                                   rel_share=self.rel_share)
 
 
 class PositionalNegativeSampler(BernoulliNegativeSampler):

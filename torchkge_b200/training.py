@@ -211,29 +211,38 @@ class _MarginStep(torch.autograd.Function):
 
     @staticmethod
     def forward(ctx, code, dim, n_ent, margin, n_neg, h, t, r, nh, nt, probs, seed, offset,
-                ent0, ent1, rel0, rel1, loss_kind=_lib.LOSS_MARGIN):
+                ent0, ent1, rel0, rel1, loss_kind=_lib.LOSS_MARGIN, nr=None, rel=None):
+        # rel: (n_rel, rel_share) for a relation-corrupting step (kge_rel_step_*; external negatives then
+        # come with nr), None for the entity step (kge_margin_step_*)
         tensors = [None if x is None else x.detach().contiguous() for x in (ent0, ent1, rel0, rel1)]
         _check_cuda(tensors[0], h, t, r)
         dev = tensors[0].device
         h, t, r = _idx(h, dev), _idx(t, dev), _idx(r, dev)
         if nh is not None:
             nh, nt = _idx(nh, dev), _idx(nt, dev)
+        if nr is not None:
+            nr = _idx(nr, dev)
         if probs is not None:
             probs = probs.to(device=dev, dtype=torch.float32).contiguous()
         loss = torch.zeros((), dtype=torch.float32, device=dev)
         a = _MarginStep._args(code, dim, n_ent, margin, n_neg, h, t, r, nh, nt, probs, seed, offset,
-                              tensors, loss, dev, loss_kind)
-        _lib.check(_lib.load().kge_margin_step_fwd(ctypes.byref(a)), "kge_margin_step_fwd")
-        ctx.meta = (code, dim, n_ent, margin, n_neg, seed, offset, loss_kind)
+                              tensors, loss, dev, loss_kind, nr, rel)
+        if rel is None:
+            _lib.check(_lib.load().kge_margin_step_fwd(ctypes.byref(a)), "kge_margin_step_fwd")
+        else:
+            _lib.check(_lib.load().kge_rel_step_fwd(ctypes.byref(a)), "kge_rel_step_fwd")
+        ctx.meta = (code, dim, n_ent, margin, n_neg, seed, offset, loss_kind, rel)
         ctx.present = [x is not None for x in tensors]
-        ctx.has_neg, ctx.has_probs = nh is not None, probs is not None
-        extra = ([nh, nt] if nh is not None else []) + ([probs] if probs is not None else [])
+        ctx.has_neg, ctx.has_nr, ctx.has_probs = nh is not None, nr is not None, probs is not None
+        extra = (([nh, nt] if nh is not None else []) + ([nr] if nr is not None else []) +
+                 ([probs] if probs is not None else []))
         ctx.save_for_backward(h, t, r, *extra, *[x for x in tensors if x is not None])
         return loss
 
     @staticmethod
     def _args(code, dim, n_ent, margin, n_neg, h, t, r, nh, nt, probs, seed, offset, tensors, loss, dev,
-              loss_kind=_lib.LOSS_MARGIN):
+              loss_kind=_lib.LOSS_MARGIN, nr=None, rel=None):
+        """kge_margin_step_args_t, or with rel = (n_rel, rel_share) kge_rel_step_args_t around it."""
         a = _lib.MarginStepArgs()
         a.tb = _tables(code, dim, tensors)
         a.n_neg, a.margin, a.b, a.n_ent = n_neg, float(margin), h.shape[0], n_ent
@@ -241,18 +250,26 @@ class _MarginStep(torch.autograd.Function):
         a.seed, a.offset = int(seed), int(offset)
         a.loss, a.stream = _ptr(loss), _stream(dev)
         a.loss_kind = int(loss_kind)
-        return a
+        if rel is None:
+            return a
+        ra = _lib.RelStepArgs()
+        ra.base = a
+        ra.n_rel, ra.rel_share, ra.nr = int(rel[0]), float(rel[1]), _ptr(nr)
+        return ra
 
     @staticmethod
     def backward(ctx, gl):
-        code, dim, n_ent, margin, n_neg, seed, offset, loss_kind = ctx.meta
+        code, dim, n_ent, margin, n_neg, seed, offset, loss_kind, rel = ctx.meta
         saved = list(ctx.saved_tensors)
         h, t, r = saved[:3]
         k = 3
-        nh = nt = probs = None
+        nh = nt = nr = probs = None
         if ctx.has_neg:
             nh, nt = saved[k], saved[k + 1]
             k += 2
+        if ctx.has_nr:
+            nr = saved[k]
+            k += 1
         if ctx.has_probs:
             probs = saved[k]
             k += 1
@@ -262,17 +279,23 @@ class _MarginStep(torch.autograd.Function):
         gl = gl.contiguous().float()
         dummy = torch.zeros((), dtype=torch.float32, device=dev)
         a = _MarginStep._args(code, dim, n_ent, margin, n_neg, h, t, r, nh, nt, probs, seed, offset,
-                              tensors, dummy, dev, loss_kind)
+                              tensors, dummy, dev, loss_kind, nr, rel)
         gs, g = _zero_grads(tensors)
-        _lib.check(_lib.load().kge_margin_step_bwd(ctypes.byref(a), ctypes.byref(g), _ptr(gl)),
-                   "kge_margin_step_bwd")
-        return (None,) * 13 + tuple(gs) + (None,)
+        if rel is None:
+            _lib.check(_lib.load().kge_margin_step_bwd(ctypes.byref(a), ctypes.byref(g), _ptr(gl)),
+                       "kge_margin_step_bwd")
+        else:
+            _lib.check(_lib.load().kge_rel_step_bwd(ctypes.byref(a), ctypes.byref(g), _ptr(gl)),
+                       "kge_rel_step_bwd")
+        return (None,) * 13 + tuple(gs) + (None,) * 3
 
 
 #: what every rank's kernels of one sharded step are told (engine.margin_step_fwd / _bwd)
-#: loss_kind: _lib.LOSS_* (default the margin loss)
-ShardedStep = collections.namedtuple("ShardedStep", "code dim n_ent ent_lo n_rows n_neg margin seed offset loss_kind",
-                                     defaults=(_lib.LOSS_MARGIN,))
+#: loss_kind: _lib.LOSS_* (default the margin loss); n_rel > 0: a relation-corrupting step that replaces an
+#: entity with probability rel_share (kge_rel_step_*), n_rel = 0 the entity step
+ShardedStep = collections.namedtuple("ShardedStep",
+                                     "code dim n_ent ent_lo n_rows n_neg margin seed offset loss_kind n_rel rel_share",
+                                     defaults=(_lib.LOSS_MARGIN, 0, 1.0))
 
 
 class _ShardedMarginStep(torch.autograd.Function):
@@ -353,7 +376,7 @@ def _signed64(x):
 
 
 def sharded_margin_step(model, heads, tails, relations, margin, n_neg, bern_probs, seed, offset, shard,
-                        engine=None, loss_kind=_lib.LOSS_MARGIN):
+                        engine=None, loss_kind=_lib.LOSS_MARGIN, rel_share=None):
     """``fused_margin_step(..., shard=shard)`` (``fused_loss_step`` with ``loss_kind``) for a model that
     holds only the entity rows [shard.lo, shard.hi) of an EntityShard with local storage; the same
     (heads, tails, relations), seed, offset, n_neg, margin and loss kind on every rank.  Returns the full
@@ -361,7 +384,10 @@ def sharded_margin_step(model, heads, tails, relations, margin, n_neg, bern_prob
     (identical) relation gradient.  Every rank counts the positive's term of a pair only for the
     negatives it scores, so the ranks' sums are the unsharded loss and gradients.
     ``engine``: CudaEngine or a stand-in with margin_step_fwd / margin_step_bwd / scatter_rows_add /
-    gather_rows."""
+    gather_rows.
+    ``rel_share``: a relation-corrupting step (``BernoulliRelationNegativeSampler``): each negative replaces
+    an entity with probability rel_share, else the relation; the rank that holds a positive's head scores
+    its relation negatives.  Every rank must pass the same rel_share (None: the entity step)."""
     # argument errors first, on every rank: none of them may leave the others waiting in a collective
     if isinstance(shard, QueryShard):
         raise ValueError("the fused training step takes an EntityShard; QueryShard (data-parallel "
@@ -376,43 +402,74 @@ def sharded_margin_step(model, heads, tails, relations, margin, n_neg, bern_prob
     code = _training_code(model)
     ent0, ent1, rel0, rel1 = _param_tensors(model, code)
     b = int(heads.shape[0])
+    n_rel, share = (0, 1.0) if rel_share is None else (int(rel0.shape[-2]), float(rel_share))
+    if rel_share is not None:
+        _check_rel_share(n_rel, share)
     step = ShardedStep(code, _kernel_dim(model, code), shard.n_ent, shard.lo, int(ent0.shape[-2]), int(n_neg),
                        float(margin), int(seed) & 0xFFFFFFFFFFFFFFFF, int(offset) & 0xFFFFFFFFFFFFFFFF,
-                       int(loss_kind))
+                       int(loss_kind), n_rel, share)
     _check_table(step, shard)
-    # one small collective: every rank must draw the same negatives for the same batch and loss
+    # one small collective: every rank must draw the same negatives for the same batch and loss.  The last
+    # field holds the loss kind and, above it, the float32 bits of 1 - rel_share: 0 for the entity step,
+    # whose draws are those of rel_share = 1
+    kind_share = step.loss_kind | struct.unpack("<I", struct.pack("<f", 1.0 - share))[0] << 8
     mine = torch.tensor([_signed64(step.seed), _signed64(step.offset), b, step.n_neg,
-                         struct.unpack("<q", struct.pack("<d", step.margin))[0], step.loss_kind],
+                         struct.unpack("<q", struct.pack("<d", step.margin))[0], kind_share],
                         dtype=torch.int64, device=rel0.device)
     everyone = shard.stack_all(mine)
     if not bool((everyone == mine).all()):
         raise ValueError("the ranks of a sharded step disagree on (seed, offset, batch size, n_neg, margin, "
-                         "loss kind): %s" % everyone.tolist())
+                         "loss kind and rel_share): %s" % everyone.tolist())
     return _ShardedMarginStep.apply(step, shard, engine or default_engine(), heads, tails, relations,
                                     bern_probs, ent0, ent1, rel0, rel1)
 
 
+def _check_rel_share(n_rel, rel_share):
+    """The relation draw is uniform on [1, n_rel): it needs two relations unless it never happens."""
+    if not 0.0 <= rel_share <= 1.0:
+        raise ValueError("rel_share must lie in [0, 1], got %r" % (rel_share,))
+    if n_rel < 2 and rel_share < 1.0:
+        raise ValueError("relation corruption draws from [1, n_rel) and needs n_rel >= 2 (n_rel = %d); "
+                         "use rel_share = 1" % n_rel)
+
+
 def _fused_step(model, heads, tails, relations, loss_kind, margin, n_neg, negatives, bern_probs, seed, offset,
-                shard):
+                shard, rel_share=None):
+    if negatives is not None and len(negatives) not in (2, 3):
+        raise ValueError("negatives must be (neg_heads, neg_tails) or (neg_heads, neg_tails, neg_rels)")
     if shard is not None:
         if negatives is not None:
             raise ValueError("external negatives are not supported by the sharded training step")
         return sharded_margin_step(model, heads, tails, relations, margin, n_neg, bern_probs, seed, offset,
-                                   shard, loss_kind=loss_kind)
+                                   shard, loss_kind=loss_kind, rel_share=rel_share)
     spec_code = _training_code(model)
     ent0, ent1, rel0, rel1 = _param_tensors(model, spec_code)
-    nh = nt = None
+    nh = nt = nr = None
+    rel = None
+    if negatives is not None and rel_share is not None:
+        raise ValueError("rel_share sets how negatives are drawn; with caller negatives give (neg_heads, "
+                         "neg_tails, neg_rels) and no rel_share")
+    if rel_share is not None:
+        rel = (int(rel0.shape[-2]), float(rel_share))
+        _check_rel_share(*rel)
     if negatives is not None:
-        nh, nt = negatives
+        nh, nt = negatives[:2]
+        if len(negatives) == 3:      # any positions may change: the draw parameters play no part
+            nr = negatives[2]
+            rel = (int(rel0.shape[-2]), 1.0)
+        lengths = {int(x.shape[0]) for x in negatives}
+        if len(lengths) != 1 or nh.shape[0] % max(int(heads.shape[0]), 1) != 0:
+            raise ValueError("the negatives must have one common length, a multiple of the batch size (got %s "
+                             "for a batch of %d)" % ([int(x.shape[0]) for x in negatives], heads.shape[0]))
         n_neg = int(nh.shape[0] // heads.shape[0])
     elif bern_probs is None:
         raise ValueError("either negatives or bern_probs must be given")
     return _MarginStep.apply(spec_code, _kernel_dim(model, spec_code), model.n_ent, margin, n_neg, heads, tails,
-                             relations, nh, nt, bern_probs, seed, offset, ent0, ent1, rel0, rel1, loss_kind)
+                             relations, nh, nt, bern_probs, seed, offset, ent0, ent1, rel0, rel1, loss_kind, nr, rel)
 
 
 def fused_loss_step(model, heads, tails, relations, criterion, n_neg=1, negatives=None, bern_probs=None,
-                    seed=0, offset=0, *, shard=None):
+                    seed=0, offset=0, *, shard=None, rel_share=None):
     """``fused_margin_step`` for any of the three losses: Bernoulli corruption (or the given
     ``negatives``), ``model(h, t, r, nh, nt)`` and ``criterion(pos, neg)`` in a single kernel,
     differentiable with respect to the embedding tables.
@@ -424,15 +481,15 @@ def fused_loss_step(model, heads, tails, relations, criterion, n_neg=1, negative
           logistic: softplus(-pos_i) + softplus(neg_ij)
           BCE     : -max(log sig(pos_i), -100) - max(log(1 - sig(neg_ij)), -100)
         and its gradients are those torch's SoftMarginLoss / BCELoss backward give.
-    shard: as in ``fused_margin_step``; every rank must pass the same kind of loss.
+    shard, rel_share, negatives: as in ``fused_margin_step``; every rank must pass the same kind of loss.
     """
     kind, margin = loss_kind_of(criterion)
     return _fused_step(model, heads, tails, relations, kind, margin, n_neg, negatives, bern_probs, seed, offset,
-                       shard)
+                       shard, rel_share)
 
 
 def fused_margin_step(model, heads, tails, relations, margin, n_neg=1, negatives=None,
-                      bern_probs=None, seed=0, offset=0, *, shard=None):
+                      bern_probs=None, seed=0, offset=0, *, shard=None, rel_share=None):
     """Loss of one training step, fused: Bernoulli corruption (or the given ``negatives =
     (neg_heads, neg_tails)``), ``model(h, t, r, nh, nt)`` and ``MarginLoss(margin)`` in a
     single kernel, differentiable with respect to the embedding tables.
@@ -448,7 +505,13 @@ def fused_margin_step(model, heads, tails, relations, margin, n_neg=1, negatives
         the full loss; the negatives are drawn on [1, shard.n_ent).  External negatives are not
         supported in this mode.
 
+    rel_share: relation-corrupting negatives (``BernoulliRelationNegativeSampler``): each negative replaces
+        an entity (head with probability bern_probs[r], else tail) with probability rel_share, else the
+        relation, uniform on [1, n_rel) -- the draws of ``kge_corrupt_batch_rel``.  None: the entity step.
+    negatives: also ``(neg_heads, neg_tails, neg_rels)``; a negative is then scored as
+        ``model.scoring_function(nh, nt, nr)`` and any of its positions may differ from the positive's.
+
     ``fused_loss_step`` takes a criterion instead of a margin (LogisticLoss, BinaryCrossEntropyLoss).
     """
     return _fused_step(model, heads, tails, relations, _lib.LOSS_MARGIN, margin, n_neg, negatives, bern_probs,
-                       seed, offset, shard)
+                       seed, offset, shard, rel_share)
