@@ -6,6 +6,7 @@
 // table to scan; the (n, n_rel) score matrix is small (n_rel relations) and is produced densely,
 // in the reference's arithmetic: rescal_query_component (oneMKL order) then the ATen cascade sum.
 #include "kernels.h"
+#include "ptx.cuh"
 
 namespace kge {
 
@@ -97,14 +98,10 @@ cudaError_t launch_rescal_rel_scores(const float* hrows, const float* trows, con
   if (n <= 0 || n_rel <= 0) return cudaSuccess;
   const size_t smem = (size_t)2 * RR_ITILE * dim * sizeof(float);
   if (smem > 200 * 1024) return cudaErrorInvalidValue;
-  static bool configured[64] = {};
-  int dev = 0;
-  cudaError_t e = cudaGetDevice(&dev);
-  if (e != cudaSuccess) return e;
-  if (smem > 48 * 1024 && (dev < 0 || dev >= 64 || !configured[dev])) {
-    e = cudaFuncSetAttribute(rescal_rel_scores_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, 200 * 1024);
+  if (smem > 48 * 1024) {
+    const cudaError_t e =
+        set_attribute_once<rescal_rel_scores_kernel>(cudaFuncAttributeMaxDynamicSharedMemorySize, 200 * 1024);
     if (e != cudaSuccess) return e;
-    if (dev >= 0 && dev < 64) configured[dev] = true;
   }
   const long long i_tiles = (n + RR_ITILE - 1) / RR_ITILE;
   for (long long y0 = 0; y0 < i_tiles; y0 += 65535) {     // gridDim.y limit

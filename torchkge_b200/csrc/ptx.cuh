@@ -1,11 +1,32 @@
 // Thin wrappers over the sm_90 PTX used by the scan pipeline:
 // mbarrier (init / expect_tx / try_wait.parity / arrive) and 1-D bulk async copy
 // (cp.async.bulk global -> shared, SASS UBLKCP) completing on an mbarrier.
+// On the host: set_attribute_once, e.g. to let a kernel use more than 48 KB of dynamic shared memory.
 #pragma once
 #include <cuda_runtime.h>
 #include <stdint.h>
 
+#include <atomic>
+
 namespace kge {
+
+// cudaFuncSetAttribute(KERNEL, attr, value) on the current device, once per (attribute, device
+// ordinal): a function attribute is a per-device property, and each caller always passes the same
+// value for a given kernel and attribute.  Ordinals of 64 and above set it on every call.  Launchers
+// run from several host threads at once, hence the atomic record.
+template <auto KERNEL>
+inline cudaError_t set_attribute_once(cudaFuncAttribute attr, int value) {
+  static std::atomic<uint64_t> done[cudaFuncAttributeMax] = {};   // [attr]: bit d set on device d
+  int dev = 0;
+  cudaError_t e = cudaGetDevice(&dev);
+  if (e != cudaSuccess) return e;
+  const bool known = attr >= 0 && attr < cudaFuncAttributeMax && dev >= 0 && dev < 64;
+  if (known && ((done[attr].load(std::memory_order_acquire) >> dev) & 1u)) return cudaSuccess;
+  e = cudaFuncSetAttribute(KERNEL, attr, value);
+  if (e == cudaSuccess && known) done[attr].fetch_or(1ull << dev, std::memory_order_release);
+  return e;
+}
+
 namespace ptx {
 
 __device__ __forceinline__ uint32_t smem_u32(const void* p) {

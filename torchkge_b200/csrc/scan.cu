@@ -336,18 +336,12 @@ cudaError_t launch_one(ScanParams& p, cudaStream_t stream) {
       if (p.code[kc * KC + kk] != FAST) m |= 1u << kk;
     p.mask[kc] = m;
   }
-  // the opt-in shared-memory size is a per-device function attribute: one flag per device ordinal
-  // (benign race: setting the attribute is idempotent)
-  static bool configured[64] = {};
-  auto kern = scan_kernel<EL, CASC, G, APPROX>;
-  int dev = 0, sms = 0;
-  cudaError_t e = cudaGetDevice(&dev);
+  constexpr auto kern = scan_kernel<EL, CASC, G, APPROX>;
+  cudaError_t e = set_attribute_once<kern>(cudaFuncAttributeMaxDynamicSharedMemorySize, (int)L::SMEM_BYTES);
   if (e != cudaSuccess) return e;
-  if (dev < 0 || dev >= 64 || !configured[dev]) {
-    e = cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)L::SMEM_BYTES);
-    if (e != cudaSuccess) return e;
-    if (dev >= 0 && dev < 64) configured[dev] = true;
-  }
+  int dev = 0, sms = 0;
+  e = cudaGetDevice(&dev);
+  if (e != cudaSuccess) return e;
   e = cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev);
   if (e != cudaSuccess) return e;
   const long long total = (long long)p.n_qt * (long long)p.n_ct;

@@ -102,75 +102,46 @@ __device__ __forceinline__ void fence_acc(float (&d)[ACC]) {
 // D[regs] (+)= A[smem] * B[smem]^T, 64 x 256 x 16, both operands K-major; accumulate = 0 overwrites D.
 // Accumulator layout (thread t of the warpgroup, warp w = t / 32, lane l): d[i] is row
 // 16 w + l / 4 + 8 ((i >> 1) & 1), column 8 (i >> 2) + 2 (l & 3) + (i & 1).
-__device__ __forceinline__ void wgmma_bf16(float (&d)[128], uint64_t desc_a, uint64_t desc_b, uint32_t accumulate) {
-  asm volatile(
-      "{\n\t"
-      ".reg .pred p;\n\t"
-      "setp.ne.b32 p, %130, 0;\n\t"
-      "wgmma.mma_async.sync.aligned.m64n256k16.f32.bf16.bf16 "
-      "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, "
-      "%16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31, "
-      "%32, %33, %34, %35, %36, %37, %38, %39, %40, %41, %42, %43, %44, %45, %46, %47, "
-      "%48, %49, %50, %51, %52, %53, %54, %55, %56, %57, %58, %59, %60, %61, %62, %63, "
-      "%64, %65, %66, %67, %68, %69, %70, %71, %72, %73, %74, %75, %76, %77, %78, %79, "
-      "%80, %81, %82, %83, %84, %85, %86, %87, %88, %89, %90, %91, %92, %93, %94, %95, "
-      "%96, %97, %98, %99, %100, %101, %102, %103, %104, %105, %106, %107, %108, %109, %110, %111, "
-      "%112, %113, %114, %115, %116, %117, %118, %119, %120, %121, %122, %123, %124, %125, %126, %127}, "
-      "%128, %129, p, 1, 1, 0, 0;\n\t"
-      "}\n"
-      : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]),
-        "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15]),
-        "+f"(d[16]), "+f"(d[17]), "+f"(d[18]), "+f"(d[19]), "+f"(d[20]), "+f"(d[21]), "+f"(d[22]), "+f"(d[23]),
-        "+f"(d[24]), "+f"(d[25]), "+f"(d[26]), "+f"(d[27]), "+f"(d[28]), "+f"(d[29]), "+f"(d[30]), "+f"(d[31]),
-        "+f"(d[32]), "+f"(d[33]), "+f"(d[34]), "+f"(d[35]), "+f"(d[36]), "+f"(d[37]), "+f"(d[38]), "+f"(d[39]),
-        "+f"(d[40]), "+f"(d[41]), "+f"(d[42]), "+f"(d[43]), "+f"(d[44]), "+f"(d[45]), "+f"(d[46]), "+f"(d[47]),
-        "+f"(d[48]), "+f"(d[49]), "+f"(d[50]), "+f"(d[51]), "+f"(d[52]), "+f"(d[53]), "+f"(d[54]), "+f"(d[55]),
-        "+f"(d[56]), "+f"(d[57]), "+f"(d[58]), "+f"(d[59]), "+f"(d[60]), "+f"(d[61]), "+f"(d[62]), "+f"(d[63]),
-        "+f"(d[64]), "+f"(d[65]), "+f"(d[66]), "+f"(d[67]), "+f"(d[68]), "+f"(d[69]), "+f"(d[70]), "+f"(d[71]),
-        "+f"(d[72]), "+f"(d[73]), "+f"(d[74]), "+f"(d[75]), "+f"(d[76]), "+f"(d[77]), "+f"(d[78]), "+f"(d[79]),
-        "+f"(d[80]), "+f"(d[81]), "+f"(d[82]), "+f"(d[83]), "+f"(d[84]), "+f"(d[85]), "+f"(d[86]), "+f"(d[87]),
-        "+f"(d[88]), "+f"(d[89]), "+f"(d[90]), "+f"(d[91]), "+f"(d[92]), "+f"(d[93]), "+f"(d[94]), "+f"(d[95]),
-        "+f"(d[96]), "+f"(d[97]), "+f"(d[98]), "+f"(d[99]), "+f"(d[100]), "+f"(d[101]), "+f"(d[102]), "+f"(d[103]),
-        "+f"(d[104]), "+f"(d[105]), "+f"(d[106]), "+f"(d[107]), "+f"(d[108]), "+f"(d[109]), "+f"(d[110]), "+f"(d[111]),
-        "+f"(d[112]), "+f"(d[113]), "+f"(d[114]), "+f"(d[115]), "+f"(d[116]), "+f"(d[117]), "+f"(d[118]), "+f"(d[119]),
-        "+f"(d[120]), "+f"(d[121]), "+f"(d[122]), "+f"(d[123]), "+f"(d[124]), "+f"(d[125]), "+f"(d[126]), "+f"(d[127])
-      : "l"(desc_a), "l"(desc_b), "r"(accumulate)
-      : "memory");
-}
-__device__ __forceinline__ void wgmma_fp16(float (&d)[128], uint64_t desc_a, uint64_t desc_b, uint32_t accumulate) {
-  asm volatile(
-      "{\n\t"
-      ".reg .pred p;\n\t"
-      "setp.ne.b32 p, %130, 0;\n\t"
-      "wgmma.mma_async.sync.aligned.m64n256k16.f32.f16.f16 "
-      "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, "
-      "%16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31, "
-      "%32, %33, %34, %35, %36, %37, %38, %39, %40, %41, %42, %43, %44, %45, %46, %47, "
-      "%48, %49, %50, %51, %52, %53, %54, %55, %56, %57, %58, %59, %60, %61, %62, %63, "
-      "%64, %65, %66, %67, %68, %69, %70, %71, %72, %73, %74, %75, %76, %77, %78, %79, "
-      "%80, %81, %82, %83, %84, %85, %86, %87, %88, %89, %90, %91, %92, %93, %94, %95, "
-      "%96, %97, %98, %99, %100, %101, %102, %103, %104, %105, %106, %107, %108, %109, %110, %111, "
-      "%112, %113, %114, %115, %116, %117, %118, %119, %120, %121, %122, %123, %124, %125, %126, %127}, "
-      "%128, %129, p, 1, 1, 0, 0;\n\t"
-      "}\n"
-      : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]),
-        "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15]),
-        "+f"(d[16]), "+f"(d[17]), "+f"(d[18]), "+f"(d[19]), "+f"(d[20]), "+f"(d[21]), "+f"(d[22]), "+f"(d[23]),
-        "+f"(d[24]), "+f"(d[25]), "+f"(d[26]), "+f"(d[27]), "+f"(d[28]), "+f"(d[29]), "+f"(d[30]), "+f"(d[31]),
-        "+f"(d[32]), "+f"(d[33]), "+f"(d[34]), "+f"(d[35]), "+f"(d[36]), "+f"(d[37]), "+f"(d[38]), "+f"(d[39]),
-        "+f"(d[40]), "+f"(d[41]), "+f"(d[42]), "+f"(d[43]), "+f"(d[44]), "+f"(d[45]), "+f"(d[46]), "+f"(d[47]),
-        "+f"(d[48]), "+f"(d[49]), "+f"(d[50]), "+f"(d[51]), "+f"(d[52]), "+f"(d[53]), "+f"(d[54]), "+f"(d[55]),
-        "+f"(d[56]), "+f"(d[57]), "+f"(d[58]), "+f"(d[59]), "+f"(d[60]), "+f"(d[61]), "+f"(d[62]), "+f"(d[63]),
-        "+f"(d[64]), "+f"(d[65]), "+f"(d[66]), "+f"(d[67]), "+f"(d[68]), "+f"(d[69]), "+f"(d[70]), "+f"(d[71]),
-        "+f"(d[72]), "+f"(d[73]), "+f"(d[74]), "+f"(d[75]), "+f"(d[76]), "+f"(d[77]), "+f"(d[78]), "+f"(d[79]),
-        "+f"(d[80]), "+f"(d[81]), "+f"(d[82]), "+f"(d[83]), "+f"(d[84]), "+f"(d[85]), "+f"(d[86]), "+f"(d[87]),
-        "+f"(d[88]), "+f"(d[89]), "+f"(d[90]), "+f"(d[91]), "+f"(d[92]), "+f"(d[93]), "+f"(d[94]), "+f"(d[95]),
-        "+f"(d[96]), "+f"(d[97]), "+f"(d[98]), "+f"(d[99]), "+f"(d[100]), "+f"(d[101]), "+f"(d[102]), "+f"(d[103]),
-        "+f"(d[104]), "+f"(d[105]), "+f"(d[106]), "+f"(d[107]), "+f"(d[108]), "+f"(d[109]), "+f"(d[110]), "+f"(d[111]),
-        "+f"(d[112]), "+f"(d[113]), "+f"(d[114]), "+f"(d[115]), "+f"(d[116]), "+f"(d[117]), "+f"(d[118]), "+f"(d[119]),
-        "+f"(d[120]), "+f"(d[121]), "+f"(d[122]), "+f"(d[123]), "+f"(d[124]), "+f"(d[125]), "+f"(d[126]), "+f"(d[127])
-      : "l"(desc_a), "l"(desc_b), "r"(accumulate)
-      : "memory");
+template <bool FP16>
+__device__ __forceinline__ void wgmma(float (&d)[128], uint64_t desc_a, uint64_t desc_b, uint32_t accumulate) {
+// AB: the operand types of the instruction, the only part that depends on the format
+#define KGE_WGMMA(AB)                                                                                                   \
+  asm volatile(                                                                                                         \
+      "{\n\t"                                                                                                           \
+      ".reg .pred p;\n\t"                                                                                               \
+      "setp.ne.b32 p, %130, 0;\n\t"                                                                                     \
+      "wgmma.mma_async.sync.aligned.m64n256k16.f32." AB " "                                                             \
+      "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, "                                         \
+      "%16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31, "                                \
+      "%32, %33, %34, %35, %36, %37, %38, %39, %40, %41, %42, %43, %44, %45, %46, %47, "                                \
+      "%48, %49, %50, %51, %52, %53, %54, %55, %56, %57, %58, %59, %60, %61, %62, %63, "                                \
+      "%64, %65, %66, %67, %68, %69, %70, %71, %72, %73, %74, %75, %76, %77, %78, %79, "                                \
+      "%80, %81, %82, %83, %84, %85, %86, %87, %88, %89, %90, %91, %92, %93, %94, %95, "                                \
+      "%96, %97, %98, %99, %100, %101, %102, %103, %104, %105, %106, %107, %108, %109, %110, %111, "                    \
+      "%112, %113, %114, %115, %116, %117, %118, %119, %120, %121, %122, %123, %124, %125, %126, %127}, "               \
+      "%128, %129, p, 1, 1, 0, 0;\n\t"                                                                                  \
+      "}\n"                                                                                                             \
+      : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]),                 \
+        "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15]),           \
+        "+f"(d[16]), "+f"(d[17]), "+f"(d[18]), "+f"(d[19]), "+f"(d[20]), "+f"(d[21]), "+f"(d[22]), "+f"(d[23]),         \
+        "+f"(d[24]), "+f"(d[25]), "+f"(d[26]), "+f"(d[27]), "+f"(d[28]), "+f"(d[29]), "+f"(d[30]), "+f"(d[31]),         \
+        "+f"(d[32]), "+f"(d[33]), "+f"(d[34]), "+f"(d[35]), "+f"(d[36]), "+f"(d[37]), "+f"(d[38]), "+f"(d[39]),         \
+        "+f"(d[40]), "+f"(d[41]), "+f"(d[42]), "+f"(d[43]), "+f"(d[44]), "+f"(d[45]), "+f"(d[46]), "+f"(d[47]),         \
+        "+f"(d[48]), "+f"(d[49]), "+f"(d[50]), "+f"(d[51]), "+f"(d[52]), "+f"(d[53]), "+f"(d[54]), "+f"(d[55]),         \
+        "+f"(d[56]), "+f"(d[57]), "+f"(d[58]), "+f"(d[59]), "+f"(d[60]), "+f"(d[61]), "+f"(d[62]), "+f"(d[63]),         \
+        "+f"(d[64]), "+f"(d[65]), "+f"(d[66]), "+f"(d[67]), "+f"(d[68]), "+f"(d[69]), "+f"(d[70]), "+f"(d[71]),         \
+        "+f"(d[72]), "+f"(d[73]), "+f"(d[74]), "+f"(d[75]), "+f"(d[76]), "+f"(d[77]), "+f"(d[78]), "+f"(d[79]),         \
+        "+f"(d[80]), "+f"(d[81]), "+f"(d[82]), "+f"(d[83]), "+f"(d[84]), "+f"(d[85]), "+f"(d[86]), "+f"(d[87]),         \
+        "+f"(d[88]), "+f"(d[89]), "+f"(d[90]), "+f"(d[91]), "+f"(d[92]), "+f"(d[93]), "+f"(d[94]), "+f"(d[95]),         \
+        "+f"(d[96]), "+f"(d[97]), "+f"(d[98]), "+f"(d[99]), "+f"(d[100]), "+f"(d[101]), "+f"(d[102]), "+f"(d[103]),     \
+        "+f"(d[104]), "+f"(d[105]), "+f"(d[106]), "+f"(d[107]), "+f"(d[108]), "+f"(d[109]), "+f"(d[110]), "+f"(d[111]), \
+        "+f"(d[112]), "+f"(d[113]), "+f"(d[114]), "+f"(d[115]), "+f"(d[116]), "+f"(d[117]), "+f"(d[118]), "+f"(d[119]), \
+        "+f"(d[120]), "+f"(d[121]), "+f"(d[122]), "+f"(d[123]), "+f"(d[124]), "+f"(d[125]), "+f"(d[126]), "+f"(d[127])  \
+      : "l"(desc_a), "l"(desc_b), "r"(accumulate)                                                                       \
+      : "memory")
+  if constexpr (FP16) KGE_WGMMA("f16.f16");
+  else KGE_WGMMA("bf16.bf16");
+#undef KGE_WGMMA
 }
 
 // Threshold tests as one FSET each: the bits of 1.0f (0x3F800000) when the test passes, else 0.
@@ -369,22 +340,25 @@ __global__ void __launch_bounds__(THREADS, 1) tc_scan_kernel(const __grid_consta
 #pragma unroll
   for (int i = 0; i < ACC; ++i) acc[i] = 0.f;
 
+  // Flushes what this warp holds for query tile qt: the rows' counts, then the near-tie buffer.  The
+  // near-tie list is kept per QUERY TILE (region = qt) so that the exact recheck of a region touches
+  // only that tile's 128 query rows (they stay L1-resident there).
+  auto flush_tile = [&](long long qt) {
+    if (qt < 0) return;
+#pragma unroll
+    for (int h = 0; h < 2; ++h) {
+      const long long pq = qt * BM + row0 + 8 * h;
+      if (cnt[h] != 0 && pq < p.n_q) atomicAdd(&p.counts[pq], cnt[h]);
+    }
+    if (amb.amb_n > 0) amb.flush(p, qt, lane);
+  };
+
   for (long long u = blockIdx.x; u < units.n_units; u += gridDim.x, ++unit_no) {
    long long qt, ct_lo, ct_hi; units.decode(u, &qt, &ct_lo, &ct_hi);
    for (long long ct = ct_lo; ct < ct_hi; ++ct) {
     const long long q0 = qt * BM + row0;
     if (qt != cur_qt) {
-      if (cur_qt >= 0) {
-#pragma unroll
-        for (int h = 0; h < 2; ++h) {
-          const long long pq = cur_qt * BM + row0 + 8 * h;
-          if (cnt[h] != 0 && pq < p.n_q) atomicAdd(&p.counts[pq], cnt[h]);
-        }
-        // the near-tie list is kept per QUERY TILE (region = qt) so that the exact recheck of a
-        // region touches only that tile's 128 query rows (they stay L1-resident there): flush
-        // what this warp buffered for the previous tile before moving on
-        if (amb.amb_n > 0) amb.flush(p, cur_qt, lane);
-      }
+      flush_tile(cur_qt);
       cur_qt = qt;
 #pragma unroll
       for (int h = 0; h < 2; ++h) {
@@ -427,15 +401,9 @@ __global__ void __launch_bounds__(THREADS, 1) tc_scan_kernel(const __grid_consta
       for (int k = 0; k < G::K16; ++k) {
         if (k < k16s) {
           const uint64_t adv = (uint64_t)(k * 2);  // 16 values = 32 B = 2 x 16-B units
-          if constexpr (FP16) {
-            wgmma_fp16(acc, a_hi + adv, b_hi + adv, (kb | k) ? 1u : 0u);
-            wgmma_fp16(acc, a_lo + adv, b_hi + adv, 1u);
-            wgmma_fp16(acc, a_hi + adv, b_lo + adv, 1u);
-          } else {
-            wgmma_bf16(acc, a_hi + adv, b_hi + adv, (kb | k) ? 1u : 0u);
-            wgmma_bf16(acc, a_lo + adv, b_hi + adv, 1u);
-            wgmma_bf16(acc, a_hi + adv, b_lo + adv, 1u);
-          }
+          wgmma<FP16>(acc, a_hi + adv, b_hi + adv, (kb | k) ? 1u : 0u);
+          wgmma<FP16>(acc, a_lo + adv, b_hi + adv, 1u);
+          wgmma<FP16>(acc, a_hi + adv, b_lo + adv, 1u);
         }
       }
       wg_commit();
@@ -564,14 +532,7 @@ __global__ void __launch_bounds__(THREADS, 1) tc_scan_kernel(const __grid_consta
     cnt[1] += ones_count(ones_gt[1]);
    }
   }
-  if (cur_qt >= 0) {
-#pragma unroll
-    for (int h = 0; h < 2; ++h) {
-      const long long pq = cur_qt * BM + row0 + 8 * h;
-      if (cnt[h] != 0 && pq < p.n_q) atomicAdd(&p.counts[pq], cnt[h]);
-    }
-    if (amb.amb_n > 0) amb.flush(p, cur_qt, lane);   // final flush of this warp's near-tie buffer
-  }
+  flush_tile(cur_qt);
 }
 
 // ------------------------------------------------------------------------------------------
@@ -1083,17 +1044,10 @@ cudaError_t launch_pack_a(const float* qplain, int qw, long long n_q, int dim, i
 namespace {
 template <bool L2, bool DUMP, bool F16, int BKT, bool RES>
 cudaError_t launch_kernel(const TcScanParams& p, int grid, size_t smem, cudaStream_t st) {
-  // per template instantiation AND per device (the attribute is a per-device property)
-  static bool configured[64] = {};
-  int dev = 0;
-  if (cudaGetDevice(&dev) != cudaSuccess) return cudaErrorInvalidDevice;
-  if (dev < 0 || dev >= 64 || !configured[dev]) {
-    const cudaError_t e = cudaFuncSetAttribute(tc_scan_kernel<L2, DUMP, F16, BKT, RES>,
-                                               cudaFuncAttributeMaxDynamicSharedMemorySize, (int)SMEM_LIMIT);
-    if (e != cudaSuccess) return e;
-    if (dev >= 0 && dev < 64) configured[dev] = true;
-  }
-  tc_scan_kernel<L2, DUMP, F16, BKT, RES><<<grid, THREADS, smem, st>>>(p);
+  constexpr auto kernel = tc_scan_kernel<L2, DUMP, F16, BKT, RES>;
+  const cudaError_t e = set_attribute_once<kernel>(cudaFuncAttributeMaxDynamicSharedMemorySize, (int)SMEM_LIMIT);
+  if (e != cudaSuccess) return e;
+  kernel<<<grid, THREADS, smem, st>>>(p);
   return cudaGetLastError();
 }
 

@@ -1341,54 +1341,40 @@ __host__ inline size_t ring_smem_bytes(const MarginStepParams& a) {
   return WARPS_PER_BLOCK * ((per_warp + 127) & ~(size_t)127);
 }
 // KGE_TRAIN_RING=0 selects the register-resident form (margin_step_fast_kernel; the sharded step then
-// takes the generic kernels).  Codes hold 31-bit row numbers: of the table, or of the shard.
+// takes the generic kernels).  Codes hold 31-bit row numbers: of the table, or of the shard; a relation
+// step's codes (a.n_rel > 0) 30-bit row numbers of either table.
 __host__ inline bool ring_step_ok(const MarginStepParams& a) {
   static const bool enabled = [] { const char* v = getenv("KGE_TRAIN_RING"); return !(v && v[0] == '0'); }();
   const long long rows = a.hrows ? a.n_rows : a.n_ent;
-  return enabled && a.n_neg <= 8192 && rows < 0x7FFFFFFFll && ring_smem_bytes(a) <= 96 * 1024;
+  const long long row_limit = a.n_rel > 0 ? 0x3FFFFFFFll : 0x7FFFFFFFll;
+  return enabled && a.n_neg <= 8192 && rows < row_limit && a.n_rel < 0x3FFFFFFFll && ring_smem_bytes(a) <= 96 * 1024;
 }
 
 // REL: margin_step_ring_rel_kernel (MINB is 0 there)
 template <int MODEL, bool BWD, int MINB, bool SHARD = false, int LOSS = KGE_LOSS_MARGIN, bool REL = false>
 cudaError_t launch_ring_variant(const MarginStepParams& a, const TrainGrads& gr, const float* gloss, cudaStream_t st) {
-  void (*kernel)(MarginStepParams, TrainGrads, const float*) =
+  constexpr void (*kernel)(MarginStepParams, TrainGrads, const float*) =
       REL ? margin_step_ring_rel_kernel<MODEL, BWD, SHARD, LOSS> : margin_step_ring_kernel<MODEL, BWD, MINB, SHARD, LOSS>;
   const size_t smem = ring_smem_bytes(a);
-  static bool configured[64] = {};
-  int dev = 0;
-  cudaError_t e = cudaGetDevice(&dev);
-  if (e != cudaSuccess) return e;
-  if (smem > 48 * 1024 && (dev < 0 || dev >= 64 || !configured[dev])) {
-    e = cudaFuncSetAttribute(kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, 96 * 1024);
+  if (smem > 48 * 1024) {
+    const cudaError_t e = set_attribute_once<kernel>(cudaFuncAttributeMaxDynamicSharedMemorySize, 96 * 1024);
     if (e != cudaSuccess) return e;
-    if (dev >= 0 && dev < 64) configured[dev] = true;
   }
   const unsigned blocks = (unsigned)((a.b + WARPS_PER_BLOCK - 1) / WARPS_PER_BLOCK);
   kernel<<<blocks, WARPS_PER_BLOCK * 32, smem, st>>>(a, gr, gloss);
   return cudaGetLastError();
 }
 
-// The relation-corrupting ring step, one kernel per (loss kind, sharded)
-template <int MODEL, bool BWD>
-cudaError_t launch_ring_rel(const MarginStepParams& a, const TrainGrads& gr, const float* gloss, cudaStream_t st) {
-  auto by_shard = [&](auto loss) -> cudaError_t {
-    constexpr int LOSS = decltype(loss)::value;
-    if (a.hrows) return launch_ring_variant<MODEL, BWD, 0, true, LOSS, true>(a, gr, gloss, st);
-    return launch_ring_variant<MODEL, BWD, 0, false, LOSS, true>(a, gr, gloss, st);
-  };
-  switch (a.loss_kind) {
-    case KGE_LOSS_LOGISTIC: return by_shard(std::integral_constant<int, KGE_LOSS_LOGISTIC>{});
-    case KGE_LOSS_BCE: return by_shard(std::integral_constant<int, KGE_LOSS_BCE>{});
-    default: return by_shard(std::integral_constant<int, KGE_LOSS_MARGIN>{});
-  }
-}
-
-// One ring kernel per (loss kind, sharded).  KGE_TRAIN_BWD_BLOCKS=5 holds the backward kernel to 96
-// registers (5 CTAs = 20 warps per SM; the unsharded margin step only).
+// One ring kernel per (relation or entity step, loss kind, sharded).  KGE_TRAIN_BWD_BLOCKS=5 holds the
+// backward kernel to 96 registers (5 CTAs = 20 warps per SM; the unsharded entity step with the margin
+// loss only).
 template <int MODEL, bool BWD>
 cudaError_t launch_ring(const MarginStepParams& a, const TrainGrads& gr, const float* gloss, cudaStream_t st) {
   auto by_shard = [&](auto loss) -> cudaError_t {
     constexpr int LOSS = decltype(loss)::value;
+    if (a.n_rel > 0)
+      return a.hrows ? launch_ring_variant<MODEL, BWD, 0, true, LOSS, true>(a, gr, gloss, st)
+                     : launch_ring_variant<MODEL, BWD, 0, false, LOSS, true>(a, gr, gloss, st);
     if (a.hrows) return launch_ring_variant<MODEL, BWD, 0, true, LOSS>(a, gr, gloss, st);
     if constexpr (BWD && LOSS == KGE_LOSS_MARGIN) {
       static const bool tight = [] { const char* v = getenv("KGE_TRAIN_BWD_BLOCKS"); return v && v[0] == '5'; }();
@@ -1515,55 +1501,30 @@ cudaError_t with_fast_model(int model, F&& f) {
   }
 }
 
-// The ring kernel where it applies; else, unsharded with the margin loss, the register-resident form;
-// else the generic kernels.  An entity-sharded step (a.hrows) that holds no rows scores no negative.
+// The ring kernel where it applies; else, for an unsharded entity step with the margin loss, the
+// register-resident form; else the generic kernels.  An entity-sharded step (a.hrows) that holds no
+// rows scores no negative.
+//
+// A relation-corrupting step (a.n_rel > 0): at rel_share >= 1 its draws are the entity step's
+// (draw_rel), so without caller negatives or an nr_out to fill it is that step.  Otherwise TransE-L1 /
+// L2 and DistMult take the ring kernel's relation kind (margin_step_ring_rel_kernel) where the ring
+// applies; everything else, and KGE_TRAIN_RING=0, takes the generic kernels, which score a negative from
+// its own (nh, nt, nr).
 template <bool BWD>
-cudaError_t launch_margin_step(const MarginStepParams& a, const TrainGrads& gr, const float* gloss,
-                               cudaStream_t st);
-
-// A relation-corrupting step.  At rel_share >= 1 its draws are the entity step's (draw_rel), so without
-// caller negatives or an nr_out to fill it is that step, on whichever kernel that one takes.  Otherwise:
-// TransE-L1 / L2 and DistMult take the ring kernel's relation kind (margin_step_ring_rel_kernel) where
-// the ring applies (its codes then hold 30-bit row numbers); everything else, and KGE_TRAIN_RING=0, the
-// generic kernels, which score a negative from its own (nh, nt, nr).  The register-resident form has no
-// relation kind.
-template <bool BWD>
-cudaError_t launch_rel_step(const MarginStepParams& a, const TrainGrads& gr, const float* gloss, cudaStream_t st) {
-  if (a.rel_share >= 1.f && !a.nh && !a.nr_out) {
-    MarginStepParams e = a;
-    e.n_rel = 0;
-    return launch_margin_step<BWD>(e, gr, gloss, st);
-  }
-  const bool shard = a.hrows != nullptr;
-  if (a.b <= 0 || (shard && a.n_rows <= 0)) return cudaSuccess;
-  const long long rows = shard ? a.n_rows : a.n_ent;
-  if (fast_step_ok(a) && ring_step_ok(a) && rows < 0x3FFFFFFFll && a.n_rel < 0x3FFFFFFFll)
-    return with_fast_model(a.model, [&](auto m) { return launch_ring_rel<decltype(m)::value, BWD>(a, gr, gloss, st); });
-  const unsigned blocks = blocks_for_warps(a.b);
-  if constexpr (BWD) {
-    if (shard) margin_step_shard_bwd_kernel<<<blocks, WARPS_PER_BLOCK * 32, 0, st>>>(a, gr, gloss);
-    else margin_step_bwd_kernel<<<blocks, WARPS_PER_BLOCK * 32, 0, st>>>(a, gr, gloss);
-  } else {
-    if (shard) margin_step_shard_fwd_kernel<<<blocks, WARPS_PER_BLOCK * 32, 0, st>>>(a);
-    else margin_step_fwd_kernel<<<blocks, WARPS_PER_BLOCK * 32, 0, st>>>(a);
-  }
-  return cudaGetLastError();
-}
-
-template <bool BWD>
-cudaError_t launch_margin_step(const MarginStepParams& a, const TrainGrads& gr, const float* gloss,
-                               cudaStream_t st) {
-  if (a.n_rel > 0) return launch_rel_step<BWD>(a, gr, gloss, st);
+cudaError_t launch_margin_step(MarginStepParams a, const TrainGrads& gr, const float* gloss, cudaStream_t st) {
+  if (a.n_rel > 0 && a.rel_share >= 1.f && !a.nh && !a.nr_out) a.n_rel = 0;
   const bool shard = a.hrows != nullptr;
   if (a.b <= 0 || (shard && a.n_rows <= 0)) return cudaSuccess;
   const unsigned blocks = blocks_for_warps(a.b);
   if (fast_step_ok(a) && ring_step_ok(a))
     return with_fast_model(a.model, [&](auto m) { return launch_ring<decltype(m)::value, BWD>(a, gr, gloss, st); });
-  if (!shard && fast_step_ok(a) && a.loss_kind == KGE_LOSS_MARGIN) {
-    return with_fast_model(a.model, [&](auto m) {
-      margin_step_fast_kernel<decltype(m)::value, BWD><<<blocks, WARPS_PER_BLOCK * 32, 0, st>>>(a, gr, gloss);
-      return cudaGetLastError();
-    });
+  if (a.n_rel <= 0) {   // the register-resident form has no relation kind
+    if (!shard && fast_step_ok(a) && a.loss_kind == KGE_LOSS_MARGIN) {
+      return with_fast_model(a.model, [&](auto m) {
+        margin_step_fast_kernel<decltype(m)::value, BWD><<<blocks, WARPS_PER_BLOCK * 32, 0, st>>>(a, gr, gloss);
+        return cudaGetLastError();
+      });
+    }
   }
   if constexpr (BWD) {
     if (shard) margin_step_shard_bwd_kernel<<<blocks, WARPS_PER_BLOCK * 32, 0, st>>>(a, gr, gloss);
