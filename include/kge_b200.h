@@ -470,6 +470,31 @@ typedef struct {
 int kge_rel_step_fwd(const kge_rel_step_args_t* a);
 int kge_rel_step_bwd(const kge_rel_step_args_t* a, const kge_grads_t* g, const float* grad_loss);
 
+/* ---- positional negatives (PositionalNegativeSampler, sampling.py:330-503) ------------------------------
+ * kge_pos_step_fwd / _bwd: the fused step of kge_margin_step_fwd / _bwd with each negative drawn in the kernel
+ * from the entities seen in its position for its relation.  The candidates are two CSR arrays per side:
+ * relation r's heads are head_ents[head_offs[r] .. head_offs[r+1]), sorted, and likewise for tails.  Philox4x32-10
+ * as kge_corrupt_batch (key = seed, counter = (j*b+i, offset)): word x replaces the head iff
+ * (x >> 8) / 2^24 < bern_probs[r[i]], else the tail; word y picks the replacement ents[offs[r] + ((y n) >> 32)],
+ * n = offs[r+1] - offs[r], or, when that slice is empty, (y n_ent) >> 32, uniform on [0, n_ent) -- entity 0
+ * included, as in the reference.  Exactly one end is replaced; true triples are not rejected.  base.nh_out /
+ * base.nt_out (optional, unsharded only) receive the negatives.  Entity-sharded (base.hrows != NULL): every
+ * rank makes the same draws and a negative is scored by the rank holding its replaced entity, as in
+ * kge_margin_step_fwd.  The argument rules are those of kge_margin_step_fwd / _bwd, plus: n_rel >= 1, both
+ * offset arrays given (n_rel + 1 entries each), an ents array NULL only when all its slices are empty, and
+ * base.nh / base.nt NULL (no caller negatives).  The caller guarantees r[i] < n_rel, non-decreasing offsets
+ * and stored entities < base.n_ent. */
+typedef struct {
+  kge_margin_step_args_t base;
+  int64_t n_rel;                        /* relations the CSR arrays cover */
+  const int64_t* head_offs;             /* (n_rel + 1) offsets into head_ents */
+  const int64_t* head_ents;             /* candidate heads, sorted within each relation */
+  const int64_t* tail_offs;             /* (n_rel + 1) offsets into tail_ents */
+  const int64_t* tail_ents;             /* candidate tails, sorted within each relation */
+} kge_pos_step_args_t;
+int kge_pos_step_fwd(const kge_pos_step_args_t* a);
+int kge_pos_step_bwd(const kge_pos_step_args_t* a, const kge_grads_t* g, const float* grad_loss);
+
 /* ---- measurement hook ------------------------------------------------------------------
  * When enabled, the dominant kernels of kge_rank_side / kge_score_all are bracketed by CUDA
  * events recorded on the launch stream: kind 0 = scalar dense scan, 1 = tensor-core scan,

@@ -1,0 +1,277 @@
+"""CPU tests of the positional fused step (PositionalNegativeSampler.fused_step, fused_*_step(positional=...)):
+the host logic of the entity-sharded step over gloo with an oracle-backed stand-in engine (a negative is
+scored by the rank holding the entity it draws; the ranks' sums give the unsharded loss and gradients; the
+agreement tells the positional step from the entity step and compares the candidate CSRs' sizes), the
+argument errors raised before any collective or kernel, the argument rules of kge_pos_step_* in a child
+process that sees no GPU, and kge_pos_step_args_t against its binding."""
+import json
+import os
+import re
+import subprocess
+import sys
+
+import pytest
+import torch
+
+import torchkge_b200 as tk
+from oracle import kge_oracle as oracle
+from tests import gloo, helpers
+from tests.test_train_loss_sharding_gloo import pair_loss
+from tests.test_train_sharding_gloo import _ENT_KEYS, _KIND_OF_CODE, _REL_KEYS, CountingShard, OracleStepEngine, \
+    _local_model
+from torchkge_b200 import _lib
+from torchkge_b200.engine import EntityShard, QueryShard
+from torchkge_b200.training import fused_loss_step, fused_margin_step, sharded_margin_step
+
+ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
+
+
+def csr(rel, ent, n_rel, n_ent):
+    key = torch.unique(rel * n_ent + ent)
+    offs = torch.zeros(n_rel + 1, dtype=torch.int64)
+    offs[1:] = torch.cumsum(torch.bincount(key // n_ent, minlength=n_rel), 0)
+    return offs, key % n_ent
+
+
+def positional_of(n_ent, n_rel, seed, n=40):
+    g = torch.Generator().manual_seed(seed)
+    rel = torch.randint(1, n_rel, (n,), generator=g)            # relation 0 has no candidates
+    hd, tl = torch.randint(0, n_ent, (n,), generator=g), torch.randint(0, n_ent, (n,), generator=g)
+    return csr(rel, hd, n_rel, n_ent) + csr(rel, tl, n_rel, n_ent)
+
+
+def pos_draws(seed, offset, r, n_neg, probs, n_ent, pos):
+    """The stand-in's positional draws: (head?, replacement), a function of (seed, offset), the CSR and n_ent."""
+    g = torch.Generator().manual_seed((seed * 1000003 + offset) % (1 << 62))
+    n = n_neg * r.shape[0]
+    u, v = torch.rand(n, generator=g), torch.rand(n, generator=g)
+    R = r.repeat(n_neg)
+    head = u < probs[R]
+    ho, he, to, te = pos
+    lo = torch.where(head, ho[R], to[R])
+    cnt = torch.where(head, ho[R + 1] - ho[R], to[R + 1] - to[R])
+    k = (v * cnt).long().clamp(max=(cnt - 1).clamp(min=0))
+    pick = lo + k
+    hv = he[pick.clamp(max=max(he.numel() - 1, 0))] if he.numel() else torch.zeros_like(pick)
+    tv = te[pick.clamp(max=max(te.numel() - 1, 0))] if te.numel() else torch.zeros_like(pick)
+    e = torch.where(cnt > 0, torch.where(head, hv, tv), (v * n_ent).long().clamp(max=n_ent - 1))
+    return head, e
+
+
+class PosStepEngine(OracleStepEngine):
+    """The stand-in engine of a positional step: a negative on the rank holding its drawn entity."""
+
+    def _partial(self, step, tables, h, t, r, probs, hrows, trows, grad):
+        assert step.pos is not None and step.n_rel == 0
+        kind = _KIND_OF_CODE[step.code]
+        b, n = h.shape[0], step.n_rows
+        ent = [x for x in tables[:2] if x is not None]
+        P = {}
+        for p, key in enumerate(_ENT_KEYS[kind]):
+            P[key] = torch.cat([ent[p], hrows[:, p], trows[:, p]]).clone().requires_grad_(grad)
+        for p, key in enumerate(_REL_KEYS[kind]):
+            P[key] = tables[2 + p].clone().requires_grad_(grad)
+        head, e = pos_draws(step.seed, step.offset, r, step.n_neg, probs, step.n_ent, step.pos)
+        own = (e >= step.ent_lo) & (e < step.ent_lo + n)
+        i = torch.arange(b).repeat(step.n_neg)[own]
+        loc, head = e[own] - step.ent_lo, head[own]
+        nh = torch.where(head, loc, n + i)
+        nt = torch.where(head, n + b + i, loc)
+        pos = oracle.score_triples(kind, P, n + i, n + b + i, r[i])
+        neg = oracle.score_triples(kind, P, nh, nt, r[i])
+        return pair_loss(step.loss_kind, pos, neg), P
+
+
+def _reference(kind, loss_kind, model, h, t, r, probs, seed, offset, n_neg, n_ent, pos):
+    P = {k: v.requires_grad_(True) for k, v in helpers.oracle_params(kind, model).items()}
+    head, e = pos_draws(seed, offset, r, n_neg, probs, n_ent, pos)
+    nh = torch.where(head, e, h.repeat(n_neg))
+    nt = torch.where(head, t.repeat(n_neg), e)
+    p = oracle.score_triples(kind, P, h, t, r).repeat(n_neg)
+    neg = oracle.score_triples(kind, P, nh, nt, r.repeat(n_neg))
+    loss = pair_loss(loss_kind, p, neg)
+    loss.backward()
+    return loss.item(), {k: v.grad for k, v in P.items()}
+
+
+def _run(rank, world, kind, loss_kind, n_ent, b, n_neg):
+    n_rel, dim = 5, 8
+    model = helpers.make_model(kind, dim, n_ent, n_rel, seed=31)
+    shard = CountingShard(n_ent, rank, world, None, local_storage=True)
+    local = _local_model(kind, model, shard.lo, shard.hi, n_rel, dim)
+    probs = torch.tensor([0.5, 1.0, 0.0, 0.3, 0.8])
+    pos = positional_of(n_ent, n_rel, seed=2)
+    eng = PosStepEngine()
+    g = torch.Generator().manual_seed(100)
+    h, t = torch.randint(0, n_ent, (b,), generator=g), torch.randint(0, n_ent, (b,), generator=g)
+    r = torch.randint(0, n_rel, (b,), generator=g)
+    loss = sharded_margin_step(local, h, t, r, 0.0, n_neg, probs, 7, 1, shard, engine=eng, loss_kind=loss_kind,
+                               positional=pos)
+    loss.backward()
+    want_loss, want = _reference(kind, loss_kind, model, h, t, r, probs, 7, 1, n_neg, n_ent, pos)
+    ok = {"loss": abs(loss.item() - want_loss) <= 1e-5 * max(1.0, abs(want_loss))}
+    names = dict(zip(_ENT_KEYS[kind], ("ent_emb.weight",) if kind != "complex" else
+                     ("re_ent_emb.weight", "im_ent_emb.weight")))
+    names.update(zip(_REL_KEYS[kind], ("rel_emb.weight",) if kind != "complex" else
+                     ("re_rel_emb.weight", "im_rel_emb.weight")))
+    params = dict(local.named_parameters())
+    for key, name in names.items():
+        ref = want[key][shard.lo:shard.hi] if "ent" in key else want[key]
+        ok[key] = torch.allclose(params[name].grad, ref, rtol=1e-4, atol=1e-6)
+    # the entity step's collectives, plus one for the CSR sizes
+    ok["collectives"] = [c[0] for c in shard.collectives] == ["stack_all", "stack_all", "all_reduce", "all_reduce",
+                                                               "all_reduce"]
+    ok["agreement_fields"] = [c[1] for c in shard.collectives[:2]] == [6, 4]
+    ok["empty_rank_skips_kernels"] = (shard.hi > shard.lo) or eng.calls == []
+    return ok
+
+
+def _worker(rank, world, case):
+    try:
+        if case[0] in ("csr", "kind"):
+            shard = EntityShard.from_group(30, local_storage=True)
+            model = _local_model("distmult", helpers.make_model("distmult", 8, 30, 4, seed=1), shard.lo, shard.hi, 4, 8)
+            h = torch.arange(5)
+            pos = positional_of(30, 4, seed=3, n=40 if rank == 0 else 41)
+            if case[0] == "kind" and rank == 1:
+                pos = None
+            try:
+                fused_loss_step(model, h, h, h % 4, tk.LogisticLoss(), n_neg=3, bern_probs=torch.full((4,), 0.5),
+                                seed=11, offset=1, shard=shard, positional=pos)
+                return {"raised": False}
+            except ValueError as e:
+                return {"raised": ("CSR" if case[0] == "csr" else "positional") in str(e)}
+        return _run(rank, world, *case)
+    except Exception as e:          # reported by the parent
+        return {"error": "%s: %s" % (type(e).__name__, e)}
+
+
+# (world, kind, loss kind, n_ent, b, n_neg)
+CASES = [
+    (2, "distmult", _lib.LOSS_LOGISTIC, 40, 12, 5),
+    (2, "complex", _lib.LOSS_MARGIN, 31, 9, 4),
+    (3, "transe_l2", _lib.LOSS_BCE, 2, 6, 3),       # n_ent < world: rank 2 holds nothing
+    (3, "distmult", _lib.LOSS_MARGIN, 50, 10, 3),
+]
+
+
+@pytest.mark.parametrize("case", CASES, ids=["%s-loss%d-w%d" % (c[1], c[2], c[0]) for c in CASES])
+def test_sharded_pos_step_equals_oracle(case):
+    world = case[0]
+    ret = gloo.spawn(world, _worker, case[1:])
+    for rank in range(world):
+        res = ret[rank]
+        assert "error" not in res, "rank %d: %s" % (rank, res.get("error"))
+        bad = [k for k, v in res.items() if not v]
+        assert not bad, "rank %d: %s" % (rank, bad)
+
+
+@pytest.mark.parametrize("what", ["csr", "kind"])
+def test_mismatch_raises_on_every_rank(what):
+    """Ranks whose CSRs differ in size, or where one runs the entity step, raise on every rank."""
+    assert gloo.spawn(2, _worker, (what,)) == {0: {"raised": True}, 1: {"raised": True}}
+
+
+def test_argument_errors():
+    kg, _, _ = helpers.make_kg(60, 5, n_facts=200, n_test=5, seed=1)
+    s = tk.PositionalNegativeSampler(kg, seed=4)
+    u = tk.UniformNegativeSampler(kg, seed=4)
+    model = helpers.make_model("distmult", 8, 60, 5, seed=2)
+    h = torch.arange(4)
+    for sampler in (s, u):
+        with pytest.raises(ValueError, match="exactly one"):
+            sampler.fused_step(model, h, h, h)
+        with pytest.raises(TypeError, match="MSELoss"):
+            sampler.fused_step(model, h, h, h, criterion=torch.nn.MSELoss())
+        with pytest.raises(ValueError, match="QueryShard"):
+            sampler.fused_step(model, h, h, h, margin=1.0, shard=QueryShard(10, 0, 1))
+        with pytest.raises(_lib.KgeLibraryError, match="CUDA"):    # CPU tensors: no CPU path
+            sampler.fused_step(model, h, h, h, margin=1.0)
+    calls = s._calls
+    with pytest.raises(ValueError, match="entities"):     # before the call count moves
+        s.fused_step(helpers.make_model("distmult", 8, 61, 5, seed=2), h, h, h, margin=1.0)
+    with pytest.raises(ValueError, match="entities"):
+        s.fused_step(model, h, h, h, margin=1.0, shard=EntityShard(99, 0, 2, local_storage=True))
+    assert s._calls == calls
+    with pytest.raises(ValueError, match="relations"):
+        s.fused_step(helpers.make_model("distmult", 8, 60, 6, seed=2), h, h, h, margin=1.0)
+    pos = positional_of(60, 5, seed=1)
+    probs = torch.full((5,), 0.5)
+    with pytest.raises(ValueError, match="caller negatives"):
+        fused_loss_step(model, h, h, h, tk.LogisticLoss(), negatives=(h, h), positional=pos)
+    with pytest.raises(ValueError, match="rel_share"):
+        fused_margin_step(model, h, h, h, 1.0, bern_probs=probs, positional=pos, rel_share=0.5)
+    with pytest.raises(ValueError, match="rel_share"):
+        fused_margin_step(model, h, h, h, 1.0, bern_probs=probs, positional=pos, rel_share=0.5,
+                          shard=EntityShard(60, 0, 1, local_storage=True))
+    with pytest.raises(ValueError, match="covers 4 relations"):
+        fused_margin_step(model, h, h, h, 1.0, bern_probs=probs, positional=positional_of(60, 4, seed=1))
+    with pytest.raises(ValueError, match="covers 4 relations"):
+        fused_margin_step(model, h, h, h, 1.0, bern_probs=probs, positional=positional_of(60, 4, seed=1),
+                          shard=EntityShard(60, 0, 1, local_storage=True))
+    with pytest.raises(ValueError, match="head_offs, head_ents"):
+        fused_margin_step(model, h, h, h, 1.0, bern_probs=probs, positional=pos[:2])
+
+
+_ABI_CHILD = r"""
+import ctypes, json, sys
+sys.path.insert(0, sys.argv[1])
+from torchkge_b200 import _lib
+lib = _lib.load()
+F = 8   # a non-NULL stand-in pointer: every call below fails its checks before touching memory
+res = {}
+def ok_args():
+    a = _lib.PosStepArgs()
+    b = a.base
+    b.tb.model, b.tb.dim, b.tb.ent0, b.tb.rel0 = _lib.DISTMULT, 8, F, F
+    b.n_neg, b.b, b.n_ent, b.h, b.t, b.r, b.bern_probs, b.loss = 2, 4, 10, F, F, F, F, F
+    a.n_rel, a.head_offs, a.head_ents, a.tail_offs, a.tail_ents = 5, F, F, F, F
+    return a
+g = _lib.Grads(F, None, F, None)
+cases = {
+    "null": lambda a: None,
+    "n_rel_0": lambda a: setattr(a, "n_rel", 0),
+    "no_head_offs": lambda a: setattr(a, "head_offs", None),
+    "no_tail_offs": lambda a: setattr(a, "tail_offs", None),
+    "caller_negatives": lambda a: (setattr(a.base, "nh", F), setattr(a.base, "nt", F)),
+    "no_probs": lambda a: setattr(a.base, "bern_probs", None),
+    "bad_loss_kind": lambda a: setattr(a.base, "loss_kind", 7),
+    "no_loss": lambda a: setattr(a.base, "loss", None),
+    "sharded_nh_out": lambda a: (setattr(a.base, "hrows", F), setattr(a.base, "trows", F),
+                                 setattr(a.base, "n_rows", 10), setattr(a.base, "nh_out", F),
+                                 setattr(a.base, "nt_out", F)),
+    "sharded_rows_past_n_ent": lambda a: (setattr(a.base, "hrows", F), setattr(a.base, "trows", F),
+                                          setattr(a.base, "n_rows", 11)),
+}
+for name, edit in cases.items():
+    a = ok_args()
+    edit(a)
+    p = None if name == "null" else ctypes.byref(a)
+    res["fwd_" + name] = lib.kge_pos_step_fwd(p)
+    res["bwd_" + name] = lib.kge_pos_step_bwd(p, ctypes.byref(g), F)
+a = ok_args()
+res["bwd_no_grad_loss"] = lib.kge_pos_step_bwd(ctypes.byref(a), ctypes.byref(g), None)
+res["bwd_no_grads"] = lib.kge_pos_step_bwd(ctypes.byref(a), None, F)
+a.base.hrows, a.base.trows, a.base.n_rows = F, F, 10
+res["bwd_sharded_no_grad_rows"] = lib.kge_pos_step_bwd(ctypes.byref(a), ctypes.byref(g), F)
+print(json.dumps(res))
+"""
+
+
+def test_entry_points_reject_malformed_calls_without_a_gpu():
+    env = dict(os.environ, CUDA_VISIBLE_DEVICES="")
+    proc = subprocess.run([sys.executable, "-c", _ABI_CHILD, ROOT], env=env, capture_output=True, text=True,
+                          timeout=300)
+    assert proc.returncode == 0, proc.stderr[-3000:]
+    res = json.loads(proc.stdout.strip().splitlines()[-1])
+    assert res == {k: 1 for k in res}    # KGE_ERR_ARG
+
+
+def test_pos_step_struct_matches_the_header_in_order():
+    """kge_pos_step_args_t in include/kge_b200.h, field by field, is _lib.PosStepArgs."""
+    header = re.sub(r"/\*.*?\*/", "", open(os.path.join(ROOT, "include", "kge_b200.h")).read(), flags=re.S)
+    body = re.search(r"typedef struct \{([^{}]*)\}\s*kge_pos_step_args_t\s*;", header, flags=re.S).group(1)
+    names = [re.findall(r"[A-Za-z_][A-Za-z0-9_]*", part)[-1]
+             for decl in body.split(";") if decl.strip() for part in decl.split(",")]
+    assert names == [n for n, _ in _lib.PosStepArgs._fields_]
+    assert _lib.PosStepArgs._fields_[0] == ("base", _lib.MarginStepArgs)

@@ -104,6 +104,14 @@ class RelStepArgs(ctypes.Structure):
     ]
 
 
+class PosStepArgs(ctypes.Structure):
+    """kge_pos_step_args_t"""
+    _fields_ = [
+        ("base", MarginStepArgs), ("n_rel", _c.c_int64),
+        ("head_offs", _p), ("head_ents", _p), ("tail_offs", _p), ("tail_ents", _p),
+    ]
+
+
 # name -> (restype, argtypes); every symbol include/kge_b200.h declares
 SIGNATURES = {
     "kge_abi_version": (_c.c_int, []),
@@ -153,6 +161,8 @@ SIGNATURES = {
                                          _c.c_float, _c.c_uint64, _c.c_uint64, _p, _p, _p, _p]),
     "kge_rel_step_fwd": (_c.c_int, [_c.POINTER(RelStepArgs)]),
     "kge_rel_step_bwd": (_c.c_int, [_c.POINTER(RelStepArgs), _c.POINTER(Grads), _p]),
+    "kge_pos_step_fwd": (_c.c_int, [_c.POINTER(PosStepArgs)]),
+    "kge_pos_step_bwd": (_c.c_int, [_c.POINTER(PosStepArgs), _c.POINTER(Grads), _p]),
     "kge_scan_timing_enable": (_c.c_int, [_c.c_int]),
     "kge_scan_timing_read": (_c.c_int, [_c.c_int, _c.POINTER(_c.c_int64), _c.POINTER(_c.c_double)]),
 }

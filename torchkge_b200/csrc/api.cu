@@ -806,6 +806,9 @@ kge::MarginStepParams to_step(const kge_margin_step_args_t* a) {
   p.n_rel = 0; p.rel_share = 1.f; p.nr = nullptr; p.nr_out = nullptr;   // the entity step
   return p;
 }
+kge::PosCSR to_pos_csr(const kge_pos_step_args_t* a) {
+  return kge::PosCSR{a->head_offs, a->head_ents, a->tail_offs, a->tail_ents};
+}
 kge::MarginStepParams to_rel_step(const kge_rel_step_args_t* a) {
   kge::MarginStepParams p = to_step(&a->base);
   p.n_rel = a->n_rel; p.rel_share = a->rel_share; p.nr = a->nr; p.nr_out = a->nr_out;
@@ -853,6 +856,26 @@ bool rel_step_ok(const kge_rel_step_args_t* a) {
   if ((a->nr == nullptr) != (a->base.nh == nullptr)) return false;
   if (a->base.hrows && a->nr_out) return false;   // sharded: no per-negative outputs
   return true;
+}
+// An ents array may be NULL only when offs[n_rel] == offs[0]: read from the device, on the step's stream, in
+// that case alone (an empty side), so a well-formed step never waits for the device here.
+bool pos_side_ok(const int64_t* offs, const int64_t* ents, int64_t n_rel, void* stream) {
+  if (ents) return true;
+  int64_t ends[2] = {0, 1};
+  cudaStream_t st = static_cast<cudaStream_t>(stream);
+  if (cudaMemcpyAsync(&ends[0], offs, sizeof(int64_t), cudaMemcpyDeviceToHost, st) != cudaSuccess ||
+      cudaMemcpyAsync(&ends[1], offs + n_rel, sizeof(int64_t), cudaMemcpyDeviceToHost, st) != cudaSuccess ||
+      cudaStreamSynchronize(st) != cudaSuccess) {
+    cudaGetLastError();   // a bad offs pointer is an argument error, not a sticky one
+    return false;
+  }
+  return ends[0] == ends[1];
+}
+bool pos_step_ok(const kge_pos_step_args_t* a) {
+  if (!a || !step_ok(&a->base) || a->n_rel < 1 || !a->head_offs || !a->tail_offs) return false;
+  if (a->base.nh) return false;   // caller negatives would make the draw meaningless
+  return pos_side_ok(a->head_offs, a->head_ents, a->n_rel, a->base.stream) &&
+         pos_side_ok(a->tail_offs, a->tail_ents, a->n_rel, a->base.stream);
 }
 }  // namespace
 
@@ -990,6 +1013,27 @@ int kge_rel_step_bwd(const kge_rel_step_args_t* a, const kge_grads_t* g, const f
   KGE_CUDA_TRY(kge::launch_margin_step_bwd(to_rel_step(a), to_grads(g), grad_loss,
                                            static_cast<cudaStream_t>(a->base.stream)),
                "rel_step_bwd");
+  return KGE_OK;
+}
+
+int kge_pos_step_fwd(const kge_pos_step_args_t* a) {
+  if (!a) return fail(KGE_ERR_ARG, "kge_pos_step_fwd: bad argument");
+  DeviceScope device_scope(a->base.tb.ent0);   // before pos_step_ok, which may read offsets
+  if (!pos_step_ok(a)) return fail(KGE_ERR_ARG, "kge_pos_step_fwd: bad argument");
+  KGE_CUDA_TRY(kge::launch_margin_step_fwd(to_step(&a->base), static_cast<cudaStream_t>(a->base.stream),
+                                           to_pos_csr(a)),
+               "pos_step_fwd");
+  return KGE_OK;
+}
+
+int kge_pos_step_bwd(const kge_pos_step_args_t* a, const kge_grads_t* g, const float* grad_loss) {
+  if (!a || !step_grads_ok(&a->base, g) || !grad_loss || !shard_grads_ok(&a->base))
+    return fail(KGE_ERR_ARG, "kge_pos_step_bwd: bad argument");
+  DeviceScope device_scope(a->base.tb.ent0);   // before pos_step_ok, which may read offsets
+  if (!pos_step_ok(a)) return fail(KGE_ERR_ARG, "kge_pos_step_bwd: bad argument");
+  KGE_CUDA_TRY(kge::launch_margin_step_bwd(to_step(&a->base), to_grads(g), grad_loss,
+                                           static_cast<cudaStream_t>(a->base.stream), to_pos_csr(a)),
+               "pos_step_bwd");
   return KGE_OK;
 }
 

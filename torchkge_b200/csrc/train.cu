@@ -118,6 +118,41 @@ __device__ __forceinline__ void corrupt_one_rel(uint64_t seed, uint64_t offset, 
   *nr = kind == NEG_REL ? e : r;
 }
 
+// The positional draw (PositionalNegativeSampler, sampling.py:476-501).  Word x decides head vs tail exactly
+// as in draw_one.  Word y picks the replacement uniformly in the sorted candidate slice of relation r on that
+// side, ents[lo + ((y n) >> 32)] with n its length, or, when the slice is empty, uniformly on [0, n_ent):
+// unlike draw_one, entity 0 is drawn, as in the reference.  True triples are not rejected.  The draw depends
+// on (seed, offset, idx, r, the candidate slices) only, so every rank of a sharded step makes it too.
+// PosSlices holds relation r's two slices: every negative of a positive shares r, so its bounds are loaded
+// once per positive.
+struct PosSlices {
+  const int64_t* head_ents;   // first candidate of each side's slice
+  const int64_t* tail_ents;
+  long long n_head, n_tail;   // slice lengths
+};
+
+__device__ __forceinline__ PosSlices pos_slices(const PosCSR& pc, long long r) {
+  PosSlices s;
+  const long long h0 = pc.head_offs[r], t0 = pc.tail_offs[r];
+  s.n_head = pc.head_offs[r + 1] - h0;
+  s.n_tail = pc.tail_offs[r + 1] - t0;
+  s.head_ents = pc.head_ents + h0;   // an ents array may be NULL only when its slices are all empty
+  s.tail_ents = pc.tail_ents + t0;
+  return s;
+}
+
+__device__ __forceinline__ bool draw_pos(uint64_t seed, uint64_t offset, uint64_t idx, float p, long long n_ent,
+                                         const PosSlices& s, long long* e_out) {
+  const uint4 rnd = philox4x32(seed, offset, idx);
+  const float u = (rnd.x >> 8) * (1.0f / 16777216.0f);
+  const bool head = u < p;
+  const long long n = head ? s.n_head : s.n_tail;
+  const int64_t* ents = head ? s.head_ents : s.tail_ents;
+  const unsigned long long y = rnd.y;
+  *e_out = n > 0 ? (long long)ents[(y * (unsigned long long)n) >> 32] : (long long)((y * (unsigned long long)n_ent) >> 32);
+  return head;
+}
+
 // ------------------------------------------------------------------------------------------
 // Per-lane view of one triple.  Lane l owns embedding indices l, l+32, ...; `cnt` of them.
 // RowPtrs: the rows it is scored from.  GradRows: the destination rows of its gradient, plane by
@@ -444,6 +479,24 @@ __device__ __forceinline__ void step_negative(const MarginStepParams& a, long lo
   }
 }
 
+// The generic kernels' negative: the positional draw in a positional step (pc.head_offs set; ps: the
+// positive's slices), else step_negative.
+__device__ __forceinline__ void generic_negative(const MarginStepParams& a, const PosCSR& pc, const PosSlices& ps,
+                                                 long long idx, float p_head, long long hi, long long ti, long long ri,
+                                                 long long* nh, long long* nt, long long* nr) {
+  if (pc.head_offs) {
+    long long e;
+    const bool head = draw_pos(a.seed, a.offset, (uint64_t)idx, p_head, a.n_ent, ps, &e);
+    *nh = head ? e : hi; *nt = head ? ti : e; *nr = ri;
+  } else {
+    step_negative(a, idx, p_head, hi, ti, ri, nh, nt, nr);
+  }
+}
+
+__device__ __forceinline__ PosSlices generic_slices(const PosCSR& pc, long long r) {
+  return pc.head_offs ? pos_slices(pc, r) : PosSlices{nullptr, nullptr, 0, 0};
+}
+
 // ---- per-pair loss terms: the one statement of each loss, used by pair_loss_fwd / _bwd_kernel and
 // by every fused step (kind: KGE_LOSS_*, a runtime value or a template constant).
 //   margin  : max(0, margin - pos + neg)                    (MarginRankingLoss, target +1, sum)
@@ -485,7 +538,7 @@ __device__ __forceinline__ void pair_loss_grads(int kind, float margin, float g,
 // Fused step, forward: one warp per positive triple.
 //   loss += sum_j pair_loss_term(pos_i, neg_ij)
 // Negatives come from (nh, nt) if given, else from Philox; optionally written out.
-__global__ void margin_step_fwd_kernel(MarginStepParams a) {
+__global__ void margin_step_fwd_kernel(MarginStepParams a, PosCSR pc) {
   const long long w = ((long long)blockIdx.x * blockDim.x + threadIdx.x) >> 5;
   const int lane = threadIdx.x & 31;
   if (w >= a.b) return;
@@ -494,11 +547,12 @@ __global__ void margin_step_fwd_kernel(MarginStepParams a) {
   const float pos = triple_score(a.model, a.dim, pp, lane, nullptr, nullptr);
   if (lane == 0 && a.pos_out) a.pos_out[w] = pos;
   const float p_head = a.nh ? 0.f : a.probs[ri];
+  const PosSlices ps = generic_slices(pc, ri);
   float loss = 0.f;
   for (int j = 0; j < a.n_neg; ++j) {
     const long long idx = (long long)j * a.b + w;
     long long nh, nt, nr;
-    step_negative(a, idx, p_head, hi, ti, ri, &nh, &nt, &nr);
+    generic_negative(a, pc, ps, idx, p_head, hi, ti, ri, &nh, &nt, &nr);
     const RowPtrs pn = table_rows(a.model, a.dim, a.tb, nh, nt, nr);
     const float neg = triple_score(a.model, a.dim, pn, lane, nullptr, nullptr);
     if (lane == 0) {
@@ -514,7 +568,7 @@ __global__ void margin_step_fwd_kernel(MarginStepParams a) {
 // Fused step, backward: recompute the same negatives and scores; pair j sends g dl/dneg to the
 // negative triple, and the positive triple gets the sum over j of g dl/dpos in one call (the margin
 // loss: +g per active hinge to the negative, -g times the active count to the positive).
-__global__ void margin_step_bwd_kernel(MarginStepParams a, TrainGrads gr, const float* gloss) {
+__global__ void margin_step_bwd_kernel(MarginStepParams a, TrainGrads gr, const float* gloss, PosCSR pc) {
   const long long w = ((long long)blockIdx.x * blockDim.x + threadIdx.x) >> 5;
   const int lane = threadIdx.x & 31;
   if (w >= a.b) return;
@@ -523,11 +577,12 @@ __global__ void margin_step_bwd_kernel(MarginStepParams a, TrainGrads gr, const 
   const RowPtrs pp = table_rows(a.model, a.dim, a.tb, hi, ti, ri);
   const float pos = triple_score(a.model, a.dim, pp, lane, nullptr, nullptr);
   const float p_head = a.nh ? 0.f : a.probs[ri];
+  const PosSlices ps = generic_slices(pc, ri);
   double gpos_sum = 0.0;   // thousands of non-integer dl/dpos terms (logistic, BCE): fp32 would drift
   for (int j = 0; j < a.n_neg; ++j) {
     const long long idx = (long long)j * a.b + w;
     long long nh, nt, nr;
-    step_negative(a, idx, p_head, hi, ti, ri, &nh, &nt, &nr);
+    generic_negative(a, pc, ps, idx, p_head, hi, ti, ri, &nh, &nt, &nr);
     const RowPtrs pn = table_rows(a.model, a.dim, a.tb, nh, nt, nr);
     const float neg = triple_score(a.model, a.dim, pn, lane, nullptr, nullptr);
     float gp, gn;
@@ -557,10 +612,12 @@ __device__ __forceinline__ RowPtrs shard_pos_rows(const MarginStepParams& a, lon
                  rel_planes(a.model, a.dim, a.tb.rel0, a.tb.rel1, ri));
 }
 
-__device__ __forceinline__ bool owned_draw(const MarginStepParams& a, long long idx, float p_head,
-                                           bool* head, long long* loc) {
+// An entity negative (draw_one, or draw_pos in a positional step): owned by the rank holding the drawn entity.
+__device__ __forceinline__ bool owned_draw(const MarginStepParams& a, const PosCSR& pc, const PosSlices& ps,
+                                           long long idx, float p_head, bool* head, long long* loc) {
   long long e;
-  *head = draw_one(a.seed, a.offset, (uint64_t)idx, p_head, a.n_ent, &e);
+  *head = pc.head_offs ? draw_pos(a.seed, a.offset, (uint64_t)idx, p_head, a.n_ent, ps, &e)
+                      : draw_one(a.seed, a.offset, (uint64_t)idx, p_head, a.n_ent, &e);
   *loc = e - a.ent_lo;
   return (unsigned long long)*loc < (unsigned long long)a.n_rows;
 }
@@ -569,12 +626,13 @@ __device__ __forceinline__ bool owned_draw(const MarginStepParams& a, long long 
 // it, true with loc = the local row of its replaced entity.  A relation-corrupting negative (a.n_rel > 0)
 // is scored by the rank that holds the positive's head: its h / t rows are hrows / trows[w], so its
 // entity gradients land in grad_hrows / grad_trows, which the ranks sum like every other.
-__device__ __forceinline__ bool owned_negative(const MarginStepParams& a, long long w, long long idx, float p_head,
-                                               long long ri, int* kind, long long* loc, long long* nr) {
+__device__ __forceinline__ bool owned_negative(const MarginStepParams& a, const PosCSR& pc, const PosSlices& ps,
+                                               long long w, long long idx, float p_head, long long ri, int* kind,
+                                               long long* loc, long long* nr) {
   *nr = ri;
   if (a.n_rel == 0) {
     bool head;
-    const bool own = owned_draw(a, idx, p_head, &head, loc);
+    const bool own = owned_draw(a, pc, ps, idx, p_head, &head, loc);
     *kind = head ? NEG_HEAD : NEG_TAIL;
     return own;
   }
@@ -590,18 +648,19 @@ __device__ __forceinline__ RowPtrs shard_kind_rows(const MarginStepParams& a, lo
   return kind == NEG_REL ? shard_pos_rows(a, w, nr) : shard_neg_rows(a, w, nr, kind == NEG_HEAD, loc);
 }
 
-__global__ void margin_step_shard_fwd_kernel(MarginStepParams a) {
+__global__ void margin_step_shard_fwd_kernel(MarginStepParams a, PosCSR pc) {
   const long long w = ((long long)blockIdx.x * blockDim.x + threadIdx.x) >> 5;
   const int lane = threadIdx.x & 31;
   if (w >= a.b) return;
   const long long ri = a.r[w];
   const float pos = triple_score(a.model, a.dim, shard_pos_rows(a, w, ri), lane, nullptr, nullptr);
   const float p_head = a.probs[ri];
+  const PosSlices ps = generic_slices(pc, ri);
   float loss = 0.f;
   for (int j = 0; j < a.n_neg; ++j) {
     int kind;
     long long loc, nr;
-    if (!owned_negative(a, w, (long long)j * a.b + w, p_head, ri, &kind, &loc, &nr)) continue;
+    if (!owned_negative(a, pc, ps, w, (long long)j * a.b + w, p_head, ri, &kind, &loc, &nr)) continue;
     const float neg = triple_score(a.model, a.dim, shard_kind_rows(a, w, nr, kind, loc), lane, nullptr, nullptr);
     if (lane == 0) loss += pair_loss_term(a.loss_kind, a.margin, pos, neg);
   }
@@ -612,7 +671,7 @@ __global__ void margin_step_shard_fwd_kernel(MarginStepParams a) {
 // it), the intact entity's and the positive's to grad_hrows / grad_trows[w], the relation's to the
 // local copy of the relation gradient; the caller sums the last three over the ranks.  The positive's
 // term is summed over the negatives this rank owns only, so the ranks' sums make up the whole.
-__global__ void margin_step_shard_bwd_kernel(MarginStepParams a, TrainGrads gr, const float* gloss) {
+__global__ void margin_step_shard_bwd_kernel(MarginStepParams a, TrainGrads gr, const float* gloss, PosCSR pc) {
   const long long w = ((long long)blockIdx.x * blockDim.x + threadIdx.x) >> 5;
   const int lane = threadIdx.x & 31;
   if (w >= a.b) return;
@@ -621,6 +680,7 @@ __global__ void margin_step_shard_bwd_kernel(MarginStepParams a, TrainGrads gr, 
   const RowPtrs pp = shard_pos_rows(a, w, ri);
   const float pos = triple_score(a.model, a.dim, pp, lane, nullptr, nullptr);
   const float p_head = a.probs[ri];
+  const PosSlices ps = generic_slices(pc, ri);
   const int np = ent_planes(a.model);
   const Planes<float> gh = buf_planes(a.grad_hrows, np, a.dim, w);
   const Planes<float> gt = buf_planes(a.grad_trows, np, a.dim, w);
@@ -629,7 +689,7 @@ __global__ void margin_step_shard_bwd_kernel(MarginStepParams a, TrainGrads gr, 
   for (int j = 0; j < a.n_neg; ++j) {
     int kind;
     long long loc, nr;
-    if (!owned_negative(a, w, (long long)j * a.b + w, p_head, ri, &kind, &loc, &nr)) continue;
+    if (!owned_negative(a, pc, ps, w, (long long)j * a.b + w, p_head, ri, &kind, &loc, &nr)) continue;
     const RowPtrs pn = shard_kind_rows(a, w, nr, kind, loc);
     const float neg = triple_score(a.model, a.dim, pn, lane, nullptr, nullptr);
     float gp, gn;
@@ -1173,10 +1233,13 @@ __device__ __forceinline__ Vec vec_load_smem(const float* row, int dim, int lane
 // REL: the relation-corrupting step (a.n_rel > 0, margin_step_ring_rel_kernel).  A relation negative's
 // code carries CODE_REL and its relation; its row streams through the same ring from the relation table.
 // SHARD: the rank holding the positive's head scores it.  Codes then hold 30-bit row numbers.
+// POS: the positional step (pc, margin_step_ring_pos_kernel): entity negatives from draw_pos,
+// whose two candidate slices the warp loads once, since all its negatives share the positive's relation.
 constexpr unsigned CODE_REL = 0x40000000u;
 
-template <int MODEL, bool BWD, bool SHARD, int LOSS, bool REL>
-__device__ __forceinline__ void ring_step(const MarginStepParams& a, const TrainGrads& gr, const float* gloss) {
+template <int MODEL, bool BWD, bool SHARD, int LOSS, bool REL, bool POS = false>
+__device__ __forceinline__ void ring_step(const MarginStepParams& a, const TrainGrads& gr, const float* gloss,
+                                          const PosCSR& pc = PosCSR{}) {
   extern __shared__ __align__(128) unsigned char ring_smem[];
   const int warp_in_block = threadIdx.x >> 5, lane = threadIdx.x & 31;
   const long long w = (long long)blockIdx.x * WARPS_PER_BLOCK + warp_in_block;
@@ -1198,6 +1261,8 @@ __device__ __forceinline__ void ring_step(const MarginStepParams& a, const Train
   const long long hi = a.h[w], ti = a.t[w], ri = a.r[w];
   const float p_head = a.nh ? 0.f : a.probs[ri];
   constexpr unsigned ROW_MASK = REL ? 0x3FFFFFFFu : 0x7FFFFFFFu;
+  PosSlices ps;
+  if constexpr (POS) ps = pos_slices(pc, ri);
   // ---- all corruptions of this positive, up front: code = entity | head flag (REL: or relation | CODE_REL) ----
   int n_loop = a.n_neg;            // SHARD: the owned negatives, compacted to the front of `codes`
   if constexpr (SHARD) {
@@ -1221,7 +1286,9 @@ __device__ __forceinline__ void ring_step(const MarginStepParams& a, const Train
             code = (unsigned)loc | (kind == NEG_HEAD ? 0x80000000u : 0u);
           }
         } else {
-          const bool head = draw_one(a.seed, a.offset, idx, p_head, a.n_ent, &e);
+          bool head;
+          if constexpr (POS) head = draw_pos(a.seed, a.offset, idx, p_head, a.n_ent, ps, &e);
+          else head = draw_one(a.seed, a.offset, idx, p_head, a.n_ent, &e);
           const unsigned long long loc = (unsigned long long)(e - a.ent_lo);
           own = loc < (unsigned long long)a.n_rows;      // n_rows < 2^31 (ring_step_ok)
           code = (unsigned)loc | (head ? 0x80000000u : 0u);
@@ -1247,6 +1314,11 @@ __device__ __forceinline__ void ring_step(const MarginStepParams& a, const Train
           codes[j] = changed > 1 ? CODE_BOTH
                      : nr != ri ? ((unsigned)nr | CODE_REL)
                                 : ((unsigned)(head ? nh : nt) | (head ? 0x80000000u : 0u));
+        } else if constexpr (POS) {   // no caller negatives (kge_pos_step_*): one end is replaced
+          long long e;
+          const bool head = draw_pos(a.seed, a.offset, (uint64_t)idx, p_head, a.n_ent, ps, &e);
+          if (!BWD && a.nh_out) { a.nh_out[idx] = head ? e : hi; a.nt_out[idx] = head ? ti : e; }
+          codes[j] = (unsigned)e | (head ? 0x80000000u : 0u);
         } else {
           if (a.nh) { nh = a.nh[idx]; nt = a.nt[idx]; }
           else corrupt_one(a.seed, a.offset, (uint64_t)idx, p_head, a.n_ent, hi, ti, &nh, &nt);
@@ -1336,6 +1408,12 @@ margin_step_ring_rel_kernel(MarginStepParams a, TrainGrads gr, const float* __re
   ring_step<MODEL, BWD, SHARD, LOSS, true>(a, gr, gloss);
 }
 
+template <int MODEL, bool BWD, bool SHARD, int LOSS>
+__global__ void __launch_bounds__(WARPS_PER_BLOCK * 32, 1)
+margin_step_ring_pos_kernel(MarginStepParams a, TrainGrads gr, const float* __restrict__ gloss, PosCSR pc) {
+  ring_step<MODEL, BWD, SHARD, LOSS, false, true>(a, gr, gloss, pc);
+}
+
 __host__ inline size_t ring_smem_bytes(const MarginStepParams& a) {
   const size_t per_warp = (size_t)RING * a.dim * 4 + (size_t)((a.n_neg + 3) & ~3) * 4 + RING * sizeof(uint64_t);
   return WARPS_PER_BLOCK * ((per_warp + 127) & ~(size_t)127);
@@ -1350,28 +1428,41 @@ __host__ inline bool ring_step_ok(const MarginStepParams& a) {
   return enabled && a.n_neg <= 8192 && rows < row_limit && a.n_rel < 0x3FFFFFFFll && ring_smem_bytes(a) <= 96 * 1024;
 }
 
-// REL: margin_step_ring_rel_kernel (MINB is 0 there)
-template <int MODEL, bool BWD, int MINB, bool SHARD = false, int LOSS = KGE_LOSS_MARGIN, bool REL = false>
-cudaError_t launch_ring_variant(const MarginStepParams& a, const TrainGrads& gr, const float* gloss, cudaStream_t st) {
-  constexpr void (*kernel)(MarginStepParams, TrainGrads, const float*) =
-      REL ? margin_step_ring_rel_kernel<MODEL, BWD, SHARD, LOSS> : margin_step_ring_kernel<MODEL, BWD, MINB, SHARD, LOSS>;
+// REL: margin_step_ring_rel_kernel, POS: margin_step_ring_pos_kernel, which also takes the CSR (MINB is 0 there)
+template <int MODEL, bool BWD, int MINB, bool SHARD, int LOSS, bool REL, bool POS>
+constexpr auto ring_kernel() {
+  if constexpr (POS) return margin_step_ring_pos_kernel<MODEL, BWD, SHARD, LOSS>;
+  else if constexpr (REL) return margin_step_ring_rel_kernel<MODEL, BWD, SHARD, LOSS>;
+  else return margin_step_ring_kernel<MODEL, BWD, MINB, SHARD, LOSS>;
+}
+
+template <int MODEL, bool BWD, int MINB, bool SHARD = false, int LOSS = KGE_LOSS_MARGIN, bool REL = false,
+          bool POS = false>
+cudaError_t launch_ring_variant(const MarginStepParams& a, const TrainGrads& gr, const float* gloss, cudaStream_t st,
+                                const PosCSR& pc = PosCSR{}) {
+  constexpr auto kernel = ring_kernel<MODEL, BWD, MINB, SHARD, LOSS, REL, POS>();
   const size_t smem = ring_smem_bytes(a);
   if (smem > 48 * 1024) {
     const cudaError_t e = set_attribute_once<kernel>(cudaFuncAttributeMaxDynamicSharedMemorySize, 96 * 1024);
     if (e != cudaSuccess) return e;
   }
   const unsigned blocks = (unsigned)((a.b + WARPS_PER_BLOCK - 1) / WARPS_PER_BLOCK);
-  kernel<<<blocks, WARPS_PER_BLOCK * 32, smem, st>>>(a, gr, gloss);
+  if constexpr (POS) kernel<<<blocks, WARPS_PER_BLOCK * 32, smem, st>>>(a, gr, gloss, pc);
+  else kernel<<<blocks, WARPS_PER_BLOCK * 32, smem, st>>>(a, gr, gloss);
   return cudaGetLastError();
 }
 
-// One ring kernel per (relation or entity step, loss kind, sharded).  KGE_TRAIN_BWD_BLOCKS=5 holds the
+// One ring kernel per (entity, relation or positional step, loss kind, sharded).  KGE_TRAIN_BWD_BLOCKS=5 holds the
 // backward kernel to 96 registers (5 CTAs = 20 warps per SM; the unsharded entity step with the margin
 // loss only).
 template <int MODEL, bool BWD>
-cudaError_t launch_ring(const MarginStepParams& a, const TrainGrads& gr, const float* gloss, cudaStream_t st) {
+cudaError_t launch_ring(const MarginStepParams& a, const TrainGrads& gr, const float* gloss, cudaStream_t st,
+                        const PosCSR& pc) {
   auto by_shard = [&](auto loss) -> cudaError_t {
     constexpr int LOSS = decltype(loss)::value;
+    if (pc.head_offs)
+      return a.hrows ? launch_ring_variant<MODEL, BWD, 0, true, LOSS, false, true>(a, gr, gloss, st, pc)
+                     : launch_ring_variant<MODEL, BWD, 0, false, LOSS, false, true>(a, gr, gloss, st, pc);
     if (a.n_rel > 0)
       return a.hrows ? launch_ring_variant<MODEL, BWD, 0, true, LOSS, true>(a, gr, gloss, st)
                      : launch_ring_variant<MODEL, BWD, 0, false, LOSS, true>(a, gr, gloss, st);
@@ -1510,15 +1601,20 @@ cudaError_t with_fast_model(int model, F&& f) {
 // L2 and DistMult take the ring kernel's relation kind (margin_step_ring_rel_kernel) where the ring
 // applies; everything else, and KGE_TRAIN_RING=0, takes the generic kernels, which score a negative from
 // its own (nh, nt, nr).
+//
+// A positional step (pc.head_offs set, n_rel 0): the ring kernel's positional kind
+// (margin_step_ring_pos_kernel) where the ring applies, else the generic kernels -- never the register-resident
+// form, as for the relation step.
 template <bool BWD>
-cudaError_t launch_margin_step(MarginStepParams a, const TrainGrads& gr, const float* gloss, cudaStream_t st) {
+cudaError_t launch_margin_step(MarginStepParams a, const TrainGrads& gr, const float* gloss, cudaStream_t st,
+                               const PosCSR& pc) {
   if (a.n_rel > 0 && a.rel_share >= 1.f && !a.nh && !a.nr_out) a.n_rel = 0;
   const bool shard = a.hrows != nullptr;
   if (a.b <= 0 || (shard && a.n_rows <= 0)) return cudaSuccess;
   const unsigned blocks = blocks_for_warps(a.b);
   if (fast_step_ok(a) && ring_step_ok(a))
-    return with_fast_model(a.model, [&](auto m) { return launch_ring<decltype(m)::value, BWD>(a, gr, gloss, st); });
-  if (a.n_rel <= 0) {   // the register-resident form has no relation kind
+    return with_fast_model(a.model, [&](auto m) { return launch_ring<decltype(m)::value, BWD>(a, gr, gloss, st, pc); });
+  if (a.n_rel <= 0 && !pc.head_offs) {   // the register-resident form has no relation or positional kind
     if (!shard && fast_step_ok(a) && a.loss_kind == KGE_LOSS_MARGIN) {
       return with_fast_model(a.model, [&](auto m) {
         margin_step_fast_kernel<decltype(m)::value, BWD><<<blocks, WARPS_PER_BLOCK * 32, 0, st>>>(a, gr, gloss);
@@ -1527,23 +1623,23 @@ cudaError_t launch_margin_step(MarginStepParams a, const TrainGrads& gr, const f
     }
   }
   if constexpr (BWD) {
-    if (shard) margin_step_shard_bwd_kernel<<<blocks, WARPS_PER_BLOCK * 32, 0, st>>>(a, gr, gloss);
-    else margin_step_bwd_kernel<<<blocks, WARPS_PER_BLOCK * 32, 0, st>>>(a, gr, gloss);
+    if (shard) margin_step_shard_bwd_kernel<<<blocks, WARPS_PER_BLOCK * 32, 0, st>>>(a, gr, gloss, pc);
+    else margin_step_bwd_kernel<<<blocks, WARPS_PER_BLOCK * 32, 0, st>>>(a, gr, gloss, pc);
   } else {
-    if (shard) margin_step_shard_fwd_kernel<<<blocks, WARPS_PER_BLOCK * 32, 0, st>>>(a);
-    else margin_step_fwd_kernel<<<blocks, WARPS_PER_BLOCK * 32, 0, st>>>(a);
+    if (shard) margin_step_shard_fwd_kernel<<<blocks, WARPS_PER_BLOCK * 32, 0, st>>>(a, pc);
+    else margin_step_fwd_kernel<<<blocks, WARPS_PER_BLOCK * 32, 0, st>>>(a, pc);
   }
   return cudaGetLastError();
 }
 }  // namespace
 
-cudaError_t launch_margin_step_fwd(const MarginStepParams& a, cudaStream_t st) {
-  return launch_margin_step<false>(a, TrainGrads{nullptr, nullptr, nullptr, nullptr}, nullptr, st);
+cudaError_t launch_margin_step_fwd(const MarginStepParams& a, cudaStream_t st, const PosCSR& pos) {
+  return launch_margin_step<false>(a, TrainGrads{nullptr, nullptr, nullptr, nullptr}, nullptr, st, pos);
 }
 
 cudaError_t launch_margin_step_bwd(const MarginStepParams& a, const TrainGrads& gr, const float* gloss,
-                                   cudaStream_t st) {
-  return launch_margin_step<true>(a, gr, gloss, st);
+                                   cudaStream_t st, const PosCSR& pos) {
+  return launch_margin_step<true>(a, gr, gloss, st, pos);
 }
 
 cudaError_t launch_pair_loss_fwd(int kind, float margin, const float* pos, const float* neg, int64_t n,

@@ -59,6 +59,18 @@ struct MarginStepParams {
   int64_t* nr_out;
 };
 
+// Positional step (head_offs != nullptr, PositionalNegativeSampler): the replacement of a negative of
+// relation r comes from the sorted slice [offs[r], offs[r + 1]) of ents on its side (draw_pos), or is uniform
+// on [0, n_ent) when that slice is empty.  All nullptr: the entity or relation step.  A kernel parameter of its
+// own, after the others, so that MarginStepParams -- and the code of the kernels that never draw positionally --
+// stay as they are.
+struct PosCSR {
+  const int64_t* head_offs;
+  const int64_t* head_ents;
+  const int64_t* tail_offs;
+  const int64_t* tail_ents;
+};
+
 cudaError_t launch_score_triples_fwd(int model, int dim, const TrainTables& tb, const int64_t* h,
                                      const int64_t* t, const int64_t* r, int64_t n, float* out,
                                      cudaStream_t st);
@@ -73,9 +85,10 @@ cudaError_t launch_corrupt_batch_rel(const int64_t* h, const int64_t* t, const i
                                      int n_neg, const float* probs, int64_t n_ent, int64_t n_rel, float rel_share,
                                      uint64_t seed, uint64_t offset, int64_t* nh, int64_t* nt, int64_t* nr,
                                      cudaStream_t st);
-cudaError_t launch_margin_step_fwd(const MarginStepParams& a, cudaStream_t st);
+// pos: the positional step's candidates (PosCSR{} for the entity and relation steps)
+cudaError_t launch_margin_step_fwd(const MarginStepParams& a, cudaStream_t st, const PosCSR& pos = PosCSR{});
 cudaError_t launch_margin_step_bwd(const MarginStepParams& a, const TrainGrads& gr, const float* gloss,
-                                   cudaStream_t st);
+                                   cudaStream_t st, const PosCSR& pos = PosCSR{});
 cudaError_t launch_scatter_rows_add(float* grad0, float* grad1, int planes, int64_t ent_lo, int64_t n_rows,
                                     int dim, const int64_t* idx, int64_t n, const float* rows, cudaStream_t st);
 // MarginLoss / LogisticLoss / BinaryCrossEntropyLoss on score arrays (kind: KGE_LOSS_*; margin is used by

@@ -465,6 +465,12 @@ class CudaEngine:
         a.ent_lo, a.n_rows = step.ent_lo, step.n_rows
         a.hrows, a.trows = _ptr(hrows), _ptr(trows)
         a.loss_kind = step.loss_kind
+        pos = getattr(step, "pos", None)
+        if pos is not None:                # positional step: kge_pos_step_* around the same arguments
+            pa = _lib.PosStepArgs()
+            pa.base, pa.n_rel = a, pos[0].shape[0] - 1
+            pa.head_offs, pa.head_ents, pa.tail_offs, pa.tail_ents = (_ptr(x) for x in pos)
+            return pa
         if getattr(step, "n_rel", 0) == 0:
             return a
         ra = _lib.RelStepArgs()           # relation-corrupting step: kge_rel_step_* around the same arguments
@@ -472,7 +478,8 @@ class CudaEngine:
         return ra
 
     def _step_call(self, a, which, *rest):
-        name = ("kge_rel_step_" if isinstance(a, _lib.RelStepArgs) else "kge_margin_step_") + which
+        name = {_lib.RelStepArgs: "kge_rel_step_", _lib.PosStepArgs: "kge_pos_step_"}.get(
+            type(a), "kge_margin_step_") + which
         _lib.check(getattr(self.lib, name)(ctypes.byref(a), *rest), name)
 
     def margin_step_fwd(self, step, tables, h, t, r, probs, hrows, trows):
@@ -482,7 +489,8 @@ class CudaEngine:
         (ent0, ent1, rel0, rel1) with this shard's entity rows (a three-plane table as one stacked
         (3, n, dim) tensor in ent0 / rel0); hrows / trows: (b, planes, dim) rows of every positive.
         step.n_rel > 0: the relation-corrupting step (kge_rel_step_fwd), whose relation negatives this shard
-        scores when it holds the positive's head."""
+        scores when it holds the positive's head.  step.pos = (head_offs, head_ents, tail_offs, tail_ents): the
+        positional step (kge_pos_step_fwd), drawn from those candidate slices."""
         loss = torch.zeros((), dtype=torch.float32, device=h.device)
         a = self._shard_step_args(step, tables, h, t, r, probs, loss, hrows, trows)
         self._step_call(a, "fwd")
@@ -494,7 +502,7 @@ class CudaEngine:
         and grad_hrows / grad_trows (b, planes, dim)."""
         dummy = torch.zeros((), dtype=torch.float32, device=h.device)   # the loss is not recomputed
         a = self._shard_step_args(step, tables, h, t, r, probs, dummy, hrows, trows)
-        base = a.base if isinstance(a, _lib.RelStepArgs) else a
+        base = a if isinstance(a, _lib.MarginStepArgs) else a.base
         base.grad_hrows, base.grad_trows = _ptr(grad_hrows), _ptr(grad_trows)
         g = _lib.Grads()
         g.ent0, g.ent1 = _plane_ptrs(grads[0], grads[1])

@@ -62,13 +62,15 @@ class UniformNegativeSampler(NegativeSampler):
     """Uniform negative sampler (Bordes et al. 2013), torchkge/sampling.py:141-223: head or tail
     with probability 1/2 each, replacement uniform on [1, n_ent) (entity 0 is never drawn, true
     triples are not rejected -- as in the reference).  Same counter-based generator as
-    ``BernoulliNegativeSampler``; ``seed`` is an extension."""
+    ``BernoulliNegativeSampler``; ``seed`` is an extension.  ``fused_step`` is the fused training step of
+    ``BernoulliNegativeSampler`` with every head probability 1/2."""
 
     def __init__(self, kg, kg_val=None, kg_test=None, n_neg=1, seed=None):
         super().__init__(kg, kg_val, kg_test, n_neg)
         self.seed = int(torch.initial_seed() if seed is None else seed) & 0xFFFFFFFFFFFFFFFF
         self._calls = 0
         self._half = None
+        self._halves = None     # (n_rel,) of 1/2 on one device: fused_step's head probabilities
 
     def corrupt_batch(self, heads, tails, relations=None, n_neg=None):
         if n_neg is None:
@@ -89,6 +91,23 @@ class UniformNegativeSampler(NegativeSampler):
                                                  self.n_ent, self.seed, self._calls, _ptr(nh), _ptr(nt),
                                                  _stream(dev)), "kge_corrupt_batch")
         return nh, nt
+
+    def _next_offset(self):
+        self._calls += 1
+        return self._calls
+
+    def fused_step(self, model, heads, tails, relations, margin=None, n_neg=None, *, criterion=None,
+                   shard=None):
+        """Extension: corruption + ``model(...)`` + the loss in ONE kernel; returns the differentiable scalar
+        loss.  Arguments and errors as in ``BernoulliNegativeSampler.fused_step``.  Draws, bit for bit, the
+        negatives ``corrupt_batch`` would draw at the same call count: the Bernoulli step with every
+        probability 1/2."""
+        n = max(int(self.kg.n_rel), int(getattr(model, "n_rel", 0)))   # every relation id the batch may hold
+        dev = heads.device
+        if self._halves is None or self._halves.device != dev or self._halves.shape[0] != n:
+            self._halves = torch.full((n,), 0.5, dtype=torch.float32, device=dev)
+        return _sampler_fused_step(self, model, heads, tails, relations, margin, n_neg, criterion, shard,
+                                   self._halves)
 
 
 class BernoulliNegativeSampler(NegativeSampler):
@@ -146,12 +165,16 @@ class BernoulliNegativeSampler(NegativeSampler):
         shard: ``EntityShard(local_storage=True)`` for a model holding only its entity rows (see
         ``training.fused_margin_step``); every rank uses a sampler with the same seed and call count,
         built on the whole graph, and passes the same batch."""
-        return _sampler_fused_step(self, model, heads, tails, relations, margin, n_neg, criterion, shard)
+        self.bern_probs = self.bern_probs.to(heads.device)
+        return _sampler_fused_step(self, model, heads, tails, relations, margin, n_neg, criterion, shard,
+                                   self.bern_probs)
 
 
-def _sampler_fused_step(sampler, model, heads, tails, relations, margin, n_neg, criterion, shard, rel_share=None):
-    """fused_step of the Bernoulli samplers: their argument checks, then the fused step at the sampler's
-    next call count (rel_share: the relation-corrupting step)."""
+def _sampler_fused_step(sampler, model, heads, tails, relations, margin, n_neg, criterion, shard, probs,
+                        rel_share=None, positional=None):
+    """fused_step of the samplers: their argument checks, then the fused step at the sampler's next call count
+    with head probabilities ``probs`` (rel_share: the relation-corrupting step; positional: the positional
+    step's CSR)."""
     if (margin is None) == (criterion is None):
         raise ValueError("fused_step takes exactly one of margin and criterion")
     if criterion is not None:
@@ -161,14 +184,16 @@ def _sampler_fused_step(sampler, model, heads, tails, relations, margin, n_neg, 
     if shard is not None and getattr(shard, "n_ent", sampler.n_ent) != sampler.n_ent:
         raise ValueError("the sampler draws on %d entities, the shard partitions %d"
                          % (sampler.n_ent, shard.n_ent))
-    sampler.bern_probs = sampler.bern_probs.to(heads.device)
+    if positional is not None and shard is None and int(model.n_ent) != sampler.n_ent:
+        # the kernel indexes the model's table with the sampler's entity ids
+        raise ValueError("the sampler draws on %d entities, the model has %d" % (sampler.n_ent, model.n_ent))
     if criterion is not None:
-        return fused_loss_step(model, heads, tails, relations, criterion, n_neg=n_neg,
-                               bern_probs=sampler.bern_probs, seed=sampler.seed,
-                               offset=sampler._next_offset(), shard=shard, rel_share=rel_share)
-    return fused_margin_step(model, heads, tails, relations, margin, n_neg=n_neg,
-                             bern_probs=sampler.bern_probs, seed=sampler.seed,
-                             offset=sampler._next_offset(), shard=shard, rel_share=rel_share)
+        return fused_loss_step(model, heads, tails, relations, criterion, n_neg=n_neg, bern_probs=probs,
+                               seed=sampler.seed, offset=sampler._next_offset(), shard=shard,
+                               rel_share=rel_share, positional=positional)
+    return fused_margin_step(model, heads, tails, relations, margin, n_neg=n_neg, bern_probs=probs,
+                             seed=sampler.seed, offset=sampler._next_offset(), shard=shard, rel_share=rel_share,
+                             positional=positional)
 
 
 class BernoulliRelationNegativeSampler(NegativeSampler):
@@ -249,8 +274,9 @@ class BernoulliRelationNegativeSampler(NegativeSampler):
         n_neg (extension) >= 1 negatives per fact, drawn as n_neg blocks of the batch; block 0 is exactly
         what ``corrupt_batch`` draws at the same call count.  With ``shard``, the rank holding a positive's
         head scores its relation negatives."""
+        self.bern_probs = self.bern_probs.to(heads.device)
         return _sampler_fused_step(self, model, heads, tails, relations, margin, n_neg, criterion, shard,
-                                   rel_share=self.rel_share)
+                                   self.bern_probs, rel_share=self.rel_share)
 
 
 class PositionalNegativeSampler(BernoulliNegativeSampler):
@@ -262,6 +288,10 @@ class PositionalNegativeSampler(BernoulliNegativeSampler):
     The reference walks Python lists fact by fact (sampling.py:476-501); here the candidate sets are
     two CSR arrays on the device and a batch is three gathers.  Draws come from a ``torch.Generator``
     on the batch's device (seeded by ``seed``): same law as the reference, not the same stream.
+
+    ``fused_step`` (extension) draws the same law inside the fused training step, from the counter-based
+    generator of ``BernoulliNegativeSampler`` keyed by ``seed`` -- so not the stream ``corrupt_batch`` draws,
+    whose ``torch.Generator`` (and with it ``TripletClassificationEvaluator``'s default negatives) is unchanged.
 
     Attributes: ``possible_heads`` / ``possible_tails`` (dict relation -> sorted list),
     ``n_poss_heads`` / ``n_poss_tails`` (LongTensor (n_rel,)), as in the reference.
@@ -327,3 +357,21 @@ class PositionalNegativeSampler(BernoulliNegativeSampler):
             drawn = torch.where(n_poss > 0, drawn, any_ent)
             out.append(torch.where(mask, drawn, orig))
         return out[0], out[1]
+
+    def fused_step(self, model, heads, tails, relations, margin=None, n_neg=None, *, criterion=None,
+                   shard=None):
+        """Extension: positional corruption + ``model(...)`` + the loss in ONE kernel; returns the differentiable
+        scalar loss.  Arguments and errors as in ``BernoulliNegativeSampler.fused_step``; the model must have the
+        sampler's ``n_ent`` entities (with ``shard``: the shard must partition them).
+
+        Each negative replaces the head with probability ``bern_probs[r]``, else the tail, by an entity drawn
+        uniformly from ``possible_heads[r]`` / ``possible_tails[r]``, or from [0, n_ent) when that list is empty,
+        as in ``corrupt_batch`` -- the same law, drawn by the counter-based generator at the sampler's next call
+        count rather than from ``corrupt_batch``'s stream.  n_neg (extension) >= 1 negatives per fact, as n_neg
+        blocks of the batch.  With ``shard`` every rank holds the whole candidate CSR; the rank holding the
+        drawn entity scores a negative."""
+        csr, _ = self._on(heads.device)
+        positional = (csr["heads"][0], csr["heads"][1], csr["tails"][0], csr["tails"][1])
+        self.bern_probs = self.bern_probs.to(heads.device)
+        return _sampler_fused_step(self, model, heads, tails, relations, margin, n_neg, criterion, shard,
+                                   self.bern_probs, positional=positional)

@@ -211,9 +211,10 @@ class _MarginStep(torch.autograd.Function):
 
     @staticmethod
     def forward(ctx, code, dim, n_ent, margin, n_neg, h, t, r, nh, nt, probs, seed, offset,
-                ent0, ent1, rel0, rel1, loss_kind=_lib.LOSS_MARGIN, nr=None, rel=None):
+                ent0, ent1, rel0, rel1, loss_kind=_lib.LOSS_MARGIN, nr=None, rel=None, pos=None):
         # rel: (n_rel, rel_share) for a relation-corrupting step (kge_rel_step_*; external negatives then
         # come with nr), None for the entity step (kge_margin_step_*)
+        # pos: (head_offs, head_ents, tail_offs, tail_ents) for a positional step (kge_pos_step_*)
         tensors = [None if x is None else x.detach().contiguous() for x in (ent0, ent1, rel0, rel1)]
         _check_cuda(tensors[0], h, t, r)
         dev = tensors[0].device
@@ -224,25 +225,33 @@ class _MarginStep(torch.autograd.Function):
             nr = _idx(nr, dev)
         if probs is not None:
             probs = probs.to(device=dev, dtype=torch.float32).contiguous()
+        if pos is not None:
+            pos = tuple(_idx(x, dev) for x in pos)
         loss = torch.zeros((), dtype=torch.float32, device=dev)
         a = _MarginStep._args(code, dim, n_ent, margin, n_neg, h, t, r, nh, nt, probs, seed, offset,
-                              tensors, loss, dev, loss_kind, nr, rel)
-        if rel is None:
-            _lib.check(_lib.load().kge_margin_step_fwd(ctypes.byref(a)), "kge_margin_step_fwd")
-        else:
-            _lib.check(_lib.load().kge_rel_step_fwd(ctypes.byref(a)), "kge_rel_step_fwd")
+                              tensors, loss, dev, loss_kind, nr, rel, pos)
+        name = _MarginStep._entry(a, "fwd")
+        _lib.check(getattr(_lib.load(), name)(ctypes.byref(a)), name)
         ctx.meta = (code, dim, n_ent, margin, n_neg, seed, offset, loss_kind, rel)
         ctx.present = [x is not None for x in tensors]
         ctx.has_neg, ctx.has_nr, ctx.has_probs = nh is not None, nr is not None, probs is not None
+        ctx.has_pos = pos is not None
         extra = (([nh, nt] if nh is not None else []) + ([nr] if nr is not None else []) +
-                 ([probs] if probs is not None else []))
+                 ([probs] if probs is not None else []) + (list(pos) if pos is not None else []))
         ctx.save_for_backward(h, t, r, *extra, *[x for x in tensors if x is not None])
         return loss
 
     @staticmethod
+    def _entry(a, which):
+        """The entry point for ``a``: kge_margin_step_<which>, kge_rel_step_<which> or kge_pos_step_<which>."""
+        return {_lib.RelStepArgs: "kge_rel_step_", _lib.PosStepArgs: "kge_pos_step_"}.get(
+            type(a), "kge_margin_step_") + which
+
+    @staticmethod
     def _args(code, dim, n_ent, margin, n_neg, h, t, r, nh, nt, probs, seed, offset, tensors, loss, dev,
-              loss_kind=_lib.LOSS_MARGIN, nr=None, rel=None):
-        """kge_margin_step_args_t, or with rel = (n_rel, rel_share) kge_rel_step_args_t around it."""
+              loss_kind=_lib.LOSS_MARGIN, nr=None, rel=None, pos=None):
+        """kge_margin_step_args_t, or with rel = (n_rel, rel_share) kge_rel_step_args_t around it, or with
+        pos = (head_offs, head_ents, tail_offs, tail_ents) kge_pos_step_args_t around it."""
         a = _lib.MarginStepArgs()
         a.tb = _tables(code, dim, tensors)
         a.n_neg, a.margin, a.b, a.n_ent = n_neg, float(margin), h.shape[0], n_ent
@@ -250,6 +259,11 @@ class _MarginStep(torch.autograd.Function):
         a.seed, a.offset = int(seed), int(offset)
         a.loss, a.stream = _ptr(loss), _stream(dev)
         a.loss_kind = int(loss_kind)
+        if pos is not None:
+            pa = _lib.PosStepArgs()
+            pa.base, pa.n_rel = a, int(pos[0].shape[0]) - 1
+            pa.head_offs, pa.head_ents, pa.tail_offs, pa.tail_ents = (_ptr(x) for x in pos)
+            return pa
         if rel is None:
             return a
         ra = _lib.RelStepArgs()
@@ -273,29 +287,30 @@ class _MarginStep(torch.autograd.Function):
         if ctx.has_probs:
             probs = saved[k]
             k += 1
+        pos = None
+        if ctx.has_pos:
+            pos = tuple(saved[k:k + 4])
+            k += 4
         it = iter(saved[k:])
         tensors = [next(it) if p else None for p in ctx.present]
         dev = h.device
         gl = gl.contiguous().float()
         dummy = torch.zeros((), dtype=torch.float32, device=dev)
         a = _MarginStep._args(code, dim, n_ent, margin, n_neg, h, t, r, nh, nt, probs, seed, offset,
-                              tensors, dummy, dev, loss_kind, nr, rel)
+                              tensors, dummy, dev, loss_kind, nr, rel, pos)
         gs, g = _zero_grads(tensors)
-        if rel is None:
-            _lib.check(_lib.load().kge_margin_step_bwd(ctypes.byref(a), ctypes.byref(g), _ptr(gl)),
-                       "kge_margin_step_bwd")
-        else:
-            _lib.check(_lib.load().kge_rel_step_bwd(ctypes.byref(a), ctypes.byref(g), _ptr(gl)),
-                       "kge_rel_step_bwd")
-        return (None,) * 13 + tuple(gs) + (None,) * 3
+        name = _MarginStep._entry(a, "bwd")
+        _lib.check(getattr(_lib.load(), name)(ctypes.byref(a), ctypes.byref(g), _ptr(gl)), name)
+        return (None,) * 13 + tuple(gs) + (None,) * 4
 
 
 #: what every rank's kernels of one sharded step are told (engine.margin_step_fwd / _bwd)
 #: loss_kind: _lib.LOSS_* (default the margin loss); n_rel > 0: a relation-corrupting step that replaces an
-#: entity with probability rel_share (kge_rel_step_*), n_rel = 0 the entity step
+#: entity with probability rel_share (kge_rel_step_*), n_rel = 0 the entity step; pos = (head_offs, head_ents,
+#: tail_offs, tail_ents): the positional step (kge_pos_step_*), every rank holding the whole CSR
 ShardedStep = collections.namedtuple("ShardedStep",
-                                     "code dim n_ent ent_lo n_rows n_neg margin seed offset loss_kind n_rel rel_share",
-                                     defaults=(_lib.LOSS_MARGIN, 0, 1.0))
+                                     "code dim n_ent ent_lo n_rows n_neg margin seed offset loss_kind n_rel rel_share "
+                                     "pos", defaults=(_lib.LOSS_MARGIN, 0, 1.0, None))
 
 
 class _ShardedMarginStep(torch.autograd.Function):
@@ -376,7 +391,7 @@ def _signed64(x):
 
 
 def sharded_margin_step(model, heads, tails, relations, margin, n_neg, bern_probs, seed, offset, shard,
-                        engine=None, loss_kind=_lib.LOSS_MARGIN, rel_share=None):
+                        engine=None, loss_kind=_lib.LOSS_MARGIN, rel_share=None, positional=None):
     """``fused_margin_step(..., shard=shard)`` (``fused_loss_step`` with ``loss_kind``) for a model that
     holds only the entity rows [shard.lo, shard.hi) of an EntityShard with local storage; the same
     (heads, tails, relations), seed, offset, n_neg, margin and loss kind on every rank.  Returns the full
@@ -387,7 +402,9 @@ def sharded_margin_step(model, heads, tails, relations, margin, n_neg, bern_prob
     gather_rows.
     ``rel_share``: a relation-corrupting step (``BernoulliRelationNegativeSampler``): each negative replaces
     an entity with probability rel_share, else the relation; the rank that holds a positive's head scores
-    its relation negatives.  Every rank must pass the same rel_share (None: the entity step)."""
+    its relation negatives.  Every rank must pass the same rel_share (None: the entity step).
+    ``positional``: (head_offs, head_ents, tail_offs, tail_ents), the whole candidate CSR on every rank (see
+    ``fused_margin_step``); a negative is scored by the rank holding the entity it draws."""
     # argument errors first, on every rank: none of them may leave the others waiting in a collective
     if isinstance(shard, QueryShard):
         raise ValueError("the fused training step takes an EntityShard; QueryShard (data-parallel "
@@ -405,21 +422,35 @@ def sharded_margin_step(model, heads, tails, relations, margin, n_neg, bern_prob
     n_rel, share = (0, 1.0) if rel_share is None else (int(rel0.shape[-2]), float(rel_share))
     if rel_share is not None:
         _check_rel_share(n_rel, share)
+    if positional is not None:
+        if rel_share is not None:
+            raise ValueError("positional negatives replace an entity: they take no rel_share")
+        positional = _positional_csr(positional, int(rel0.shape[-2]), rel0.device)
     step = ShardedStep(code, _kernel_dim(model, code), shard.n_ent, shard.lo, int(ent0.shape[-2]), int(n_neg),
                        float(margin), int(seed) & 0xFFFFFFFFFFFFFFFF, int(offset) & 0xFFFFFFFFFFFFFFFF,
-                       int(loss_kind), n_rel, share)
+                       int(loss_kind), n_rel, share, positional)
     _check_table(step, shard)
     # one small collective: every rank must draw the same negatives for the same batch and loss.  The last
     # field holds the loss kind and, above it, the float32 bits of 1 - rel_share: 0 for the entity step,
-    # whose draws are those of rel_share = 1
+    # whose draws are those of rel_share = 1; bit 40 marks the positional step
     kind_share = step.loss_kind | struct.unpack("<I", struct.pack("<f", 1.0 - share))[0] << 8
+    if positional is not None:
+        kind_share |= 1 << 40
     mine = torch.tensor([_signed64(step.seed), _signed64(step.offset), b, step.n_neg,
                          struct.unpack("<q", struct.pack("<d", step.margin))[0], kind_share],
                         dtype=torch.int64, device=rel0.device)
     everyone = shard.stack_all(mine)
     if not bool((everyone == mine).all()):
         raise ValueError("the ranks of a sharded step disagree on (seed, offset, batch size, n_neg, margin, "
-                         "loss kind and rel_share): %s" % everyone.tolist())
+                         "loss kind, rel_share and positional or not): %s" % everyone.tolist())
+    if positional is not None:
+        # every rank is positional here (the check above): a second collective of the CSR's sizes, so ranks
+        # whose samplers were built on different graphs raise on every rank
+        sizes = torch.tensor([int(x.shape[0]) for x in positional], dtype=torch.int64, device=rel0.device)
+        every_size = shard.stack_all(sizes)
+        if not bool((every_size == sizes).all()):
+            raise ValueError("the ranks of a positional sharded step hold different candidate CSRs (sizes of "
+                             "head_offs, head_ents, tail_offs, tail_ents per rank: %s)" % every_size.tolist())
     return _ShardedMarginStep.apply(step, shard, engine or default_engine(), heads, tails, relations,
                                     bern_probs, ent0, ent1, rel0, rel1)
 
@@ -433,19 +464,41 @@ def _check_rel_share(n_rel, rel_share):
                          "use rel_share = 1" % n_rel)
 
 
+def _positional_csr(positional, n_rel, dev):
+    """The positional step's (head_offs, head_ents, tail_offs, tail_ents) as int64 tensors on dev, after
+    checking that they are two CSRs over the model's n_rel relations."""
+    if len(positional) != 4:
+        raise ValueError("positional must be (head_offs, head_ents, tail_offs, tail_ents)")
+    for name, x in zip(("head_offs", "head_ents", "tail_offs", "tail_ents"), positional):
+        if not isinstance(x, torch.Tensor) or x.dim() != 1:
+            raise ValueError("positional: %s must be a 1-D tensor" % name)
+    for name, offs in (("head_offs", positional[0]), ("tail_offs", positional[2])):
+        if offs.shape[0] != n_rel + 1:
+            raise ValueError("positional: %s covers %d relations, the model has %d" % (name, offs.shape[0] - 1, n_rel))
+    return tuple(_idx(x, dev) for x in positional)
+
+
 def _fused_step(model, heads, tails, relations, loss_kind, margin, n_neg, negatives, bern_probs, seed, offset,
-                shard, rel_share=None):
+                shard, rel_share=None, positional=None):
     if negatives is not None and len(negatives) not in (2, 3):
         raise ValueError("negatives must be (neg_heads, neg_tails) or (neg_heads, neg_tails, neg_rels)")
+    if positional is not None and negatives is not None:
+        raise ValueError("positional sets how negatives are drawn; it takes no caller negatives")
+    if positional is not None and rel_share is not None:
+        raise ValueError("positional negatives replace an entity: they take no rel_share")
     if shard is not None:
         if negatives is not None:
             raise ValueError("external negatives are not supported by the sharded training step")
         return sharded_margin_step(model, heads, tails, relations, margin, n_neg, bern_probs, seed, offset,
-                                   shard, loss_kind=loss_kind, rel_share=rel_share)
+                                   shard, loss_kind=loss_kind, rel_share=rel_share, positional=positional)
     spec_code = _training_code(model)
     ent0, ent1, rel0, rel1 = _param_tensors(model, spec_code)
     nh = nt = nr = None
     rel = None
+    if positional is not None:
+        positional = _positional_csr(positional, int(rel0.shape[-2]), rel0.device)
+        if bern_probs is None:
+            raise ValueError("a positional step needs bern_probs")
     if negatives is not None and rel_share is not None:
         raise ValueError("rel_share sets how negatives are drawn; with caller negatives give (neg_heads, "
                          "neg_tails, neg_rels) and no rel_share")
@@ -465,11 +518,12 @@ def _fused_step(model, heads, tails, relations, loss_kind, margin, n_neg, negati
     elif bern_probs is None:
         raise ValueError("either negatives or bern_probs must be given")
     return _MarginStep.apply(spec_code, _kernel_dim(model, spec_code), model.n_ent, margin, n_neg, heads, tails,
-                             relations, nh, nt, bern_probs, seed, offset, ent0, ent1, rel0, rel1, loss_kind, nr, rel)
+                             relations, nh, nt, bern_probs, seed, offset, ent0, ent1, rel0, rel1, loss_kind, nr, rel,
+                             positional)
 
 
 def fused_loss_step(model, heads, tails, relations, criterion, n_neg=1, negatives=None, bern_probs=None,
-                    seed=0, offset=0, *, shard=None, rel_share=None):
+                    seed=0, offset=0, *, shard=None, rel_share=None, positional=None):
     """``fused_margin_step`` for any of the three losses: Bernoulli corruption (or the given
     ``negatives``), ``model(h, t, r, nh, nt)`` and ``criterion(pos, neg)`` in a single kernel,
     differentiable with respect to the embedding tables.
@@ -481,15 +535,16 @@ def fused_loss_step(model, heads, tails, relations, criterion, n_neg=1, negative
           logistic: softplus(-pos_i) + softplus(neg_ij)
           BCE     : -max(log sig(pos_i), -100) - max(log(1 - sig(neg_ij)), -100)
         and its gradients are those torch's SoftMarginLoss / BCELoss backward give.
-    shard, rel_share, negatives: as in ``fused_margin_step``; every rank must pass the same kind of loss.
+    shard, rel_share, negatives, positional: as in ``fused_margin_step``; every rank must pass the same kind of
+    loss.
     """
     kind, margin = loss_kind_of(criterion)
     return _fused_step(model, heads, tails, relations, kind, margin, n_neg, negatives, bern_probs, seed, offset,
-                       shard, rel_share)
+                       shard, rel_share, positional)
 
 
 def fused_margin_step(model, heads, tails, relations, margin, n_neg=1, negatives=None,
-                      bern_probs=None, seed=0, offset=0, *, shard=None, rel_share=None):
+                      bern_probs=None, seed=0, offset=0, *, shard=None, rel_share=None, positional=None):
     """Loss of one training step, fused: Bernoulli corruption (or the given ``negatives =
     (neg_heads, neg_tails)``), ``model(h, t, r, nh, nt)`` and ``MarginLoss(margin)`` in a
     single kernel, differentiable with respect to the embedding tables.
@@ -511,7 +566,14 @@ def fused_margin_step(model, heads, tails, relations, margin, n_neg=1, negatives
     negatives: also ``(neg_heads, neg_tails, neg_rels)``; a negative is then scored as
         ``model.scoring_function(nh, nt, nr)`` and any of its positions may differ from the positive's.
 
+    positional: ``(head_offs, head_ents, tail_offs, tail_ents)``, positional negatives
+        (``PositionalNegativeSampler``): the head (probability bern_probs[r]) or the tail is replaced by an
+        entity drawn uniformly from relation r's sorted candidates on that side, ents[offs[r]:offs[r + 1]], or
+        uniformly from [0, n_ent) when there are none -- the draws of ``kge_pos_step_fwd``.  Both CSRs cover the
+        model's relations; their entities must be ids of the model's table (the sampler checks this).  Not with
+        ``negatives`` or ``rel_share``.  With ``shard`` every rank passes the whole CSR.
+
     ``fused_loss_step`` takes a criterion instead of a margin (LogisticLoss, BinaryCrossEntropyLoss).
     """
     return _fused_step(model, heads, tails, relations, _lib.LOSS_MARGIN, margin, n_neg, negatives, bern_probs,
-                       seed, offset, shard, rel_share)
+                       seed, offset, shard, rel_share, positional)
