@@ -25,7 +25,7 @@ from tests import helpers, shard_threads  # noqa: E402
 from tests.test_relpred_sharding_gloo import OracleRelEngine  # noqa: E402
 from tests.test_sharding_gloo import OracleEngine  # noqa: E402
 from tests.test_topk_sharding_gloo import OracleTopkEngine, key_order  # noqa: E402
-from tests.test_train_sharding_gloo import OracleStepEngine, _local_model  # noqa: E402
+from tests.train_kit import OracleStepEngine  # noqa: E402
 from torchkge_b200 import _lib  # noqa: E402
 from torchkge_b200.data import filter_csr  # noqa: E402
 from torchkge_b200.engine import (EntityShard, ModelSpec, QueryShard, rank_link_prediction,  # noqa: E402
@@ -127,7 +127,7 @@ def _train(kind):
         model = helpers.make_model(kind, DIM, n_ent, N_REL, seed=6)
         h, t, r = _graph(n_ent, n)
         shard = EntityShard(n_ent, rank, world, group, local_storage=True)
-        local = _local_model(kind, model, shard.lo, shard.hi, N_REL, DIM)
+        local = helpers.local_model(kind, model, shard.lo, shard.hi, N_REL, DIM)
         with torch.enable_grad():
             loss = sharded_margin_step(local, h, t, r, 0.5, 2, torch.full((N_REL,), 0.5), 7, 1, shard,
                                        engine=OracleStepEngine())

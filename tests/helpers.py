@@ -244,169 +244,9 @@ def rescal_order_matches_here(d):
     return _RESCAL_ORDER[d]
 
 
-# ---------------------------------------------------------------------------- fused training step
-from torchkge_b200 import _lib  # noqa: E402
-from torchkge_b200.engine import EntityShard, _exchanged_rows  # noqa: E402
-from torchkge_b200.training import (ShardedStep, _kernel_dim, _MarginStep, _param_tensors, _row_spec,  # noqa: E402
-                                    _training_code)
-
-DEV = "cuda:0"
-LOSS_KINDS = {"margin": _lib.LOSS_MARGIN, "logistic": _lib.LOSS_LOGISTIC, "bce": _lib.LOSS_BCE}
-
-
-def close_grad(a, b, rtol=1e-4):
-    """Gradient tables are sums of many signed terms accumulated by atomics in arbitrary order: rtol on
-    the element plus an absolute floor of 1e-5 of the table's largest entry (tests/test_train_gpu.py)."""
-    b = b.detach().cpu().float()
-    torch.testing.assert_close(a.detach().cpu().float(), b, rtol=rtol, atol=1e-5 * float(b.abs().max()) + 1e-9)
-
-
-def train_leaves(model):
-    """The model's tables in ModelSpec order as fresh leaves (RotatE: the (cos, sin) planes; Analogy:
-    stacked (3, n, dim) tables)."""
-    code = _training_code(model)
-    ts = [None if x is None else x.detach().clone().contiguous().requires_grad_(True)
-          for x in _param_tensors(model, code)]
-    return code, _kernel_dim(model, code), ts
-
-
-def train_model(kind, d, n_ent, n_rel, seed):
-    """A model on cuda:0 whose entity rows are not unit rows where the model normalises them."""
-    model = make_model(kind, d, n_ent, n_rel, seed=seed)
-    if kind in ("transe_l1", "transe_l2", "distmult", "rescal"):
-        with torch.no_grad():
-            model.ent_emb.weight.mul_(1.0 + torch.rand(n_ent, 1))   # un-normalised rows
-    if kind.startswith("toruse"):
-        model.normalize_parameters()
-    return model.to(DEV)
-
-
-def negatives(h, t, n_ent, n_neg, gen):
-    """Head and tail corruption mixed, a negative equal to its positive, a few with both ends replaced."""
-    b = h.shape[0]
-    nh, nt = h.repeat(n_neg), t.repeat(n_neg)
-    which = torch.rand(b * n_neg, generator=gen) < 0.45
-    rnd = torch.randint(1, n_ent, (b * n_neg,), generator=gen)
-    nh = torch.where(which, rnd, nh)
-    nt = torch.where(~which, rnd, nt)
-    nt[0], nh[0] = t[0], h[0]
-    both = torch.arange(7, b * n_neg, 97)
-    nh[both] = (h.repeat(n_neg)[both] + 3) % n_ent
-    nt[both] = (t.repeat(n_neg)[both] + 5) % n_ent
-    return nh, nt
-
-
-def torch_loss(loss, pos, neg, margin=0.0):
-    """utils/losses.py restated with torch's own modules (pos already repeated n_neg times).
-    "logistic_stable": the same loss through softplus -- SoftMarginLoss evaluates log(1 + exp(-y x)) as
-    written and overflows to inf beyond |x| ~ 88, where the package's LogisticLoss, fused or not, is finite."""
-    if loss == "margin":
-        return torch.nn.MarginRankingLoss(margin=margin, reduction="sum")(pos, neg, torch.ones_like(pos))
-    if loss == "logistic_stable":
-        return torch.nn.functional.softplus(-pos).sum() + torch.nn.functional.softplus(neg).sum()
-    if loss == "logistic":
-        crit = torch.nn.SoftMarginLoss(reduction="sum")
-        return crit(pos, torch.ones_like(pos)) + crit(neg, -torch.ones_like(neg))
-    crit = torch.nn.BCELoss(reduction="sum")
-    return crit(torch.sigmoid(pos), torch.ones_like(pos)) + crit(torch.sigmoid(neg), torch.zeros_like(neg))
-
-
-def _torus_scores(kind, ent, rel, h, t, r):
-    """translation.py:706-720 with dissimilarities.py:28-43 (torus L1 / L2)."""
-    x = (torch.frac(ent[h]) + torch.frac(rel[r])) - torch.frac(ent[t])
-    if kind == "toruse_l1":
-        ax = x.abs()
-        return -(2 * torch.minimum(ax, 1 - ax)).sum(dim=1)
-    x2 = x * x
-    return -(4 * torch.minimum(x2, 1 - x2)).sum(dim=1)
-
-
-def cpu_pos_neg(kind, leaves, h, t, r, nh, nt):
-    """oracle.forward_pos_neg over CPU copies of the kernel's leaves (TorusE restated above)."""
-    e0, e1, r0, r1 = leaves
-    if kind.startswith("toruse"):
-        n_neg = nh.shape[0] // h.shape[0]
-        return (_torus_scores(kind, e0, r0, h, t, r).repeat(n_neg),
-                _torus_scores(kind, e0, r0, nh, nt, r.repeat(n_neg)))
-    if kind in ("transe_l1", "transe_l2", "distmult"):
-        P = {"ent": e0, "rel": r0}
-    elif kind == "rescal":
-        P = {"ent": e0, "rel_mat": r0}
-    elif kind == "analogy":
-        P = {"sc_ent": e0[0], "re_ent": e0[1], "im_ent": e0[2], "sc_rel": r0[0], "re_rel": r0[1], "im_rel": r0[2]}
-    else:
-        P = {"re_ent": e0, "im_ent": e1, "re_rel": r0, "im_rel": r1}
-    return oracle.forward_pos_neg(kind, P, h, t, r, nh, nt)
-
-
-def cpu_leaves(ts, dtype=torch.float32):
-    """CPU copies of the kernel's leaves, as fresh leaves of `dtype`."""
-    return [None if x is None else x.detach().cpu().to(dtype).clone().requires_grad_(True) for x in ts]
-
-
-def check_against_cpu(model, kind, loss, h, t, r, nh, nt, rtol=2e-4, ref=None):
-    """fused step on the GPU (external negatives) vs torch autograd on the CPU (torch_loss(ref or loss)),
-    same leaf tables."""
-    code, dim, ts = train_leaves(model)
-    got = _MarginStep.apply(code, dim, model.n_ent, 0.0, nh.shape[0] // h.shape[0], h.to(DEV), t.to(DEV),
-                            r.to(DEV), nh.to(DEV), nt.to(DEV), None, 0, 0, *ts, LOSS_KINDS[loss])
-    got.backward()
-    cpu = cpu_leaves(ts)
-    pos, neg = cpu_pos_neg(kind, cpu, h.cpu(), t.cpu(), r.cpu(), nh.cpu(), nt.cpu())
-    want = torch_loss(ref or loss, pos, neg)
-    want.backward()
-    assert abs(got.item() - want.item()) <= 2e-5 * abs(want.item()) + 1e-12, (got.item(), want.item())
-    for a, b in zip(ts, cpu):
-        if a is not None:
-            close_grad(a.grad, b.grad, rtol)
-    return ts, cpu
-
-
-def unsharded(model, h, t, r, probs, margin, n_neg, seed, offset, loss_kind=_lib.LOSS_MARGIN):
-    """(loss, [grad tables]) of the fused step on the whole table, Philox negatives."""
-    code, dim, ts = train_leaves(model)
-    loss = _MarginStep.apply(code, dim, model.n_ent, margin, n_neg, h, t, r, None, None, probs, seed, offset, *ts,
-                             loss_kind)
-    loss.backward()
-    return loss.item(), [None if x is None else x.grad for x in ts]
-
-
-def emulated(model, h, t, r, probs, margin, n_neg, seed, offset, world, eng, loss_kind=_lib.LOSS_MARGIN):
-    """What `world` ranks compute, one rank range after the other on one device: the loss, the
-    relation gradients and grad_hrows / grad_trows summed over the ranks (the all-reduces), then
-    every rank's scatter into its own rows."""
-    code, dim, ts = train_leaves(model)
-    tabs = [None if x is None else x.detach() for x in ts]
-    n_ent, b = model.n_ent, h.shape[0]
-    full = ShardedStep(code, dim, n_ent, 0, n_ent, n_neg, float(margin), seed, offset, loss_kind)
-    rows = _exchanged_rows(_row_spec(full, tabs), torch.cat([h, t]), EntityShard(n_ent), eng)
-    hrows, trows = rows[:b], rows[b:]
-    loss = torch.zeros((), dtype=torch.float32, device=DEV)
-    grad_rows = torch.zeros_like(rows)
-    grel = [None if x is None else torch.zeros_like(x) for x in tabs[2:]]
-    gent = [None if x is None else torch.zeros_like(x) for x in tabs[:2]]
-    parts = []
-    for rank in range(world):
-        sh = EntityShard(n_ent, rank, world, local_storage=True)
-        n = sh.hi - sh.lo
-        # every rank's entity rows and entity gradient are views of rows [lo, hi) of one table (a
-        # three-plane table keeps its planes equally spaced)
-        local = [None if x is None else x.narrow(-2, sh.lo, n) for x in tabs[:2]] + tabs[2:]
-        lg = [None if x is None else x.narrow(-2, sh.lo, n) for x in gent]
-        parts.append((sh, lg))
-        if n == 0:
-            continue
-        step = ShardedStep(code, dim, n_ent, sh.lo, n, n_neg, float(margin), seed, offset, loss_kind)
-        loss += eng.margin_step_fwd(step, local, h, t, r, probs, hrows, trows)
-        g_rows = torch.zeros_like(rows)
-        g_rel = [None if x is None else torch.zeros_like(x) for x in tabs[2:]]
-        gl = torch.ones((), dtype=torch.float32, device=DEV)
-        eng.margin_step_bwd(step, local, lg + g_rel, h, t, r, probs, gl, hrows, trows, g_rows[:b], g_rows[b:])
-        grad_rows += g_rows
-        for a, c in zip(grel, g_rel):
-            if a is not None:
-                a += c
-    for sh, lg in parts:          # after the all-reduce: every rank adds the rows it holds
-        if sh.hi > sh.lo:
-            eng.scatter_rows_add(code, dim, lg[0], lg[1], sh.lo, torch.cat([h, t]), grad_rows)
-    return loss.item(), gent + grel
+# ---------------------------------------------------------------------------- entity-sharded models
+def local_model(kind, model, lo, hi, n_rel, dim):
+    """The same model holding only entity rows [lo, hi), on the model's device."""
+    part = make_model(kind, dim, hi - lo, n_rel, seed=0)
+    part.load_state_dict({name: w[lo:hi] if "ent_emb" in name else w for name, w in model.state_dict().items()})
+    return part.to(next(model.parameters()).device)

@@ -18,13 +18,6 @@ STORAGES = ["local", "full", "query"]
 
 
 # ------------------------------------------------------------------ helpers
-def local_model(kind, model, lo, hi, n_rel, dim):
-    """The same model holding only entity rows [lo, hi)."""
-    part = helpers.make_model(kind, dim, hi - lo, n_rel, seed=0)
-    part.load_state_dict({name: w[lo:hi] if "ent_emb" in name else w for name, w in model.state_dict().items()})
-    return part.to(next(model.parameters()).device)
-
-
 def make_shard(storage, rank, world, group, n_ent, n_facts):
     if storage == "query":
         return QueryShard(n_facts, rank, world, group)
@@ -37,7 +30,7 @@ def sharded_evaluator(kind, model, kg, dim, directed, storage, world):
 
     def rank_fn(rank, group):
         shard = make_shard(storage, rank, world, group, n_ent, kg.n_facts)
-        m = local_model(kind, model, shard.lo, shard.hi, n_rel, dim) if storage == "local" else model
+        m = helpers.local_model(kind, model, shard.lo, shard.hi, n_rel, dim) if storage == "local" else model
         ev = tk.RelationPredictionEvaluator(m, kg, directed, shard=shard)
         ev.evaluate(b_size=64, verbose=False)
         return ev.rank_true_rels, ev.filt_rank_true_rels
@@ -184,13 +177,13 @@ def test_argument_errors():
     with pytest.raises(ValueError, match="local_storage=True"):     # the whole table, not rows [0, 20)
         tk.RelationPredictionEvaluator(model, kg, shard=EntityShard(n_ent, 0, 2, local_storage=True)).evaluate(8)
     with pytest.raises(ValueError, match="partitions 40 entities, the model has 20"):
-        part = local_model("distmult", model, 0, 20, n_rel, dim)
+        part = helpers.local_model("distmult", model, 0, 20, n_rel, dim)
         tk.RelationPredictionEvaluator(part, kg, shard=EntityShard(n_ent, 0, 2)).evaluate(8)
     rot = helpers.make_model("rotate", dim, n_ent, n_rel).to(DEV)
     with pytest.raises(NotImplementedError):
         tk.RelationPredictionEvaluator(rot, kg, shard=QueryShard(kg.n_facts, 0, 2)).evaluate(8)
     # the index check uses the global entity count: a local model of 20 rows takes ids up to 39 ...
-    part = local_model("distmult", model, 20, 40, n_rel, dim)
+    part = helpers.local_model("distmult", model, 20, 40, n_rel, dim)
     shard = EntityShard(n_ent, 1, 2, local_storage=True)
     bad = tk.KnowledgeGraph(torch.tensor([39]), torch.tensor([40]), torch.tensor([0]), n_ent + 1, n_rel,
                             dict_of_heads={}, dict_of_tails={})
@@ -223,7 +216,7 @@ def _api_worker(rank, world, backend):
             full = EntityShard.from_group(n_ent)
             for name, shard, m in (
                     ("entity-local", EntityShard.from_group(n_ent, local_storage=True),
-                     local_model(kind, model, full.lo, full.hi, n_rel, dim)),
+                     helpers.local_model(kind, model, full.lo, full.hi, n_rel, dim)),
                     ("query", QueryShard.from_group(kg_test.n_facts), model)):
                 got_r = tk.RelationPredictionEvaluator(m, kg_test, directed=False, shard=shard)
                 got_r.evaluate(b_size=64, verbose=False)

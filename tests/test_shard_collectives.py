@@ -13,7 +13,7 @@ import torchkge_b200 as tk
 from tests import helpers
 from tests.golden import make_golden_collectives as gen
 from tests.test_sharding_gloo import OracleEngine
-from tests.test_train_sharding_gloo import Shard
+from tests.train_kit import NoCollectiveShard
 from torchkge_b200 import _lib
 from torchkge_b200.engine import (ModelSpec, QueryShard, rank_link_prediction, topk_entity_inference,
                                   topk_relation_inference)
@@ -38,8 +38,8 @@ def _table_case(case, n_ent=20):
     whole table as this rank's rows, 'full_narrowed' declares this rank's rows as the whole table."""
     spec = ModelSpec.from_model(helpers.make_model("distmult", 8, n_ent, gen.N_REL, seed=1))
     if case == "local_whole":
-        return spec, Shard(n_ent, 1, 2, local_storage=True), "should hold 10 entity rows .*, the model holds 20 entity rows"
-    shard = Shard(n_ent, 1, 2)
+        return spec, NoCollectiveShard(n_ent, 1, 2, local_storage=True), "should hold 10 entity rows .*, the model holds 20 entity rows"
+    shard = NoCollectiveShard(n_ent, 1, 2)
     return spec.narrowed(shard.lo, shard.hi), shard, "should hold 20 entity rows .*, the model holds 10 entity rows"
 
 

@@ -248,13 +248,6 @@ def test_merge_rejects_arguments_out_of_range():
 
 
 # ------------------------------------------------------------------ 4./5. public API, two processes
-def _local_model(kind, model, lo, hi, n_rel, dim):
-    """The same model holding only entity rows [lo, hi)."""
-    part = helpers.make_model(kind, dim, hi - lo, n_rel, seed=0)
-    part.load_state_dict({name: w[lo:hi] if "ent_emb" in name else w for name, w in model.state_dict().items()})
-    return part.to(next(model.parameters()).device)
-
-
 def _api_worker(rank, world, backend):
     dev = torch.device("cuda:%d" % (rank if backend == "nccl" else 0))
     torch.cuda.set_device(dev)
@@ -275,7 +268,7 @@ def _api_worker(rank, world, backend):
             for name, shard, m in (
                     ("entity-full", full, model),
                     ("entity-local", EntityShard.from_group(n_ent, local_storage=True),
-                     _local_model(kind, model, full.lo, full.hi, n_rel, dim)),
+                     helpers.local_model(kind, model, full.lo, full.hi, n_rel, dim)),
                     ("query", QueryShard.from_group(ents.shape[0]), model)):
                 got_e = tk.EntityInference(m, ents, rels, top_k=30, missing="heads", dictionary=dictionary,
                                            shard=shard)

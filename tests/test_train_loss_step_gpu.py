@@ -13,13 +13,13 @@ import torch
 
 import torchkge_b200 as tk
 from tests import helpers
+from tests import train_kit as kit
+from tests.train_kit import DEV
 from torchkge_b200 import _lib
-from torchkge_b200.engine import _ptr, _stream
-from torchkge_b200.training import _MarginStep, fused_loss_step, fused_margin_step, loss_kind_of
+from torchkge_b200.engine import _ptr
+from torchkge_b200.training import fused_loss_step, fused_margin_step, loss_kind_of
 
 pytestmark = pytest.mark.gpu
-DEV = "cuda:0"
-ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 ALL_KINDS = ["transe_l1", "transe_l2", "distmult", "rescal", "complex", "rotate", "analogy", "toruse_l1",
              "toruse_l2"]
 LOSSES = {"logistic": (tk.LogisticLoss, _lib.LOSS_LOGISTIC), "bce": (tk.BinaryCrossEntropyLoss, _lib.LOSS_BCE)}
@@ -38,7 +38,7 @@ def test_fused_step_matches_reference_golden(case, loss):
     assert got.item() == pytest.approx(float(z["loss_" + loss]), rel=1e-5)
     got.backward()
     for name, p in model.named_parameters():
-        helpers.close_grad(p.grad, torch.from_numpy(z["g_%s:%s" % (loss, name)]))
+        kit.close_grad(p.grad, torch.from_numpy(z["g_%s:%s" % (loss, name)]))
 
 
 # ---------------------------------------------------------------- 2. every training kind vs CPU autograd
@@ -47,12 +47,12 @@ def test_fused_step_matches_reference_golden(case, loss):
 def test_every_kind_matches_cpu_autograd(kind, loss):
     n_ent, n_rel, b, n_neg = 300, 6, 64, 5
     d = 12 if kind == "rescal" else 40
-    model = helpers.train_model(kind, d, n_ent, n_rel, seed=4)
+    model = kit.train_model(kind, d, n_ent, n_rel, seed=4)
     gen = torch.Generator().manual_seed(6)
     h, t = torch.randint(0, n_ent, (b,), generator=gen), torch.randint(0, n_ent, (b,), generator=gen)
     r = torch.randint(0, n_rel, (b,), generator=gen)
-    nh, nt = helpers.negatives(h, t, n_ent, n_neg, gen)
-    helpers.check_against_cpu(model, kind, loss, h, t, r, nh, nt)
+    nh, nt = kit.negatives(h, t, n_ent, n_neg, gen)
+    kit.check_against_cpu(model, kind, loss, h, t, r, nh, nt)
 
 
 # ---------------------------------------------------------------- 3. the ring kernel's shapes
@@ -67,32 +67,26 @@ def test_ring_shapes_match_cpu_autograd(kind, d, n_neg, source, loss):
     """External negatives (mixed sides, one equal to its positive, some with both ends replaced) and
     Philox draws (the ring's own draw loop; the CPU side gets kge_corrupt_batch's negatives)."""
     n_ent, n_rel, b = 900, 7, 96
-    model = helpers.train_model(kind, d, n_ent, n_rel, seed=11)
+    model = kit.train_model(kind, d, n_ent, n_rel, seed=11)
     gen = torch.Generator().manual_seed(d + n_neg)
     h, t = torch.randint(0, n_ent, (b,), generator=gen), torch.randint(0, n_ent, (b,), generator=gen)
     r = torch.randint(0, n_rel, (b,), generator=gen)
     if source == "external":
-        nh, nt = helpers.negatives(h, t, n_ent, n_neg, gen)
-        helpers.check_against_cpu(model, kind, loss, h, t, r, nh, nt)
+        nh, nt = kit.negatives(h, t, n_ent, n_neg, gen)
+        kit.check_against_cpu(model, kind, loss, h, t, r, nh, nt)
         return
     probs = torch.rand(n_rel, generator=gen).to(DEV)
     hd, td, rd = h.to(DEV), t.to(DEV), r.to(DEV)
-    nh = torch.empty(b * n_neg, dtype=torch.int64, device=DEV)
-    nt = torch.empty_like(nh)
-    _lib.check(_lib.load().kge_corrupt_batch(_ptr(hd), _ptr(td), _ptr(rd), b, n_neg, _ptr(probs), n_ent, 31, 2,
-                                             _ptr(nh), _ptr(nt), _stream(hd.device)), "kge_corrupt_batch")
-    code, dim, ts = helpers.train_leaves(model)
-    got = _MarginStep.apply(code, dim, n_ent, 0.0, n_neg, hd, td, rd, None, None, probs, 31, 2, *ts,
-                            LOSSES[loss][1])
-    got.backward()
-    cpu = [None if x is None else x.detach().cpu().clone().requires_grad_(True) for x in ts]
-    pos, neg = helpers.cpu_pos_neg(kind, cpu, h, t, r, nh.cpu(), nt.cpu())
-    want = helpers.torch_loss(loss, pos, neg)
+    nh, nt = kit.corrupt_batch(hd, td, rd, probs, n_neg, n_ent, 31, 2)
+    got, grads = kit.whole_table_step(model, hd, td, rd, n_neg=n_neg, loss=loss, probs=probs, seed=31, offset=2)
+    cpu = kit.cpu_leaves(kit.train_leaves(model)[2])
+    pos, neg = kit.cpu_pos_neg(kind, cpu, h, t, r, nh.cpu(), nt.cpu())
+    want = kit.torch_loss(loss, pos, neg)
     want.backward()
-    assert got.item() == pytest.approx(want.item(), rel=2e-5)
-    for a, c in zip(ts, cpu):
+    assert got == pytest.approx(want.item(), rel=2e-5)
+    for a, c in zip(grads, cpu):
         if a is not None:
-            helpers.close_grad(a.grad, c.grad, rtol=2e-4)
+            kit.close_grad(a, c.grad, rtol=2e-4)
 
 
 # ---------------------------------------------------------------- 4. saturated sigmoids
@@ -119,20 +113,20 @@ def test_saturated_scores(kind, d, loss):
     gen = torch.Generator().manual_seed(22)
     h, t = torch.randint(0, n_ent, (b,), generator=gen), torch.randint(0, n_ent, (b,), generator=gen)
     r = torch.randint(0, n_rel, (b,), generator=gen)
-    nh, nt = helpers.negatives(h, t, n_ent, n_neg, gen)
+    nh, nt = kit.negatives(h, t, n_ent, n_neg, gen)
     with torch.no_grad():
-        code, dim, ts = helpers.train_leaves(model)
-        pos, neg = helpers.cpu_pos_neg(kind, [None if x is None else x.cpu() for x in ts], h, t, r, nh, nt)
+        pos, neg = kit.cpu_pos_neg(kind, [None if x is None else x.cpu() for x in kit.train_leaves(model)[2]], h,
+                                   t, r, nh, nt)
     sat = r.repeat(n_neg) > 0
     assert (pos[sat].abs() > 100).all() and (neg[sat].abs() > 100).all()
     assert (pos[~sat].abs() < 20).all()
-    ts, cpu = helpers.check_against_cpu(model, kind, loss, h, t, r, nh, nt,
-                                ref="logistic_stable" if loss == "logistic" else None)
-    for a, c in zip(ts, cpu):
+    grads, cpu = kit.check_against_cpu(model, kind, loss, h, t, r, nh, nt,
+                                       ref="logistic_stable" if loss == "logistic" else None)
+    for a, c in zip(grads, cpu):
         if a is not None:
-            assert torch.equal(a.grad.cpu() == 0, c.grad == 0)
+            assert torch.equal(a.cpu() == 0, c.grad == 0)
     if loss == "bce":      # every pair of relations 1 and 2 is saturated: their rows get exactly 0
-        assert (ts[2].grad[1:] == 0).all() and (cpu[2].grad[1:] == 0).all()
+        assert (grads[2][1:] == 0).all() and (cpu[2].grad[1:] == 0).all()
 
 
 # ---------------------------------------------------------------- 5. through the sampler
@@ -157,7 +151,7 @@ def test_sampler_fused_step_equals_three_calls(loss):
     model.zero_grad()
     fused.backward()
     for n, p in model.named_parameters():
-        helpers.close_grad(p.grad, g1[n])
+        kit.close_grad(p.grad, g1[n])
 
 
 class MarginLoss(torch.nn.Module):
@@ -171,7 +165,7 @@ class MarginLoss(torch.nn.Module):
 @pytest.mark.parametrize("crit", ["package", "torchkge"])
 def test_margin_criterion_equals_fused_margin_step(crit):
     n_ent, n_rel, d, b = 500, 5, 200, 128
-    model = helpers.train_model("distmult", d, n_ent, n_rel, seed=2)
+    model = kit.train_model("distmult", d, n_ent, n_rel, seed=2)
     gen = torch.Generator().manual_seed(3)
     h, t = torch.randint(0, n_ent, (b,), generator=gen).to(DEV), torch.randint(0, n_ent, (b,), generator=gen).to(DEV)
     r = torch.randint(0, n_rel, (b,), generator=gen).to(DEV)
@@ -186,19 +180,16 @@ def test_margin_criterion_equals_fused_margin_step(crit):
     got.backward()
     assert got.item() == pytest.approx(want.item(), rel=1e-6)
     for n, p in model.named_parameters():
-        helpers.close_grad(p.grad, g1[n])
+        kit.close_grad(p.grad, g1[n])
 
 
 # ---------------------------------------------------------------- 6. ABI and argument errors
 def test_margin_step_args_field_order_and_abi_version():
-    header = re.sub(r"/\*.*?\*/", "", open(os.path.join(ROOT, "include", "kge_b200.h")).read(), flags=re.S)
-    body = re.search(r"typedef struct \{([^{}]*)\}\s*kge_margin_step_args_t\s*;", header, flags=re.S).group(1)
-    names = [re.findall(r"[A-Za-z_][A-Za-z0-9_]*", part)[-1]
-             for decl in body.split(";") if decl.strip() for part in decl.split(",")]
+    names = kit.header_fields("kge_margin_step_args_t")
     assert names == [n for n, _ in _lib.MarginStepArgs._fields_]
     assert names[-1] == "loss_kind"
     assert _lib.load().kge_abi_version() == 11 == _lib.ABI_VERSION
-    assert re.search(r"#define KGE_LOSS_MARGIN 0\b", header)
+    assert re.search(r"#define KGE_LOSS_MARGIN 0\b", kit.header())
 
 
 def test_unknown_loss_kind_is_an_argument_error():

@@ -12,68 +12,18 @@ Every step is profiled and the kernels that ran are checked against a Python sta
 rule (expected_kernels), which test_launch_rule_mirrors_train_cu pins to the constants of train.cu.
 Tolerances: the loss within 2e-5 relative of the float64 loss, gradients within rtol 2e-4 plus a floor
 of 1e-5 of the table's largest entry (tests/test_train_gpu.py), scores written out within 1e-5."""
-import ctypes
 import os
 import re
-import subprocess
-import sys
-import time
 
 import pytest
 import torch
 
-from tests import helpers
-from torchkge_b200 import _lib
-from torchkge_b200.engine import CudaEngine, _ptr, _stream
-from torchkge_b200.training import _MarginStep
+from tests import train_kit as kit
+from tests.train_kit import (DEV, FAST_MAX_DIM, RING_MAX_NEG, RING_SLOTS, SMEM_DEFAULT, SMEM_MAX, WARPS_PER_BLOCK,
+                             expected_kernels, kernel_signature, last_n_neg_within, launched)
+from torchkge_b200.engine import CudaEngine
 
-ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
-TRAIN_CU = os.path.join(ROOT, "torchkge_b200", "csrc", "train.cu")
-DEV = helpers.DEV
 SWITCHES = ("KGE_TRAIN_RING", "KGE_TRAIN_BWD_BLOCKS")
-
-# ---------------------------------------------------------------- the launch rule, restated
-RING_SLOTS = 8                 # RING: rows in flight per warp
-WARPS_PER_BLOCK = 4
-FAST_MAX_DIM = 256             # 4 floats x 32 lanes x FAST_NCH chunks
-SMEM_DEFAULT = 48 * 1024       # dynamic shared memory without cudaFuncSetAttribute
-SMEM_MAX = 96 * 1024           # what launch_ring_variant raises the limit to
-RING_MAX_NEG = 8192
-FAST_KINDS = {"transe_l1": _lib.TRANSE_L1, "transe_l2": _lib.TRANSE_L2, "distmult": _lib.DISTMULT}
-
-
-def _pad(x, m):
-    return (x + m - 1) // m * m
-
-
-def ring_smem_bytes(dim, n_neg):
-    """Dynamic shared memory of one ring block: per warp RING rows, the codes of every negative and
-    one mbarrier per slot, each warp's part rounded up to 128 bytes."""
-    per_warp = RING_SLOTS * dim * 4 + _pad(n_neg, 4) * 4 + RING_SLOTS * 8
-    return WARPS_PER_BLOCK * _pad(per_warp, 128)
-
-
-def last_n_neg_within(dim, limit):
-    """The largest n_neg whose ring block fits in `limit` bytes."""
-    n = 1
-    while ring_smem_bytes(dim, n + 1) <= limit:
-        n += 1
-    return n
-
-
-def expected_kernels(kind, dim, n_neg, loss, shard, env=None):
-    """Signatures (see kernel_signature) of the forward and backward kernels one step launches."""
-    env = os.environ if env is None else env
-    ring_on = env.get("KGE_TRAIN_RING", "")[:1] != "0"
-    tight = env.get("KGE_TRAIN_BWD_BLOCKS", "")[:1] == "5"
-    fast = kind in FAST_KINDS and dim % 4 == 0 and dim <= FAST_MAX_DIM
-    if fast and ring_on and n_neg <= RING_MAX_NEG and ring_smem_bytes(dim, n_neg) <= SMEM_MAX:
-        minb = 5 if tight and not shard and loss == "margin" else 0
-        lk = helpers.LOSS_KINDS[loss]
-        return {("ring", FAST_KINDS[kind], False, 0, shard, lk), ("ring", FAST_KINDS[kind], True, minb, shard, lk)}
-    if fast and not shard and loss == "margin":
-        return {("fast", FAST_KINDS[kind], False), ("fast", FAST_KINDS[kind], True)}
-    return {("shard_fwd",), ("shard_bwd",)} if shard else {("fwd",), ("bwd",)}
 
 
 def forward_of(kernels):
@@ -81,12 +31,19 @@ def forward_of(kernels):
 
 
 def test_launch_rule_mirrors_train_cu():
-    """The constants and conditions above are the ones train.cu launches by."""
-    src = open(TRAIN_CU).read()
+    """The constants and branches of expected_kernels are the ones train.cu launches by."""
+    src = re.sub(r"//[^\n]*", "", open(kit.TRAIN_CU).read())
     flat = re.sub(r"\s+", " ", src)
 
     def const(name):
         return int(re.search(r"constexpr int %s = (\d+);" % name, src).group(1))
+
+    def body(head):
+        return re.sub(r"\s+", " ", re.search(re.escape(head) + r".*?\n}", src, flags=re.S).group(0))
+
+    def in_order(text, *parts):
+        at = [text.find(p) for p in parts]
+        assert -1 not in at and at == sorted(at), [p for p, i in zip(parts, at) if i < 0] or at
 
     assert const("RING") == RING_SLOTS
     assert const("WARPS_PER_BLOCK") == WARPS_PER_BLOCK
@@ -96,70 +53,48 @@ def test_launch_rule_mirrors_train_cu():
     # rounded up to 128 bytes
     assert ("const size_t per_warp = (size_t)RING * a.dim * 4 + (size_t)((a.n_neg + 3) & ~3) * 4 + "
             "RING * sizeof(uint64_t); return WARPS_PER_BLOCK * ((per_warp + 127) & ~(size_t)127);") in flat
-    body = re.search(r"bool ring_step_ok\(.*?\n}", src, flags=re.S).group(0)
-    assert "a.n_neg <= %d" % RING_MAX_NEG in body and "ring_smem_bytes(a) <= 96 * 1024" in body
-    assert "getenv(\"KGE_TRAIN_RING\"); return !(v && v[0] == '0');" in re.sub(r"\s+", " ", body)
-    launch = re.search(r"cudaError_t launch_ring_variant\(.*?\n}", src, flags=re.S).group(0)
+    ok = body("bool ring_step_ok(")
+    assert "a.n_neg <= %d" % RING_MAX_NEG in ok and "ring_smem_bytes(a) <= 96 * 1024" in ok
+    assert "getenv(\"KGE_TRAIN_RING\"); return !(v && v[0] == '0');" in ok
+    launch = body("cudaError_t launch_ring_variant(")
     assert "smem > 48 * 1024" in launch and "cudaFuncAttributeMaxDynamicSharedMemorySize, 96 * 1024" in launch
-    assert "getenv(\"KGE_TRAIN_BWD_BLOCKS\"); return v && v[0] == '5';" in flat
     assert ("return (a.model == KGE_TRANSE_L1 || a.model == KGE_TRANSE_L2 || a.model == KGE_DISTMULT) && "
             "a.dim % 4 == 0 && a.dim <= FAST_MAX_DIM;") in flat
-    # the choice itself: ring, else (unsharded margin) the register form, else the generic kernels
-    assert ("if (fast_step_ok(a) && ring_step_ok(a)) return with_fast_model(" in flat and
-            "if (!shard && fast_step_ok(a) && a.loss_kind == KGE_LOSS_MARGIN) {" in flat)
+    # the choice itself: a relation step at rel_share >= 1 without caller negatives or nr_out is the entity
+    # step; then the ring; else the register form for the unsharded entity step with the margin loss only
+    # (never for a relation or positional step); else the generic kernels
+    step = body("cudaError_t launch_margin_step(")
+    in_order(step, "if (a.n_rel > 0 && a.rel_share >= 1.f && !a.nh && !a.nr_out) a.n_rel = 0;",
+             "if (fast_step_ok(a) && ring_step_ok(a)) return with_fast_model(a.model, [&](auto m) { return "
+             "launch_ring<decltype(m)::value, BWD>(a, gr, gloss, st, pc); });",
+             "if (a.n_rel <= 0 && !pc.head_offs) { if (!shard && fast_step_ok(a) && a.loss_kind == KGE_LOSS_MARGIN) "
+             "{ return with_fast_model(a.model, [&](auto m) { margin_step_fast_kernel<decltype(m)::value, BWD><<<",
+             "if (shard) margin_step_shard_bwd_kernel<<<", "else margin_step_bwd_kernel<<<",
+             "if (shard) margin_step_shard_fwd_kernel<<<", "else margin_step_fwd_kernel<<<")
+    assert step.count("margin_step_fast_kernel") == 1 and step.count("launch_ring<") == 1
+    # the ring's kinds: positional, relation, then the entity step, where MINB = 5 (KGE_TRAIN_BWD_BLOCKS=5)
+    # only for the unsharded margin backward; the kernels' template arguments in kernel_signature's order
+    ring = body("cudaError_t launch_ring(")
+    in_order(ring, "if (pc.head_offs) return a.hrows ? launch_ring_variant<MODEL, BWD, 0, true, LOSS, false, true>"
+                   "(a, gr, gloss, st, pc) : launch_ring_variant<MODEL, BWD, 0, false, LOSS, false, true>(a, gr, "
+                   "gloss, st, pc);",
+             "if (a.n_rel > 0) return a.hrows ? launch_ring_variant<MODEL, BWD, 0, true, LOSS, true>(a, gr, gloss, "
+             "st) : launch_ring_variant<MODEL, BWD, 0, false, LOSS, true>(a, gr, gloss, st);",
+             "if (a.hrows) return launch_ring_variant<MODEL, BWD, 0, true, LOSS>(a, gr, gloss, st); "
+             "if constexpr (BWD && LOSS == KGE_LOSS_MARGIN) { static const bool tight = [] { const char* v = "
+             "getenv(\"KGE_TRAIN_BWD_BLOCKS\"); return v && v[0] == '5'; }(); if (tight) return "
+             "launch_ring_variant<MODEL, true, 5, false, LOSS>(a, gr, gloss, st); } "
+             "return launch_ring_variant<MODEL, BWD, 0, false, LOSS>(a, gr, gloss, st);",
+             "case KGE_LOSS_LOGISTIC: return by_shard(std::integral_constant<int, KGE_LOSS_LOGISTIC>{}); "
+             "case KGE_LOSS_BCE: return by_shard(std::integral_constant<int, KGE_LOSS_BCE>{}); "
+             "default: return by_shard(std::integral_constant<int, KGE_LOSS_MARGIN>{});")
+    assert ring.count("launch_ring_variant<") == 7
+    assert ("if constexpr (POS) return margin_step_ring_pos_kernel<MODEL, BWD, SHARD, LOSS>; else if constexpr "
+            "(REL) return margin_step_ring_rel_kernel<MODEL, BWD, SHARD, LOSS>; else return "
+            "margin_step_ring_kernel<MODEL, BWD, MINB, SHARD, LOSS>;") in flat
     assert (SMEM_DEFAULT, SMEM_MAX) == (48 * 1024, 96 * 1024)
     # n_neg <= 8192 never decides: the codes alone pass 96 KB first, at every dim the ring takes
     assert all(last_n_neg_within(d, SMEM_MAX) < RING_MAX_NEG for d in range(4, FAST_MAX_DIM + 1, 4))
-
-
-# ---------------------------------------------------------------- which kernels ran
-_KERNEL = r"margin_step_(ring|fast|shard_fwd|shard_bwd|fwd|bwd)_kernel"
-_DEMANGLED = re.compile(r"(?<![\w])" + _KERNEL + r"(?:<([^<>]*)>)?\(")
-_MANGLED = re.compile(r"\d" + _KERNEL + r"(?:I((?:L[ib]\d+E)+)E)?")
-
-
-def kernel_signature(name):
-    """("ring", model, bwd, minb, shard, loss), ("fast", model, bwd), ("fwd",), ("bwd",), ("shard_fwd",) or
-    ("shard_bwd",) for a fused-step kernel's (demangled or mangled) name; None for any other kernel."""
-    m = _DEMANGLED.search(name)
-    if m:
-        args = [] if m.group(2) is None else [a.strip() for a in m.group(2).split(",")]
-        args = [a == "true" if a in ("true", "false") else int(re.sub(r"^\(\w+\)", "", a)) for a in args]
-    else:
-        m = _MANGLED.search(name)
-        if not m:
-            return None
-        args = [bool(int(v)) if k == "b" else int(v) for k, v in re.findall(r"L([ib])(\d+)E", m.group(2) or "")]
-    return (m.group(1),) + tuple(args)
-
-
-def _cuda_kernel_names(fn):
-    with torch.profiler.profile(activities=[torch.profiler.ProfilerActivity.CUDA]) as prof:
-        torch.cuda.synchronize()
-        fn()
-        torch.cuda.synchronize()
-    return [e.name for e in prof.events() if e.device_type == torch.autograd.DeviceType.CUDA]
-
-
-def launched(fn, expected, tries=4):
-    """The set of fused-step kernel signatures that ran on the GPU while fn() ran.  torch.profiler now and
-    then leaves a kernel out of its record, so fn (which must be repeatable) runs up to `tries` times
-    under it until every expected kernel has been seen; the union is returned, so a kernel that should
-    not run still shows."""
-    ran, names = set(), []
-    for _ in range(tries):
-        names = _cuda_kernel_names(fn)
-        ran |= {s for s in map(kernel_signature, names) if s is not None}
-        if ran >= expected:
-            break
-    if not ran:
-        control = _cuda_kernel_names(lambda: torch.ones(4, device=DEV).add_(1))
-        if not control:
-            pytest.fail("torch.profiler records no CUDA kernels here, not even torch's own: the kernel each "
-                        "step runs cannot be checked")
-        if not names:
-            pytest.fail("torch.profiler recorded a torch kernel but none while the fused step ran")
-    return ran
 
 
 def test_kernel_signature_parses_both_name_forms():
@@ -173,11 +108,15 @@ def test_kernel_signature_parses_both_name_forms():
                             "StepParamsENS_10TrainGradsEPKf") == ("ring", 1, False, 0, True, 2)
     assert kernel_signature("_ZN3kge12_GLOBAL__N_128margin_step_shard_bwd_kernelENS_16MarginStepParamsE") == \
         ("shard_bwd",)
+    assert kernel_signature(ns + "margin_step_ring_rel_kernel<1, true, false, 2>(kge::MarginStepParams, "
+                            "kge::TrainGrads, float const*)") == ("ring_rel", 1, True, False, 2)
+    assert kernel_signature("_ZN3kge12_GLOBAL__N_127margin_step_ring_pos_kernelILi0ELb0ELb1ELi1EEEvNS_16Margin"
+                            "StepParamsENS_10TrainGradsEPKfNS_6PosCSRE") == ("ring_pos", 0, False, True, 1)
     assert kernel_signature("void at::native::vectorized_elementwise_kernel<4>(int)") is None
 
 
 # ---------------------------------------------------------------- data and the float64 reference
-KINDS = tuple(FAST_KINDS)
+KINDS = tuple(kit.FAST_KINDS)
 DIMS = (36, 200, 256)
 N_ENT, N_REL = 1500, 11
 SEED, OFFSET = 4099, 7
@@ -190,59 +129,31 @@ def boundaries(dim):
     return (a, a + 1, b, b + 1)
 
 
-def draw(h, t, r, probs, n_neg):
-    """kge_corrupt_batch's negatives: the ones every fused kernel draws at (SEED, OFFSET)."""
-    nh = torch.empty(h.shape[0] * n_neg, dtype=torch.int64, device=DEV)
-    nt = torch.empty_like(nh)
-    _lib.check(_lib.load().kge_corrupt_batch(_ptr(h), _ptr(t), _ptr(r), h.shape[0], n_neg, _ptr(probs), N_ENT, SEED,
-                                             OFFSET, _ptr(nh), _ptr(nt), _stream(h.device)), "kge_corrupt_batch")
-    return nh, nt
-
-
 def problem(kind, dim, n_neg, source, seed):
     """A model, a batch of 23 positives (the last block holds three warps) on the GPU, Bernoulli
-    probabilities and the negatives: external ones (helpers.negatives) or the kernel's own draws."""
-    model = helpers.train_model(kind, dim, N_ENT, N_REL, seed=seed)
+    probabilities and the negatives: external ones (train_kit.negatives) or the kernel's own draws."""
+    model = kit.train_model(kind, dim, N_ENT, N_REL, seed=seed)
     gen = torch.Generator().manual_seed(seed + n_neg)
-    b = 23
-    h, t = torch.randint(0, N_ENT, (b,), generator=gen), torch.randint(0, N_ENT, (b,), generator=gen)
-    r = torch.randint(0, N_REL, (b,), generator=gen)
-    probs = torch.rand(N_REL, generator=gen)
-    h, t, r, probs = h.to(DEV), t.to(DEV), r.to(DEV), probs.to(DEV)
+    h, t, r, probs = kit.batch(N_ENT, N_REL, 23, gen)
     if source == "external":
-        nh, nt = helpers.negatives(h.cpu(), t.cpu(), N_ENT, n_neg, gen)
-        nh, nt = nh.to(DEV), nt.to(DEV)
+        nh, nt = (x.to(DEV) for x in kit.negatives(h.cpu(), t.cpu(), N_ENT, n_neg, gen))
     else:
-        nh, nt = draw(h, t, r, probs, n_neg)
+        nh, nt = kit.corrupt_batch(h, t, r, probs, n_neg, N_ENT, SEED, OFFSET)
     return model, h, t, r, probs, nh, nt
 
 
-def margin_between(diff, q=0.5):
-    """A float32 margin m in the widest gap between neighbouring values of pos - neg near its q-quantile:
-    about half the hinges are active, and none lies so close to its kink that float32 and float64 could
-    disagree on whether it is."""
-    s = torch.sort(diff.detach().flatten()).values
-    k = int(q * (s.shape[0] - 1))
-    w = min(200, s.shape[0] // 4)
-    if w == 0:
-        return float(torch.tensor(float(s[0]) + 0.5, dtype=torch.float32))
-    lo, hi = k - w, k + w
-    i = lo + int(torch.argmax(s[lo + 1:hi + 1] - s[lo:hi]))
-    return float(torch.tensor(float(s[i] + s[i + 1]) / 2, dtype=torch.float32))
-
-
-def reference(kind, ts, h, t, r, nh, nt, loss):
-    """float64 CPU autograd of the oracle's scores on copies of the kernel's leaves:
-    (loss, [grads], pos, neg, margin); the margin is chosen here (margin_between)."""
-    cpu = helpers.cpu_leaves(ts, torch.float64)
-    pos, neg = helpers.cpu_pos_neg(kind, cpu, h.cpu(), t.cpu(), r.cpu(), nh.cpu(), nt.cpu())
-    margin = margin_between(pos - neg) if loss == "margin" else 0.0
+def reference_with_margin(kind, model, h, t, r, nh, nt, loss):
+    """train_kit.reference on the model's leaves, (loss, [grads], pos, neg, margin), with the margin chosen
+    here (margin_between) so that between 5 and 95 % of the hinges are active."""
+    ts = kit.train_leaves(model)[2]
+    margin = 0.0
     if loss == "margin":
+        pos, neg = kit.cpu_pos_neg(kind, kit.cpu_leaves(ts, torch.float64), h.cpu(), t.cpu(), r.cpu(), nh.cpu(),
+                                   nt.cpu())
+        margin = kit.margin_between(pos - neg)
         active = float(((margin - pos + neg) > 0).double().mean())
         assert 0.05 <= active <= 0.95, active
-    want = helpers.torch_loss(loss, pos, neg, margin)
-    want.backward()
-    return want.item(), [None if x is None else x.grad for x in cpu], pos.detach(), neg.detach(), margin
+    return kit.reference(kind, ts, h, t, r, nh, nt, loss, margin) + (margin,)
 
 
 def assert_matches_reference(got_loss, got_grads, want_loss, want_grads, h, t):
@@ -251,10 +162,10 @@ def assert_matches_reference(got_loss, got_grads, want_loss, want_grads, h, t):
     assert got_loss == pytest.approx(want_loss, rel=2e-5)
     for a, c in zip(got_grads, want_grads):
         if c is not None:
-            helpers.close_grad(a, c, rtol=2e-4)
+            kit.close_grad(a, c, rtol=2e-4)
     only_neg = torch.ones(N_ENT, dtype=torch.bool)
     only_neg[torch.cat([h, t]).cpu()] = False
-    helpers.close_grad(got_grads[0].cpu()[only_neg], want_grads[0][only_neg], rtol=2e-4)
+    kit.close_grad(got_grads[0].cpu()[only_neg], want_grads[0][only_neg], rtol=2e-4)
 
 
 def _unsharded_cases():
@@ -275,23 +186,17 @@ UNSHARDED = _unsharded_cases()
 @pytest.mark.parametrize("kind,d,n_neg,loss", UNSHARDED, ids=["%s-d%d-neg%d-%s" % c for c in UNSHARDED])
 def test_step_matches_float64_autograd(kind, d, n_neg, loss, source):
     model, h, t, r, probs, nh, nt = problem(kind, d, n_neg, source, seed=d + 3)
-    code, dim, ts = helpers.train_leaves(model)
-    want_loss, want_grads, _, _, margin = reference(kind, ts, h, t, r, nh, nt, loss)
-    lk = helpers.LOSS_KINDS[loss]
+    want_loss, want_grads, _, _, margin = reference_with_margin(kind, model, h, t, r, nh, nt, loss)
+    negs = dict(negatives=(nh, nt)) if source == "external" else dict(n_neg=n_neg, probs=probs, seed=SEED,
+                                                                      offset=OFFSET)
 
-    def step(leaves):
-        if source == "external":
-            got = _MarginStep.apply(code, dim, N_ENT, margin, n_neg, h, t, r, nh, nt, None, 0, 0, *leaves, lk)
-        else:
-            got = _MarginStep.apply(code, dim, N_ENT, margin, n_neg, h, t, r, None, None, probs, SEED, OFFSET,
-                                    *leaves, lk)
-        got.backward()
-        return got.item()
+    def step():
+        return kit.whole_table_step(model, h, t, r, loss=loss, margin=margin, **negs)
 
-    got = step(ts)
-    assert_matches_reference(got, [None if x is None else x.grad for x in ts], want_loss, want_grads, h, t)
+    got, grads = step()
+    assert_matches_reference(got, grads, want_loss, want_grads, h, t)
     expected = expected_kernels(kind, d, n_neg, loss, shard=False)
-    assert launched(lambda: step(helpers.train_leaves(model)[2]), expected) == expected
+    assert launched(step, expected) == expected
 
 
 # ---------------------------------------------------------------- 3. optional outputs
@@ -308,25 +213,17 @@ def test_optional_outputs(kind, route, source):
     d = 200
     n_neg = boundaries(d)[which]
     model, h, t, r, probs, nh, nt = problem(kind, d, n_neg, source, seed=17)
-    code, dim, ts = helpers.train_leaves(model)
-    want_loss, _, pos, neg, margin = reference(kind, ts, h, t, r, nh, nt, loss)
+    want_loss, _, pos, neg, margin = reference_with_margin(kind, model, h, t, r, nh, nt, loss)
     b = h.shape[0]
-    tabs = [None if x is None else x.detach() for x in ts]
-    pos_out, neg_out = torch.full((b,), float("nan"), device=DEV), torch.full((b * n_neg,), float("nan"), device=DEV)
-    ids = [torch.full((b * n_neg,), -1, dtype=torch.int64, device=DEV) for _ in range(2)]
-    out = torch.zeros((), device=DEV)
-    ext = source == "external"
-    a = _MarginStep._args(code, dim, N_ENT, margin, n_neg, h, t, r, nh if ext else None, nt if ext else None,
-                          probs, SEED, OFFSET, tabs, out, h.device, helpers.LOSS_KINDS[loss])
-    a.pos_out, a.neg_out, a.nh_out, a.nt_out = _ptr(pos_out), _ptr(neg_out), _ptr(ids[0]), _ptr(ids[1])
-    assert _lib.load().kge_margin_step_fwd(ctypes.byref(a)) == 0
-    torch.cuda.synchronize()
-    assert torch.equal(ids[0], nh) and torch.equal(ids[1], nt)
-    torch.testing.assert_close(pos_out.cpu().double(), pos[:b], rtol=1e-5, atol=1e-6)
-    torch.testing.assert_close(neg_out.cpu().double(), neg, rtol=1e-5, atol=1e-6)
-    assert out.item() == pytest.approx(want_loss, rel=2e-5)
+    kw = dict(n_neg=n_neg, loss=loss, margin=margin, probs=probs, seed=SEED, offset=OFFSET,
+              negatives=(nh, nt) if source == "external" else None)
+    out = kit.forward_outputs(model, h, t, r, **kw)
+    assert torch.equal(out["nh"], nh) and torch.equal(out["nt"], nt)
+    torch.testing.assert_close(out["pos"].cpu().double(), pos[:b], rtol=1e-5, atol=1e-6)
+    torch.testing.assert_close(out["neg"].cpu().double(), neg, rtol=1e-5, atol=1e-6)
+    assert out["loss"].item() == pytest.approx(want_loss, rel=2e-5)
     expected = forward_of(expected_kernels(kind, d, n_neg, loss, shard=False))
-    assert launched(lambda: _lib.load().kge_margin_step_fwd(ctypes.byref(a)), expected) == expected
+    assert launched(lambda: kit.forward_outputs(model, h, t, r, **kw), expected) == expected
 
 
 # ---------------------------------------------------------------- 4. sharded, at the boundaries
@@ -337,23 +234,21 @@ SHARDED = ([(k, d, boundaries(d)[i], "margin") for k in KINDS for d in DIMS for 
 @pytest.mark.gpu
 @pytest.mark.parametrize("kind,d,n_neg,loss", SHARDED, ids=["%s-d%d-neg%d-%s" % c for c in SHARDED])
 def test_sharded_step_matches_unsharded_and_float64_autograd(kind, d, n_neg, loss):
-    """Emulated shards (helpers.emulated: every rank's kernels on its row range, the all-reduces as sums)."""
+    """Emulated shards (train_kit.emulated: every rank's kernels on its row range, the all-reduces as sums)."""
     model, h, t, r, probs, nh, nt = problem(kind, d, n_neg, "drawn", seed=d + 5)
-    _, _, ts = helpers.train_leaves(model)
-    want_loss, want_grads, _, _, margin = reference(kind, ts, h, t, r, nh, nt, loss)
-    lk = helpers.LOSS_KINDS[loss]
-    one_loss, one_grads = helpers.unsharded(model, h, t, r, probs, margin, n_neg, SEED, OFFSET, lk)
+    want_loss, want_grads, _, _, margin = reference_with_margin(kind, model, h, t, r, nh, nt, loss)
+    kw = dict(n_neg=n_neg, probs=probs, loss=loss, margin=margin, seed=SEED, offset=OFFSET)
+    one_loss, one_grads = kit.whole_table_step(model, h, t, r, **kw)
     eng = CudaEngine()
     expected = expected_kernels(kind, d, n_neg, loss, shard=True)
     for world in (1, 3, 8):
-        got_loss, got_grads = helpers.emulated(model, h, t, r, probs, margin, n_neg, SEED, OFFSET, world, eng, lk)
+        got_loss, got_grads = kit.emulated(model, h, t, r, world, eng, **kw)
         assert got_loss == pytest.approx(one_loss, rel=1e-5, abs=1e-6)
         for a, c in zip(got_grads, one_grads):
             if c is not None:
-                helpers.close_grad(a, c, rtol=1e-4)
+                kit.close_grad(a, c, rtol=1e-4)
         assert_matches_reference(got_loss, got_grads, want_loss, want_grads, h, t)
-        ran = launched(lambda: helpers.emulated(model, h, t, r, probs, margin, n_neg, SEED, OFFSET, world, eng, lk),
-                       expected)
+        ran = launched(lambda: kit.emulated(model, h, t, r, world, eng, **kw), expected)
         assert ran == expected, world
 
 
@@ -368,12 +263,5 @@ def test_environment_variants(switch):
     if any(v in os.environ for v in SWITCHES):
         pytest.skip("runs in the parent process only (%s is set here)" % ", ".join(v for v in SWITCHES
                                                                                 if v in os.environ))
-    name, value = switch.split("=")
-    env = dict(os.environ, **{name: value})
-    cmd = [sys.executable] + (["-s"] if sys.flags.no_user_site else []) + \
-        ["-m", "pytest", "-q", "-p", "no:cacheprovider", os.path.abspath(__file__)]
-    start = time.time()
-    proc = subprocess.run(cmd, cwd=ROOT, env=env, capture_output=True, text=True, timeout=1200)
-    print("%s: %.0f s\n%s" % (switch, time.time() - start, proc.stdout[-600:]))
-    assert proc.returncode == 0, "%s\n%s\n%s" % (switch, proc.stdout[-6000:], proc.stderr[-3000:])
-    assert " passed" in proc.stdout and " skipped" in proc.stdout, proc.stdout[-2000:]
+    out = kit.rerun(__file__, switch)
+    assert " skipped" in out, out[-2000:]

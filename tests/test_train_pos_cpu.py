@@ -4,33 +4,16 @@ scored by the rank holding the entity it draws; the ranks' sums give the unshard
 agreement tells the positional step from the entity step and compares the candidate CSRs' sizes), the
 argument errors raised before any collective or kernel, the argument rules of kge_pos_step_* in a child
 process that sees no GPU, and kge_pos_step_args_t against its binding."""
-import json
-import os
-import re
-import subprocess
-import sys
-
 import pytest
 import torch
 
 import torchkge_b200 as tk
-from oracle import kge_oracle as oracle
 from tests import gloo, helpers
-from tests.test_train_loss_sharding_gloo import pair_loss
-from tests.test_train_sharding_gloo import _ENT_KEYS, _KIND_OF_CODE, _REL_KEYS, CountingShard, OracleStepEngine, \
-    _local_model
+from tests.train_kit import (CountingShard, OracleStepEngine, csr, every_rank_ok, grads_match, header_fields,
+                             malformed_calls, oracle_loss, stand_in_pos_draws)
 from torchkge_b200 import _lib
 from torchkge_b200.engine import EntityShard, QueryShard
 from torchkge_b200.training import fused_loss_step, fused_margin_step, sharded_margin_step
-
-ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
-
-
-def csr(rel, ent, n_rel, n_ent):
-    key = torch.unique(rel * n_ent + ent)
-    offs = torch.zeros(n_rel + 1, dtype=torch.int64)
-    offs[1:] = torch.cumsum(torch.bincount(key // n_ent, minlength=n_rel), 0)
-    return offs, key % n_ent
 
 
 def positional_of(n_ent, n_rel, seed, n=40):
@@ -40,68 +23,21 @@ def positional_of(n_ent, n_rel, seed, n=40):
     return csr(rel, hd, n_rel, n_ent) + csr(rel, tl, n_rel, n_ent)
 
 
-def pos_draws(seed, offset, r, n_neg, probs, n_ent, pos):
-    """The stand-in's positional draws: (head?, replacement), a function of (seed, offset), the CSR and n_ent."""
-    g = torch.Generator().manual_seed((seed * 1000003 + offset) % (1 << 62))
-    n = n_neg * r.shape[0]
-    u, v = torch.rand(n, generator=g), torch.rand(n, generator=g)
-    R = r.repeat(n_neg)
-    head = u < probs[R]
-    ho, he, to, te = pos
-    lo = torch.where(head, ho[R], to[R])
-    cnt = torch.where(head, ho[R + 1] - ho[R], to[R + 1] - to[R])
-    k = (v * cnt).long().clamp(max=(cnt - 1).clamp(min=0))
-    pick = lo + k
-    hv = he[pick.clamp(max=max(he.numel() - 1, 0))] if he.numel() else torch.zeros_like(pick)
-    tv = te[pick.clamp(max=max(te.numel() - 1, 0))] if te.numel() else torch.zeros_like(pick)
-    e = torch.where(cnt > 0, torch.where(head, hv, tv), (v * n_ent).long().clamp(max=n_ent - 1))
-    return head, e
-
-
-class PosStepEngine(OracleStepEngine):
-    """The stand-in engine of a positional step: a negative on the rank holding its drawn entity."""
-
-    def _partial(self, step, tables, h, t, r, probs, hrows, trows, grad):
-        assert step.pos is not None and step.n_rel == 0
-        kind = _KIND_OF_CODE[step.code]
-        b, n = h.shape[0], step.n_rows
-        ent = [x for x in tables[:2] if x is not None]
-        P = {}
-        for p, key in enumerate(_ENT_KEYS[kind]):
-            P[key] = torch.cat([ent[p], hrows[:, p], trows[:, p]]).clone().requires_grad_(grad)
-        for p, key in enumerate(_REL_KEYS[kind]):
-            P[key] = tables[2 + p].clone().requires_grad_(grad)
-        head, e = pos_draws(step.seed, step.offset, r, step.n_neg, probs, step.n_ent, step.pos)
-        own = (e >= step.ent_lo) & (e < step.ent_lo + n)
-        i = torch.arange(b).repeat(step.n_neg)[own]
-        loc, head = e[own] - step.ent_lo, head[own]
-        nh = torch.where(head, loc, n + i)
-        nt = torch.where(head, n + b + i, loc)
-        pos = oracle.score_triples(kind, P, n + i, n + b + i, r[i])
-        neg = oracle.score_triples(kind, P, nh, nt, r[i])
-        return pair_loss(step.loss_kind, pos, neg), P
-
-
 def _reference(kind, loss_kind, model, h, t, r, probs, seed, offset, n_neg, n_ent, pos):
-    P = {k: v.requires_grad_(True) for k, v in helpers.oracle_params(kind, model).items()}
-    head, e = pos_draws(seed, offset, r, n_neg, probs, n_ent, pos)
+    head, e = stand_in_pos_draws(seed, offset, r, n_neg, probs, n_ent, pos)
     nh = torch.where(head, e, h.repeat(n_neg))
     nt = torch.where(head, t.repeat(n_neg), e)
-    p = oracle.score_triples(kind, P, h, t, r).repeat(n_neg)
-    neg = oracle.score_triples(kind, P, nh, nt, r.repeat(n_neg))
-    loss = pair_loss(loss_kind, p, neg)
-    loss.backward()
-    return loss.item(), {k: v.grad for k, v in P.items()}
+    return oracle_loss(kind, loss_kind, model, h, t, r, nh, nt)
 
 
 def _run(rank, world, kind, loss_kind, n_ent, b, n_neg):
     n_rel, dim = 5, 8
     model = helpers.make_model(kind, dim, n_ent, n_rel, seed=31)
     shard = CountingShard(n_ent, rank, world, None, local_storage=True)
-    local = _local_model(kind, model, shard.lo, shard.hi, n_rel, dim)
+    local = helpers.local_model(kind, model, shard.lo, shard.hi, n_rel, dim)
     probs = torch.tensor([0.5, 1.0, 0.0, 0.3, 0.8])
     pos = positional_of(n_ent, n_rel, seed=2)
-    eng = PosStepEngine()
+    eng = OracleStepEngine()
     g = torch.Generator().manual_seed(100)
     h, t = torch.randint(0, n_ent, (b,), generator=g), torch.randint(0, n_ent, (b,), generator=g)
     r = torch.randint(0, n_rel, (b,), generator=g)
@@ -110,14 +46,7 @@ def _run(rank, world, kind, loss_kind, n_ent, b, n_neg):
     loss.backward()
     want_loss, want = _reference(kind, loss_kind, model, h, t, r, probs, 7, 1, n_neg, n_ent, pos)
     ok = {"loss": abs(loss.item() - want_loss) <= 1e-5 * max(1.0, abs(want_loss))}
-    names = dict(zip(_ENT_KEYS[kind], ("ent_emb.weight",) if kind != "complex" else
-                     ("re_ent_emb.weight", "im_ent_emb.weight")))
-    names.update(zip(_REL_KEYS[kind], ("rel_emb.weight",) if kind != "complex" else
-                     ("re_rel_emb.weight", "im_rel_emb.weight")))
-    params = dict(local.named_parameters())
-    for key, name in names.items():
-        ref = want[key][shard.lo:shard.hi] if "ent" in key else want[key]
-        ok[key] = torch.allclose(params[name].grad, ref, rtol=1e-4, atol=1e-6)
+    ok.update(grads_match(kind, local, want, shard))
     # the entity step's collectives, plus one for the CSR sizes
     ok["collectives"] = [c[0] for c in shard.collectives] == ["stack_all", "stack_all", "all_reduce", "all_reduce",
                                                                "all_reduce"]
@@ -130,7 +59,8 @@ def _worker(rank, world, case):
     try:
         if case[0] in ("csr", "kind"):
             shard = EntityShard.from_group(30, local_storage=True)
-            model = _local_model("distmult", helpers.make_model("distmult", 8, 30, 4, seed=1), shard.lo, shard.hi, 4, 8)
+            whole = helpers.make_model("distmult", 8, 30, 4, seed=1)
+            model = helpers.local_model("distmult", whole, shard.lo, shard.hi, 4, 8)
             h = torch.arange(5)
             pos = positional_of(30, 4, seed=3, n=40 if rank == 0 else 41)
             if case[0] == "kind" and rank == 1:
@@ -157,13 +87,7 @@ CASES = [
 
 @pytest.mark.parametrize("case", CASES, ids=["%s-loss%d-w%d" % (c[1], c[2], c[0]) for c in CASES])
 def test_sharded_pos_step_equals_oracle(case):
-    world = case[0]
-    ret = gloo.spawn(world, _worker, case[1:])
-    for rank in range(world):
-        res = ret[rank]
-        assert "error" not in res, "rank %d: %s" % (rank, res.get("error"))
-        bad = [k for k, v in res.items() if not v]
-        assert not bad, "rank %d: %s" % (rank, bad)
+    every_rank_ok(gloo.spawn(case[0], _worker, case[1:]), case[0])
 
 
 @pytest.mark.parametrize("what", ["csr", "kind"])
@@ -214,21 +138,8 @@ def test_argument_errors():
 
 
 _ABI_CHILD = r"""
-import ctypes, json, sys
-sys.path.insert(0, sys.argv[1])
-from torchkge_b200 import _lib
-lib = _lib.load()
-F = 8   # a non-NULL stand-in pointer: every call below fails its checks before touching memory
-res = {}
-def ok_args():
-    a = _lib.PosStepArgs()
-    b = a.base
-    b.tb.model, b.tb.dim, b.tb.ent0, b.tb.rel0 = _lib.DISTMULT, 8, F, F
-    b.n_neg, b.b, b.n_ent, b.h, b.t, b.r, b.bern_probs, b.loss = 2, 4, 10, F, F, F, F, F
-    a.n_rel, a.head_offs, a.head_ents, a.tail_offs, a.tail_ents = 5, F, F, F, F
-    return a
-g = _lib.Grads(F, None, F, None)
-cases = {
+fields = dict(n_rel=5, head_offs=F, head_ents=F, tail_offs=F, tail_ents=F)
+step_cases(_lib.PosStepArgs, fields, lib.kge_pos_step_fwd, lib.kge_pos_step_bwd, {
     "null": lambda a: None,
     "n_rel_0": lambda a: setattr(a, "n_rel", 0),
     "no_head_offs": lambda a: setattr(a, "head_offs", None),
@@ -242,36 +153,16 @@ cases = {
                                  setattr(a.base, "nt_out", F)),
     "sharded_rows_past_n_ent": lambda a: (setattr(a.base, "hrows", F), setattr(a.base, "trows", F),
                                           setattr(a.base, "n_rows", 11)),
-}
-for name, edit in cases.items():
-    a = ok_args()
-    edit(a)
-    p = None if name == "null" else ctypes.byref(a)
-    res["fwd_" + name] = lib.kge_pos_step_fwd(p)
-    res["bwd_" + name] = lib.kge_pos_step_bwd(p, ctypes.byref(g), F)
-a = ok_args()
-res["bwd_no_grad_loss"] = lib.kge_pos_step_bwd(ctypes.byref(a), ctypes.byref(g), None)
-res["bwd_no_grads"] = lib.kge_pos_step_bwd(ctypes.byref(a), None, F)
-a.base.hrows, a.base.trows, a.base.n_rows = F, F, 10
-res["bwd_sharded_no_grad_rows"] = lib.kge_pos_step_bwd(ctypes.byref(a), ctypes.byref(g), F)
-print(json.dumps(res))
+})
 """
 
 
 def test_entry_points_reject_malformed_calls_without_a_gpu():
-    env = dict(os.environ, CUDA_VISIBLE_DEVICES="")
-    proc = subprocess.run([sys.executable, "-c", _ABI_CHILD, ROOT], env=env, capture_output=True, text=True,
-                          timeout=300)
-    assert proc.returncode == 0, proc.stderr[-3000:]
-    res = json.loads(proc.stdout.strip().splitlines()[-1])
+    res = malformed_calls(_ABI_CHILD)
     assert res == {k: 1 for k in res}    # KGE_ERR_ARG
 
 
 def test_pos_step_struct_matches_the_header_in_order():
     """kge_pos_step_args_t in include/kge_b200.h, field by field, is _lib.PosStepArgs."""
-    header = re.sub(r"/\*.*?\*/", "", open(os.path.join(ROOT, "include", "kge_b200.h")).read(), flags=re.S)
-    body = re.search(r"typedef struct \{([^{}]*)\}\s*kge_pos_step_args_t\s*;", header, flags=re.S).group(1)
-    names = [re.findall(r"[A-Za-z_][A-Za-z0-9_]*", part)[-1]
-             for decl in body.split(";") if decl.strip() for part in decl.split(",")]
-    assert names == [n for n, _ in _lib.PosStepArgs._fields_]
+    assert header_fields("kge_pos_step_args_t") == [n for n, _ in _lib.PosStepArgs._fields_]
     assert _lib.PosStepArgs._fields_[0] == ("base", _lib.MarginStepArgs)

@@ -9,7 +9,7 @@ import torch
 import torchkge_b200 as tk
 from tests import helpers
 from tests.shard_threads import run_ranks, thread_collectives
-from tests.test_relpred_shard_gpu import STORAGES, local_model, make_shard
+from tests.test_relpred_shard_gpu import STORAGES, make_shard
 from torchkge_b200.engine import EntityShard
 
 DEV = "cuda:0"
@@ -51,7 +51,7 @@ def test_scores_thresholds_accuracy_equal_unsharded(kind, monkeypatch):
         for storage in STORAGES:
             def rank_fn(rank, group):
                 shard = make_shard(storage, rank, world, group, n_ent, kg_test.n_facts)
-                m = local_model(kind, model, shard.lo, shard.hi, n_rel, dim) if storage == "local" else model
+                m = helpers.local_model(kind, model, shard.lo, shard.hi, n_rel, dim) if storage == "local" else model
                 ev = tk.TripletClassificationEvaluator(m, kg_val, kg_test, shard=shard)
                 ev.sampler = sampler(kg_val, kg_test, 900 + 13 * rank)      # seeded differently
                 pos = ev.get_scores(kg_test.head_idx, kg_test.tail_idx, kg_test.relations, 100)
@@ -87,7 +87,7 @@ def test_empty_shards_and_fewer_facts_than_ranks(monkeypatch):
         for storage in STORAGES:
             def rank_fn(rank, group):
                 shard = make_shard(storage, rank, 8, group, n_ent, kg_test.n_facts)
-                m = local_model(kind, model, shard.lo, shard.hi, n_rel, dim) if storage == "local" else model
+                m = helpers.local_model(kind, model, shard.lo, shard.hi, n_rel, dim) if storage == "local" else model
                 ev = tk.TripletClassificationEvaluator(m, kg_val, kg_test, shard=shard)
                 ev.sampler = sampler(kg_val, kg_test, 5 + rank)
                 s = ev.get_scores(h, t, r, 3)
@@ -107,7 +107,7 @@ def test_argument_errors_before_any_collective(monkeypatch):
     ev = tk.TripletClassificationEvaluator(model, kg_val, kg_test, shard=EntityShard(40, 0, 2, local_storage=True))
     with pytest.raises(ValueError, match="should hold 20 entity rows"):
         ev.evaluate(b_size=64)
-    part = local_model("distmult", model, 0, 20, 3, 8)
+    part = helpers.local_model("distmult", model, 0, 20, 3, 8)
     ev = tk.TripletClassificationEvaluator(part, kg_val, kg_test, shard=EntityShard(40, 0, 2))
     with pytest.raises(ValueError, match="should hold 40 entity rows"):
         ev.accuracy(b_size=64)
@@ -115,7 +115,7 @@ def test_argument_errors_before_any_collective(monkeypatch):
     from torchkge_b200.models import l1_dissimilarity
     tor.dissimilarity = l1_dissimilarity            # plain L1 on fractional parts: no per-triple kernel
     tor = tor.to(DEV)
-    part = local_model("toruse_l1", tor, 0, 20, 3, 8)
+    part = helpers.local_model("toruse_l1", tor, 0, 20, 3, 8)
     part.dissimilarity = l1_dissimilarity
     ev = tk.TripletClassificationEvaluator(part, kg_val, kg_test, shard=EntityShard(40, 0, 2, local_storage=True))
     with pytest.raises(NotImplementedError):
