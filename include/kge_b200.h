@@ -495,6 +495,19 @@ typedef struct {
 int kge_pos_step_fwd(const kge_pos_step_args_t* a);
 int kge_pos_step_bwd(const kge_pos_step_args_t* a, const kge_grads_t* g, const float* grad_loss);
 
+/* ---- data redundancy (torchkge/utils/data_redundancy.py: duplicates, count_triplets) ------------------
+ * kge_cooccurrence: relation co-occurrence counts over two sets of facts.  Each side is a sorted array of
+ * distinct keys (h * n_ent + t) * n_rel + r, cut into segments of equal (h, t): segment s holds keys
+ * [offs[s], offs[s+1]) and pairs[s] = h * n_ent + t, ascending in s.  For every left segment (h, t) whose
+ * partner -- the right segment of (h, t), or of (t, h) when flip != 0 -- exists, every key r_a of the left
+ * segment and r_b of the partner add 1 to counts[r_a * n_rel + r_b] (n_rel x n_rel, uint64, zeroed by the
+ * caller); upper != 0 keeps only r_a < r_b.  So counts[a][b] = |{(h, t) of a} & {(h, t) of b}|, or with
+ * flip = |{(h, t) of a} & {(t, h) of b}|, self-loops included.  Arguments: n_ent >= 1, n_rel >= 1, every
+ * pointer non-NULL; the caller guarantees the key layout above.  n_left == 0 or n_right == 0 is a no-op. */
+int kge_cooccurrence(const int64_t* left_keys, const int64_t* left_offs, const int64_t* left_pairs, int64_t n_left,
+                     const int64_t* right_keys, const int64_t* right_offs, const int64_t* right_pairs, int64_t n_right,
+                     int64_t n_ent, int64_t n_rel, int flip, int upper, uint64_t* counts, void* stream);
+
 /* ---- measurement hook ------------------------------------------------------------------
  * When enabled, the dominant kernels of kge_rank_side / kge_score_all are bracketed by CUDA
  * events recorded on the launch stream: kind 0 = scalar dense scan, 1 = tensor-core scan,

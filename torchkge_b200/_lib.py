@@ -163,6 +163,8 @@ SIGNATURES = {
     "kge_rel_step_bwd": (_c.c_int, [_c.POINTER(RelStepArgs), _c.POINTER(Grads), _p]),
     "kge_pos_step_fwd": (_c.c_int, [_c.POINTER(PosStepArgs)]),
     "kge_pos_step_bwd": (_c.c_int, [_c.POINTER(PosStepArgs), _c.POINTER(Grads), _p]),
+    "kge_cooccurrence": (_c.c_int, [_p, _p, _p, _c.c_int64, _p, _p, _p, _c.c_int64, _c.c_int64, _c.c_int64,
+                                    _c.c_int, _c.c_int, _p, _p]),
     "kge_scan_timing_enable": (_c.c_int, [_c.c_int]),
     "kge_scan_timing_read": (_c.c_int, [_c.c_int, _c.POINTER(_c.c_int64), _c.POINTER(_c.c_double)]),
 }

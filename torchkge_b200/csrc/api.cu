@@ -776,6 +776,23 @@ int kge_topk_dense(const float* scores, int64_t n, int64_t n_cand, int k, const 
   return KGE_OK;
 }
 
+int kge_cooccurrence(const int64_t* left_keys, const int64_t* left_offs, const int64_t* left_pairs, int64_t n_left,
+                     const int64_t* right_keys, const int64_t* right_offs, const int64_t* right_pairs, int64_t n_right,
+                     int64_t n_ent, int64_t n_rel, int flip, int upper, uint64_t* counts, void* stream) {
+  if (n_left == 0 || n_right == 0) return KGE_OK;
+  if (n_left < 0 || n_right < 0 || n_ent < 1 || n_rel < 1)
+    return fail(KGE_ERR_ARG, "kge_cooccurrence", "bad sizes");
+  if (!left_keys || !left_offs || !left_pairs || !right_keys || !right_offs || !right_pairs || !counts)
+    return fail(KGE_ERR_ARG, "kge_cooccurrence", "null pointer");
+  DeviceScope device_scope(counts);
+  KGE_CUDA_TRY(kge::launch_cooccurrence(left_keys, left_offs, left_pairs, n_left, right_keys, right_offs, right_pairs,
+                                        n_right, n_ent, n_rel, flip != 0, upper != 0,
+                                        reinterpret_cast<unsigned long long*>(counts),
+                                        static_cast<cudaStream_t>(stream)),
+               "cooccurrence");
+  return KGE_OK;
+}
+
 // ------------------------------------ training side ------------------------------------
 namespace {
 bool tables_ok(const kge_tables_t* tb) {

@@ -164,4 +164,12 @@ cudaError_t launch_rank_dense(const float* scores, int64_t n, int64_t n_c, const
                               int32_t* raw_count, int32_t* filt_sub, float* true_score_out, cudaStream_t stream);
 cudaError_t launch_dense_to_pairs(const float* scores, int64_t n, int64_t n_c, int2* pairs, cudaStream_t stream);
 
+// ---- relation co-occurrence of the data-redundancy analysis (redundancy.cu) ----
+// counts[r_a * n_rel + r_b] += 1 for every key r_a of a left segment and r_b of the right segment with the
+// same (h, t) pair, or (t, h) when flip; upper: only r_a < r_b
+cudaError_t launch_cooccurrence(const int64_t* lkeys, const int64_t* loffs, const int64_t* lpairs, int64_t n_left,
+                                const int64_t* rkeys, const int64_t* roffs, const int64_t* rpairs, int64_t n_right,
+                                int64_t n_ent, int64_t n_rel, bool flip, bool upper, unsigned long long* counts,
+                                cudaStream_t stream);
+
 }  // namespace kge
