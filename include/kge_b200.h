@@ -318,6 +318,14 @@ int kge_topk_merge(const int64_t* pred_in, const float* scores_in, int n_lists, 
  * kge_rank_dense / kge_topk_dense consume. */
 int kge_rescal_rel_scores(const float* hrows, const float* trows, const float* rel_mat, int dim, int64_t n,
                           int64_t n_rel, float* scores, void* stream);
+/* TransH relation prediction (models/interfaces.py:261-272 with the projections of
+ * models/translation.py:253-254): scores[i][c] = -||(P_c(h_i) + r_c) - P_c(t_i)||^2, where
+ * P_c(e) = e - (e . w_c) w_c is computed as kge_transh_project computes it and the norm is summed in
+ * ATen's L2-norm order.  hrows / trows: [n][dim] raw entity rows, rel / norm_vect: [n_rel][dim]
+ * (rel_emb.weight, norm_vect.weight), scores: [n][n_rel] out, for kge_rank_dense / kge_topk_dense.
+ * dim <= 8192. */
+int kge_transh_rel_scores(const float* hrows, const float* trows, const float* rel, const float* norm_vect,
+                          int dim, int64_t n, int64_t n_rel, float* scores, void* stream);
 /* get_rank + filter_scores (utils/operations.py:37-61, utils/modeling.py:91-102) on a dense (n, n_cand)
  * score matrix, counters ADDED INTO as by kge_rank_side: raw_count[i] += #{c : s >= s_true};
  * filt_sub[i] += listed candidates with s >= s_true (minus the -inf quirk).  s_true = true_score_in[i]
@@ -345,6 +353,14 @@ typedef struct {
   float* ent0; float* ent1; float* rel0; float* rel1;
 } kge_grads_t;
 
+/* TransH's projected entity table for one relation (models/translation.py:270-284, evaluate_projections):
+ * out[e][k] = fl(ent[e][k] - fl(nc_e * w[k])), nc_e = (ent[e] * w).sum() summed in ATen's inner-dimension
+ * order.  ent: [n_rows][dim] raw ent_emb.weight, norm_row: [dim] raw norm_vect.weight row, out: [n_rows][dim]
+ * (caller-provided).  The result feeds kge_pack_table / kge_tc_pack_table and kge_rank_side /
+ * kge_topk_side as a KGE_TRANSE_L2 table.  dim <= 8192. */
+int kge_transh_project(const float* ent, const float* norm_row, int64_t n_rows, int dim, float* out,
+                       void* stream);
+
 /* Model.scoring_function (models/translation.py:69-81, models/bilinear.py:60-71, 188-199,
  * 460-473): scores[i] of triple (h[i], r[i], t[i]); TransE / DistMult / RESCAL L2-normalise
  * the gathered entity rows first (eps 1e-12). */
@@ -354,6 +370,17 @@ int kge_score_triples_fwd(const kge_tables_t* tb, const int64_t* h, const int64_
 int kge_score_triples_bwd(const kge_tables_t* tb, const kge_grads_t* g, const int64_t* h,
                           const int64_t* t, const int64_t* r, int64_t n, const float* grad_scores,
                           void* stream);
+/* TransH's scoring_function (models/translation.py:183-202): scores[i] = -||P(h~) + r - P(t~)||^2 with h~,
+ * t~ and the relation's normal vector w~ L2-normalised (eps 1e-12) and P(v) = v - (v . w~) w~.  Its own
+ * tables (ent_emb.weight, rel_emb.weight, norm_vect.weight, each [rows][dim]) rather than a kge_tables_t. */
+int kge_transh_score_triples_fwd(const float* ent, const float* rel, const float* norm_vect, int dim,
+                                 const int64_t* h, const int64_t* t, const int64_t* r, int64_t n, float* scores,
+                                 void* stream);
+/* accumulates d(sum_i grad_scores[i] * scores[i]) / d(tables) into the three gradient tables */
+int kge_transh_score_triples_bwd(const float* ent, const float* rel, const float* norm_vect, float* grad_ent,
+                                 float* grad_rel, float* grad_norm_vect, int dim, const int64_t* h,
+                                 const int64_t* t, const int64_t* r, int64_t n, const float* grad_scores,
+                                 void* stream);
 
 /* BernoulliNegativeSampler.corrupt_batch (sampling.py:278-327): nh/nt of length b*n_neg laid
  * out as n_neg blocks of the batch; negative j of fact i corrupts the head with probability

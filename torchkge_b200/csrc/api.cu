@@ -734,6 +734,30 @@ int kge_rescal_rel_scores(const float* hrows, const float* trows, const float* r
   return KGE_OK;
 }
 
+int kge_transh_rel_scores(const float* hrows, const float* trows, const float* rel, const float* norm_vect,
+                          int dim, int64_t n, int64_t n_rel, float* scores, void* stream) {
+  if (n == 0 || n_rel == 0) return KGE_OK;
+  if (n < 0 || n_rel < 0 || dim < 1 || !hrows || !trows || !rel || !norm_vect || !scores)
+    return fail(KGE_ERR_ARG, "kge_transh_rel_scores: bad argument");
+  if (dim > kge::SCAN_MAX_DIM) return fail(KGE_ERR_UNSUPPORTED, "kge_transh_rel_scores: dim > 8192");
+  DeviceScope device_scope(scores);
+  KGE_CUDA_TRY(kge::launch_transh_rel_scores(hrows, trows, rel, norm_vect, dim, n, n_rel, scores,
+                                             static_cast<cudaStream_t>(stream)),
+               "transh_rel_scores");
+  return KGE_OK;
+}
+
+int kge_transh_project(const float* ent, const float* norm_row, int64_t n_rows, int dim, float* out,
+                       void* stream) {
+  if (n_rows == 0) return KGE_OK;
+  if (n_rows < 0 || dim < 1 || !ent || !norm_row || !out) return fail(KGE_ERR_ARG, "kge_transh_project: bad argument");
+  if (dim > kge::SCAN_MAX_DIM) return fail(KGE_ERR_UNSUPPORTED, "kge_transh_project: dim > 8192");
+  DeviceScope device_scope(out);
+  KGE_CUDA_TRY(kge::launch_transh_project(ent, norm_row, n_rows, dim, out, static_cast<cudaStream_t>(stream)),
+               "transh_project");
+  return KGE_OK;
+}
+
 int kge_rank_dense(const float* scores, int64_t n, int64_t n_cand, const int64_t* true_idx,
                    const float* true_score_in, const int64_t* filt_offs, const int64_t* filt_ids,
                    int32_t* raw_count, int32_t* filt_sub, float* true_score, void* stream) {
@@ -919,6 +943,34 @@ int kge_score_triples_bwd(const kge_tables_t* tb, const kge_grads_t* g, const in
   KGE_CUDA_TRY(kge::launch_score_triples_bwd(tb->model, tb->dim, to_tables(tb), to_grads(g), h, t, r, n,
                                              grad_scores, static_cast<cudaStream_t>(stream)),
                "score_triples_bwd");
+  return KGE_OK;
+}
+
+int kge_transh_score_triples_fwd(const float* ent, const float* rel, const float* norm_vect, int dim,
+                                 const int64_t* h, const int64_t* t, const int64_t* r, int64_t n, float* scores,
+                                 void* stream) {
+  if (n == 0) return KGE_OK;
+  if (n < 0 || dim < 1 || !ent || !rel || !norm_vect || !h || !t || !r || !scores)
+    return fail(KGE_ERR_ARG, "kge_transh_score_triples_fwd: bad argument");
+  DeviceScope device_scope(ent);
+  KGE_CUDA_TRY(kge::launch_transh_score_fwd(ent, rel, norm_vect, dim, h, t, r, n, scores,
+                                            static_cast<cudaStream_t>(stream)),
+               "transh_score_triples_fwd");
+  return KGE_OK;
+}
+
+int kge_transh_score_triples_bwd(const float* ent, const float* rel, const float* norm_vect, float* grad_ent,
+                                 float* grad_rel, float* grad_norm_vect, int dim, const int64_t* h,
+                                 const int64_t* t, const int64_t* r, int64_t n, const float* grad_scores,
+                                 void* stream) {
+  if (n == 0) return KGE_OK;
+  if (n < 0 || dim < 1 || !ent || !rel || !norm_vect || !grad_ent || !grad_rel || !grad_norm_vect || !h || !t ||
+      !r || !grad_scores)
+    return fail(KGE_ERR_ARG, "kge_transh_score_triples_bwd: bad argument");
+  DeviceScope device_scope(ent);
+  KGE_CUDA_TRY(kge::launch_transh_score_bwd(ent, rel, norm_vect, grad_ent, grad_rel, grad_norm_vect, dim, h, t, r,
+                                            n, grad_scores, static_cast<cudaStream_t>(stream)),
+               "transh_score_triples_bwd");
   return KGE_OK;
 }
 

@@ -386,6 +386,21 @@ __global__ void finalize_kernel(const int32_t* __restrict__ raw, const int32_t* 
   filt_ranks[i] = r - (int64_t)sub[i];
 }
 
+// TransH: out[row] = projection of ent[row] on the hyperplane of normal w (reduce.cuh:
+// transh_project_elem).  One warp per row; the lanes share the row's normal component nc.
+__global__ void __launch_bounds__(256) transh_project_kernel(const float* __restrict__ ent,
+                                                             const float* __restrict__ w, long long n_rows,
+                                                             int dim, float* __restrict__ out) {
+  const long long row = ((long long)blockIdx.x * blockDim.x + threadIdx.x) >> 5;
+  const int lane = threadIdx.x & 31;
+  if (row >= n_rows) return;   // whole warps leave together: the shuffles below see full warps
+  const float* e = ent + (size_t)row * dim;
+  const float nc = dim < 8 ? pair_score_natural<EL_DOT1>(dim, e, e, w, w)
+                           : pair_score_chains<EL_DOT1>(dim, e, e, w, w, lane);
+  float* o = out + (size_t)row * dim;
+  for (int k = lane; k < dim; k += 32) o[k] = transh_project_elem(e[k], nc, w[k]);
+}
+
 inline unsigned filter_blocks(long long n_filt) {
   const long long want = (n_filt + 3) / 4;  // >= one warp per entry group; grid-stride beyond
   return (unsigned)(want < 1 ? 1 : (want > 132LL * 64 ? 132LL * 64 : want));   // 64 blocks per H100 SM
@@ -471,6 +486,13 @@ cudaError_t launch_filter(int el, bool cascade, int dim, int64_t n, int64_t n_fi
         dim, n, n_filt, qplain, ent0, ent1, ent_lo, n_rows, offs, ids, qid, perm, code, s_true, filt_sub);
     return cudaGetLastError();
   });
+}
+
+cudaError_t launch_transh_project(const float* ent, const float* w, int64_t n_rows, int dim, float* out,
+                                  cudaStream_t stream) {
+  if (n_rows <= 0) return cudaSuccess;
+  transh_project_kernel<<<blocks_for(n_rows * 32, 256), 256, 0, stream>>>(ent, w, n_rows, dim, out);
+  return cudaGetLastError();
 }
 
 cudaError_t launch_finalize(const int32_t* raw, const int32_t* sub, int64_t n, int64_t* ranks,

@@ -49,6 +49,41 @@ __global__ void __launch_bounds__(RR_THREADS)
   if (lane == 0) scores[(size_t)i * n_rel + c] = s;
 }
 
+// TransH relation case (interfaces.py:261-272 with the projections of translation.py:253-254): grid
+// (n_rel, ceil(n / warps)), one warp per (fact i, relation c).  The warp projects h_i and t_i on the
+// hyperplane of relation c into its shared-memory rows, then scores -||(P_c(h) + r_c) - P_c(t)||^2 in the
+// L2-norm order: EL_L2_HEAD with candidate P_c(h), query planes (r_c, P_c(t)).
+__global__ void transh_rel_scores_kernel(const float* __restrict__ hrows, const float* __restrict__ trows,
+                                         const float* __restrict__ rel, const float* __restrict__ norm_vect,
+                                         int dim, long long n, long long n_rel, float* __restrict__ scores) {
+  extern __shared__ float sm[];       // per warp: [dim] P_c(h), then [dim] P_c(t)
+  const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
+  const long long c = blockIdx.x;
+  const long long i = (long long)blockIdx.y * (blockDim.x >> 5) + warp;
+  if (i >= n) return;
+  float* ph = sm + (size_t)warp * 2 * dim;
+  float* pt = ph + dim;
+  const float* w = norm_vect + (size_t)c * dim;
+  const float* r = rel + (size_t)c * dim;
+  const float* h = hrows + (size_t)i * dim;
+  const float* t = trows + (size_t)i * dim;
+  float nh, nt;
+  if (dim < 8) {
+    nh = pair_score_natural<EL_DOT1>(dim, h, h, w, w);
+    nt = pair_score_natural<EL_DOT1>(dim, t, t, w, w);
+  } else {
+    nh = pair_score_chains<EL_DOT1>(dim, h, h, w, w, lane);
+    nt = pair_score_chains<EL_DOT1>(dim, t, t, w, w, lane);
+  }
+  for (int k = lane; k < dim; k += 32) {
+    ph[k] = transh_project_elem(h[k], nh, w[k]);
+    pt[k] = transh_project_elem(t[k], nt, w[k]);
+  }
+  __syncwarp();
+  const float s = pair_score_chains<EL_L2_HEAD>(dim, r, pt, ph, ph, lane);
+  if (lane == 0) scores[(size_t)i * n_rel + c] = s;
+}
+
 // One warp per row of a dense (n, n_c) score matrix:
 //   raw_count[i] += #{c : s[i][c] >= s_true(i)},
 //   filt_sub[i]  += sum over the row's CSR entries of [s[i][c] >= s_true(i)] - [s_true(i) == -inf]
@@ -111,6 +146,33 @@ cudaError_t launch_rescal_rel_scores(const float* hrows, const float* trows, con
     rescal_rel_scores_kernel<<<grid, RR_THREADS, smem, stream>>>(hrows + (size_t)i_off * dim, trows + (size_t)i_off * dim,
                                                                rel_mat, dim, n - i_off, n_rel,
                                                                scores + (size_t)i_off * n_rel);
+  }
+  return cudaGetLastError();
+}
+
+cudaError_t launch_transh_rel_scores(const float* hrows, const float* trows, const float* rel,
+                                     const float* norm_vect, int dim, int64_t n, int64_t n_rel, float* scores,
+                                     cudaStream_t stream) {
+  if (n <= 0 || n_rel <= 0) return cudaSuccess;
+  // up to 8 warps (facts) per CTA within 48 KB of shared memory; one warp past dim 6144
+  const size_t per_warp = (size_t)2 * dim * sizeof(float);
+  long long warps = (long long)(48 * 1024 / per_warp);
+  warps = warps < 1 ? 1 : (warps > 8 ? 8 : warps);
+  const size_t smem = (size_t)warps * per_warp;
+  if (smem > 200 * 1024) return cudaErrorInvalidValue;
+  if (smem > 48 * 1024) {
+    const cudaError_t e =
+        set_attribute_once<transh_rel_scores_kernel>(cudaFuncAttributeMaxDynamicSharedMemorySize, 200 * 1024);
+    if (e != cudaSuccess) return e;
+  }
+  const long long i_tiles = (n + warps - 1) / warps;
+  for (long long y0 = 0; y0 < i_tiles; y0 += 65535) {     // gridDim.y limit
+    const long long ny = i_tiles - y0 < 65535 ? i_tiles - y0 : 65535;
+    dim3 grid((unsigned)n_rel, (unsigned)ny);
+    const long long i_off = y0 * warps;
+    transh_rel_scores_kernel<<<grid, (unsigned)(32 * warps), smem, stream>>>(
+        hrows + (size_t)i_off * dim, trows + (size_t)i_off * dim, rel, norm_vect, dim, n - i_off, n_rel,
+        scores + (size_t)i_off * n_rel);
   }
   return cudaGetLastError();
 }

@@ -136,6 +136,10 @@ cudaError_t launch_filter(int el, bool cascade, int dim, int64_t n, int64_t n_fi
 cudaError_t launch_finalize(const int32_t* raw, const int32_t* sub, int64_t n, int64_t* ranks,
                             int64_t* filt_ranks, cudaStream_t stream);
 
+// out[row][k] = TransH projection of ent[row] on the hyperplane of normal w (reduce.cuh: transh_project_elem)
+cudaError_t launch_transh_project(const float* ent, const float* w, int64_t n_rows, int dim, float* out,
+                                  cudaStream_t stream);
+
 // ---- top-k selection over collected candidates (topk.cu) ----
 // best[q][k] sorted 64-bit keys (score order, then smaller id first; 0 = empty slot).
 // Merges the `count[q]` (or `dense_count`) entries of col_buf[q] into best[q], masking ids listed in
@@ -159,6 +163,10 @@ cudaError_t launch_topk_lists_merge(const int64_t* pred_in, const float* scores_
 // scores[i][c] = ((h_i^T M_c) * t_i).sum()   RESCAL relation case, bilinear.py:115-121
 cudaError_t launch_rescal_rel_scores(const float* hrows, const float* trows, const float* rel_mat, int dim,
                                      int64_t n, int64_t n_rel, float* scores, cudaStream_t stream);
+// scores[i][c] = -||(P_c(h_i) + r_c) - P_c(t_i)||^2   TransH relation case, interfaces.py:261-272
+cudaError_t launch_transh_rel_scores(const float* hrows, const float* trows, const float* rel,
+                                     const float* norm_vect, int dim, int64_t n, int64_t n_rel, float* scores,
+                                     cudaStream_t stream);
 cudaError_t launch_rank_dense(const float* scores, int64_t n, int64_t n_c, const int64_t* true_idx,
                               const float* true_score_in, const int64_t* offs, const int64_t* ids,
                               int32_t* raw_count, int32_t* filt_sub, float* true_score_out, cudaStream_t stream);

@@ -385,6 +385,14 @@ __device__ __forceinline__ float rescal_query_component(bool tail, int d, int j,
   return acc;
 }
 
+// TransH's projection of an entity row e on the hyperplane of normal w (translation.py:279-281,
+// evaluate_projections):  P[k] = fl(e[k] - fl(nc * w[k]))  with  nc = (e * w).sum()  summed in ATen's
+// inner-dimension order (pair_score_natural / pair_score_chains of EL_DOT1 give that sum).  The inputs
+// are the raw ent_emb / norm_vect rows: the reference does not re-normalise them there.
+__device__ __forceinline__ float transh_project_elem(float e, float nc, float w) {
+  return __fsub_rn(e, __fmul_rn(nc, w));
+}
+
 // Exact adjudication of the near-tie band (the list is kept as one region per CTA of the scan).
 // Chain-parallel: the independent chains of the ATen reduction are spread over the lanes of a
 // warp -- 8 lanes per pair for the L2 norm (4 pairs per warp), 32 lanes per pair for the

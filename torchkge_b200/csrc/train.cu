@@ -411,6 +411,92 @@ __device__ void triple_backward(int model, int dim, const RowPtrs& p, const Grad
   }
 }
 
+// ---- TransH scoring_function (translation.py:183-202): with h~, t~, w~ the L2-normalised head, tail and
+// normal vector of the relation, a = h~ . w~, b = t~ . w~,
+//   x = (h~ - a w~) + r - (t~ - b w~),   score = -|x|^2.
+// Its own tables (ent, rel, norm_vect) rather than a model code: the tables of the other models cannot carry it.
+struct TransHRows {
+  const float* h; const float* t; const float* r; const float* w;
+  float ih, it, iw;   // 1 / max(|row|, eps)
+  float a, b;         // h~ . w~ and t~ . w~
+};
+
+__device__ __forceinline__ TransHRows transh_rows(const float* ent, const float* rel, const float* nv, int dim,
+                                                  long long h, long long t, long long r, int lane) {
+  TransHRows p;
+  p.h = ent + (size_t)h * dim; p.t = ent + (size_t)t * dim;
+  p.r = rel + (size_t)r * dim; p.w = nv + (size_t)r * dim;
+  p.ih = inv_norm_of(p.h, dim, lane); p.it = inv_norm_of(p.t, dim, lane); p.iw = inv_norm_of(p.w, dim, lane);
+  float a = 0.f, b = 0.f;
+  for (int k = lane; k < dim; k += 32) {
+    const float wn = p.w[k] * p.iw;
+    a = fmaf(p.h[k] * p.ih, wn, a);
+    b = fmaf(p.t[k] * p.it, wn, b);
+  }
+  p.a = warp_sum(a); p.b = warp_sum(b);
+  return p;
+}
+
+__device__ __forceinline__ float transh_x(const TransHRows& p, int k) {
+  const float wn = p.w[k] * p.iw;
+  return (p.h[k] * p.ih - p.a * wn) + p.r[k] - (p.t[k] * p.it - p.b * wn);
+}
+
+__global__ void transh_score_fwd_kernel(const float* __restrict__ ent, const float* __restrict__ rel,
+                                        const float* __restrict__ nv, int dim, const int64_t* __restrict__ h,
+                                        const int64_t* __restrict__ t, const int64_t* __restrict__ r, long long n,
+                                        float* __restrict__ out) {
+  const long long w = ((long long)blockIdx.x * blockDim.x + threadIdx.x) >> 5;
+  const int lane = threadIdx.x & 31;
+  if (w >= n) return;
+  const TransHRows p = transh_rows(ent, rel, nv, dim, h[w], t[w], r[w], lane);
+  float s = 0.f;
+  for (int k = lane; k < dim; k += 32) { const float x = transh_x(p, k); s = fmaf(x, x, s); }
+  s = warp_sum(s);
+  if (lane == 0) out[w] = -s;
+}
+
+// With G = dscore/dx = -2x and c = w~ . G:
+//   dscore/dh~ = G - c w~,   dscore/dt~ = -(G - c w~),   dscore/dr = G,   dscore/dw~ = -(a - b) G - c (h~ - t~),
+// each then through F.normalize:  d/dv = (G_v - v~ (v~ . G_v)) / max(|v|, eps), where
+//   h~ . G_h = h~.G - c a,   t~ . G_t = -(t~.G - c b),   w~ . G_w = -2 c (a - b).
+__global__ void transh_score_bwd_kernel(const float* __restrict__ ent, const float* __restrict__ rel,
+                                        const float* __restrict__ nv, float* __restrict__ g_ent,
+                                        float* __restrict__ g_rel, float* __restrict__ g_nv, int dim,
+                                        const int64_t* __restrict__ h, const int64_t* __restrict__ t,
+                                        const int64_t* __restrict__ r, long long n, const float* __restrict__ gout) {
+  const long long w = ((long long)blockIdx.x * blockDim.x + threadIdx.x) >> 5;
+  const int lane = threadIdx.x & 31;
+  if (w >= n) return;
+  const float g = gout[w];
+  if (g == 0.f) return;
+  const long long hi = h[w], ti = t[w], ri = r[w];
+  const TransHRows p = transh_rows(ent, rel, nv, dim, hi, ti, ri, lane);
+  float c = 0.f, hg = 0.f, tg = 0.f;
+  for (int k = lane; k < dim; k += 32) {
+    const float G = -2.f * transh_x(p, k);
+    c = fmaf(p.w[k] * p.iw, G, c);
+    hg = fmaf(p.h[k] * p.ih, G, hg);
+    tg = fmaf(p.t[k] * p.it, G, tg);
+  }
+  c = warp_sum(c); hg = warp_sum(hg); tg = warp_sum(tg);
+  const float dot_h = hg - c * p.a, dot_t = -(tg - c * p.b), dot_w = -2.f * c * (p.a - p.b);
+  float* gh = g_ent + (size_t)hi * dim;
+  float* gt = g_ent + (size_t)ti * dim;
+  float* gr = g_rel + (size_t)ri * dim;
+  float* gw = g_nv + (size_t)ri * dim;
+  for (int k = lane; k < dim; k += 32) {
+    const float hn = p.h[k] * p.ih, tn = p.t[k] * p.it, wn = p.w[k] * p.iw;
+    const float G = -2.f * transh_x(p, k);
+    const float Gh = G - c * wn;
+    const float Gw = -(p.a - p.b) * G - c * (hn - tn);
+    atomicAdd(gh + k, g * (Gh - hn * dot_h) * p.ih);
+    atomicAdd(gt + k, g * (-Gh - tn * dot_t) * p.it);
+    atomicAdd(gr + k, g * G);
+    atomicAdd(gw + k, g * (Gw - wn * dot_w) * p.iw);
+  }
+}
+
 // ------------------------------------------------------------------------------------------
 __global__ void score_triples_fwd_kernel(int model, int dim, TrainTables tb,
                                          const int64_t* __restrict__ h,
@@ -1556,6 +1642,24 @@ cudaError_t launch_score_triples_bwd(int model, int dim, const TrainTables& tb, 
   if (n <= 0) return cudaSuccess;
   score_triples_bwd_kernel<<<blocks_for_warps(n), WARPS_PER_BLOCK * 32, 0, st>>>(model, dim, tb, gr, h,
                                                                                  t, r, n, gout);
+  return cudaGetLastError();
+}
+
+cudaError_t launch_transh_score_fwd(const float* ent, const float* rel, const float* norm_vect, int dim,
+                                    const int64_t* h, const int64_t* t, const int64_t* r, int64_t n, float* out,
+                                    cudaStream_t st) {
+  if (n <= 0) return cudaSuccess;
+  transh_score_fwd_kernel<<<blocks_for_warps(n), WARPS_PER_BLOCK * 32, 0, st>>>(ent, rel, norm_vect, dim, h, t, r,
+                                                                                n, out);
+  return cudaGetLastError();
+}
+
+cudaError_t launch_transh_score_bwd(const float* ent, const float* rel, const float* norm_vect, float* g_ent,
+                                    float* g_rel, float* g_norm_vect, int dim, const int64_t* h, const int64_t* t,
+                                    const int64_t* r, int64_t n, const float* gout, cudaStream_t st) {
+  if (n <= 0) return cudaSuccess;
+  transh_score_bwd_kernel<<<blocks_for_warps(n), WARPS_PER_BLOCK * 32, 0, st>>>(
+      ent, rel, norm_vect, g_ent, g_rel, g_norm_vect, dim, h, t, r, n, gout);
   return cudaGetLastError();
 }
 

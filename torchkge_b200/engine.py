@@ -42,6 +42,8 @@ class ModelSpec:
         self.ent2, self.rel2 = ent2, rel2
         self.ent_lo = int(ent_lo)    # global id of row 0 of ent0/ent1
         self.n_rows = int(ent0.shape[0])
+        #: TransH only (transh_spec): the raw norm_vect table; ent0 / rel0 are then ent_emb / rel_emb
+        self.norm_vect = None
         if code == _lib.ANALOGY:
             for name, planes in (("entity", (ent0, ent1, ent2)), ("relation", (rel0, rel1, rel2))):
                 if planes[0] is None and name == "relation":
@@ -126,9 +128,42 @@ class ModelSpec:
             r = cls.stacked([model.sc_rel_emb.weight, model.re_rel_emb.weight, model.im_rel_emb.weight])
             return cls(_lib.ANALOGY, model.scalar_dim, model.n_ent, model.n_rel, e[0], e[1], r[0], r[1],
                        ent2=e[2], rel2=r[2])
+        if name == "TransHModel":
+            # every entry point that supports TransH builds its spec with transh_spec; the others (the
+            # fused training step, sharded calls, inference_scoring_function) end here
+            raise NotImplementedError(
+                "TransHModel is supported by the unsharded LinkPredictionEvaluator, RelationPredictionEvaluator, "
+                "TripletClassificationEvaluator, EntityInference, RelationInference and scoring_function only "
+                "(not by the fused training step or shard=)")
         raise NotImplementedError(
-            "%s has no CUDA link-prediction path (supported: TransE L1/L2, TorusE torus_L1/torus_L2, "
+            "%s has no CUDA link-prediction path (supported: TransE L1/L2, TransH, TorusE torus_L1/torus_L2, "
             "DistMult, RESCAL, ComplEx, Analogy, RotatE)" % name)
+
+
+def is_transh(model):
+    """TransHModel of this package or (duck-typed, by class name) of the reference."""
+    return type(model).__name__ == "TransHModel"
+
+
+def transh_spec(model):
+    """The spec of a TransH model (translation.py:168-181): the entity and relation tables read as a
+    TransE-L2 model's, plus the raw normal vectors.  The scans never see ent_emb itself: every TransH path
+    projects it per relation first (rank_link_prediction_transh, topk_entity_inference, transh_rel_scores)."""
+    f = ModelSpec._f32
+    spec = ModelSpec(_lib.TRANSE_L2, model.emb_dim, model.n_ent, model.n_rel, f(model.ent_emb.weight), None,
+                     f(model.rel_emb.weight), None)
+    spec.norm_vect = f(model.norm_vect.weight)
+    return spec
+
+
+def _is_transh_spec(spec):
+    return getattr(spec, "norm_vect", None) is not None
+
+
+def _refuse_transh_shard(spec, shard):
+    """Sharded TransH calls are not supported: raised on every rank, before any collective."""
+    if _is_transh_spec(spec) and shard is not None:
+        raise NotImplementedError("TransHModel does not support shard= (EntityShard / QueryShard)")
 
 
 def _ptr(t):
@@ -224,8 +259,10 @@ class CudaEngine:
     def clear_cache(self):
         self._tc_cache.clear()
 
-    def pack_tc(self, spec):
-        """Tensor-core operand image of the shard, or None when the model has no such path."""
+    def pack_tc(self, spec, cache=True):
+        """Tensor-core operand image of the shard, or None when the model has no such path.
+        ``cache=False``: build it without the checksummed cache (a table rewritten in place for every call,
+        such as TransH's per-relation projection buffer)."""
         if not self.tensor_core:
             return None
         nbytes = self.lib.kge_tc_packed_bytes(spec.code, spec.n_rows, spec.dim)
@@ -234,7 +271,7 @@ class CudaEngine:
         dev = spec.ent0.device
         # a three-plane spec reads a stacked COPY of the weights made for this call (ModelSpec.stacked):
         # its address changes every time, so there is nothing to cache an image under
-        if self.tc_cache_entries <= 0 or getattr(spec, "ent2", None) is not None:
+        if not cache or self.tc_cache_entries <= 0 or getattr(spec, "ent2", None) is not None:
             out = torch.empty(nbytes, dtype=torch.uint8, device=dev)
             _lib.check(self.lib.kge_tc_pack_table(spec.code, _ptr(spec.ent0), _ptr(spec.ent1), spec.n_rows,
                                                   spec.dim, _ptr(out), _stream(dev)), "kge_tc_pack_table")
@@ -390,6 +427,26 @@ class CudaEngine:
         scores = torch.empty((n, spec.n_rel), dtype=torch.float32, device=dev)
         _lib.check(self.lib.kge_rescal_rel_scores(_ptr(hrows), _ptr(trows), _ptr(spec.rel0), spec.dim, n,
                                                   spec.n_rel, _ptr(scores), _stream(dev)), "kge_rescal_rel_scores")
+        self.launches += 1
+        return scores
+
+    def transh_project(self, spec, rel, out):
+        """out (n_rows, dim) <- the entity rows of ``spec`` (transh_spec) projected on the hyperplane of
+        relation ``rel`` (kge_transh_project, translation.py:279-281)."""
+        _need_cuda(spec.ent0, out)
+        _lib.check(self.lib.kge_transh_project(_ptr(spec.ent0), _ptr(spec.norm_vect[rel]), spec.n_rows, spec.dim,
+                                               _ptr(out), _stream(out.device)), "kge_transh_project")
+        self.launches += 1
+        return out
+
+    def transh_rel_scores(self, spec, hrows, trows):
+        """(n, n_rel) scores -||(P_c(h) + r_c) - P_c(t)||^2 of every relation c: TransH's relation case
+        (interfaces.py:261-272), dense like RESCAL's."""
+        n, dev = hrows.shape[0], hrows.device
+        scores = torch.empty((n, spec.n_rel), dtype=torch.float32, device=dev)
+        _lib.check(self.lib.kge_transh_rel_scores(_ptr(hrows), _ptr(trows), _ptr(spec.rel0), _ptr(spec.norm_vect),
+                                                  spec.dim, n, spec.n_rel, _ptr(scores), _stream(dev)),
+                   "kge_transh_rel_scores")
         self.launches += 1
         return scores
 
@@ -666,7 +723,11 @@ def shard_spec(model, shard=None, who="evaluate", n=None, build=ModelSpec.from_m
     """The ModelSpec the engine reads for ``model`` (``build(model)``) under ``shard``, after the shard's
     argument checks: under an EntityShard with local storage the model holds entity rows [lo, hi) and its
     row 0 is entity lo (_check_table); a QueryShard must cover ``n`` facts, when ``n`` is given.  The
-    checks come first, then the model must be on a CUDA device."""
+    checks come first, then the model must be on a CUDA device.  TransH: no shard, and transh_spec."""
+    if is_transh(model):
+        if shard is not None:
+            raise NotImplementedError("TransHModel does not support shard= (EntityShard / QueryShard)")
+        build = transh_spec
     spec = build(model)
     if isinstance(shard, EntityShard):
         if shard.local_storage:
@@ -711,7 +772,7 @@ class LazyRanks:
 
 
 def rank_link_prediction(spec, h_idx, t_idx, r_idx, filt_tail, filt_head, shard=None,
-                         engine=None, chunk=DEFAULT_CHUNK, packed=None, exact=False, sync=True):
+                         engine=None, chunk=DEFAULT_CHUNK, packed=None, exact=False, sync=True, tc_cache=True):
     """Rank every triple's true tail and head against all entities, raw and filtered.
 
     spec       ModelSpec holding either the full entity table or exactly this rank's shard
@@ -723,10 +784,13 @@ def rank_link_prediction(spec, h_idx, t_idx, r_idx, filt_tail, filt_head, shard=
     shard      EntityShard when the table is range-partitioned over a process group
     exact      True: scalar ATen-order scan only (no tensor-core / approximate bound-and-refine)
     sync       False: return a LazyRanks (no host synchronisation at all inside this call)
+    tc_cache   False: build the tensor-core image without the engine's cache (CudaEngine.pack_tc)
     Returns (rank_heads, rank_tails, filt_rank_heads, filt_rank_tails), int64 device tensors.
     """
     engine = engine or default_engine()
     n = h_idx.shape[0]
+    if _is_transh_spec(spec):
+        raise ValueError("a TransH spec is ranked by rank_link_prediction_transh")
     table = spec
     if shard is not None:
         _check_table(spec, shard)
@@ -737,7 +801,9 @@ def rank_link_prediction(spec, h_idx, t_idx, r_idx, filt_tail, filt_head, shard=
     mark("step begin")
     dev = spec.ent0.device
     with _device_guard(dev):
-        tc_packed = engine.pack_tc(spec) if (hasattr(engine, "pack_tc") and not exact) else None
+        tc_packed = None
+        if hasattr(engine, "pack_tc") and not exact:
+            tc_packed = engine.pack_tc(spec) if tc_cache else engine.pack_tc(spec, cache=False)
         mark("pack_tc")
         if packed is None and tc_packed is None:
             packed = engine.pack(spec)   # scalar-scan layout: only when there is no tensor-core path
@@ -813,6 +879,59 @@ def rank_link_prediction(spec, h_idx, t_idx, r_idx, filt_tail, filt_head, shard=
     return lazy.get() if sync else lazy
 
 
+def relation_groups(r_idx, n_rel):
+    """Facts grouped by relation: (order, order_host, groups) with ``order`` the device permutation that sorts
+    r_idx (stable), ``order_host`` its host copy and ``groups`` the host list of (relation, lo, hi) of the
+    sorted facts, relations without facts left out.  One device -> host copy."""
+    order = torch.argsort(r_idx, stable=True)
+    both = torch.cat([torch.bincount(r_idx, minlength=n_rel), order]).cpu()   # the one host synchronisation
+    counts, order_host = both[:n_rel].tolist(), both[n_rel:]
+    groups, lo = [], 0
+    for rel, c in enumerate(counts):
+        if c:
+            groups.append((rel, lo, lo + c))
+            lo += c
+    return order, order_host, groups
+
+
+def rank_link_prediction_transh(spec, h_idx, t_idx, r_idx, groups, filt_tail, filt_head, engine=None,
+                                chunk=DEFAULT_CHUNK, exact=False, sync=True):
+    """rank_link_prediction for TransH (transh_spec): the facts come sorted by relation, ``groups`` the
+    (relation, lo, hi) of relation_groups.  Per relation, the entity table is projected on its hyperplane into
+    one reused buffer (kge_transh_project) and the group is ranked on it as TransE-L2 -- tail queries
+    fl(P_r(h) + r) against the projected candidates, head candidates (P_r(c) + r) - P_r(t), exactly the
+    reference's arithmetic on its projected_entities (interfaces.py:249-260) -- with the filter CSR rows of
+    the group.  The tensor-core image of the buffer is rebuilt per relation, without the cache.
+    Arguments and result as rank_link_prediction's (no shard)."""
+    engine = engine or default_engine()
+    n = h_idx.shape[0]
+    dev = spec.ent0.device
+    with _device_guard(dev):
+        proj = torch.empty_like(spec.ent0)
+        ranks = [torch.empty(n, dtype=torch.int64, device=dev) for _ in range(4)]
+        filts = [f() if callable(f) else f for f in (filt_tail, filt_head)]
+        ranges = [(lo, hi) for _, lo, hi in groups]
+        parts = [_csr_cut(f, ranges) for f in filts]    # one device -> host read per CSR
+        flags = []
+        for (rel, lo, hi), ft, fh in zip(groups, parts[0], parts[1]):
+            engine.transh_project(spec, rel, proj)
+            pspec = ModelSpec(spec.code, spec.dim, spec.n_ent, spec.n_rel, proj, None, spec.rel0, None)
+            lazy = rank_link_prediction(pspec, h_idx[lo:hi], t_idx[lo:hi], r_idx[lo:hi], ft, fh, engine=engine,
+                                        chunk=chunk, exact=exact, sync=False, tc_cache=False)
+            for out, x in zip(ranks, lazy.ranks):
+                out[lo:hi] = x
+            if lazy.overflow is not None:
+                flags.append(lazy.overflow.view(1))
+        overflow = torch.cat(flags).sum() if flags else None
+
+    def redo():
+        return rank_link_prediction_transh(spec, h_idx, t_idx, r_idx, groups, filts[0], filts[1], engine=engine,
+                                           chunk=chunk, exact=True)
+
+    lazy = LazyRanks(tuple(ranks), overflow, redo)
+    return lazy.get() if sync else lazy
+
+
 def relation_spec(spec):
     """The model seen from relation prediction: the candidate table is the RELATION table
     (``inference_prepare_candidates(..., entities=False)``: translation.py:118-121,
@@ -829,6 +948,20 @@ def relation_spec(spec):
             "%s has no scan-based relation-prediction path (TransE L1/L2, DistMult, ComplEx, Analogy have; "
             "RESCAL goes through the dense kge_rescal_rel_scores)" % _lib.MODEL_NAMES.get(spec.code, spec.code))
     return ModelSpec(spec.code, spec.dim, spec.n_rel, spec.n_rel, cand0, cand1, None, None, ent2=cand2)
+
+
+def _dense_relations(spec):
+    """Models whose relation case is a dense (n, n_rel) score matrix rather than a scan over a candidate table:
+    RESCAL (per-fact vectors h^T M_c, bilinear.py:115-121) and TransH (rows projected per relation,
+    interfaces.py:261-272)."""
+    return spec.code == _lib.RESCAL or _is_transh_spec(spec)
+
+
+def _dense_rel_scores(engine, spec, hrows, trows):
+    """(n, n_rel) relation scores of the facts (hrows, ?, trows), hrows / trows (n, dim), for _dense_relations."""
+    if _is_transh_spec(spec):
+        return engine.transh_rel_scores(spec, hrows, trows)
+    return engine.rescal_rel_scores(spec, hrows, trows)
 
 
 def rank_relation_prediction(spec, h_idx, t_idx, r_idx, filt, directed=True, engine=None,
@@ -852,7 +985,8 @@ def rank_relation_prediction(spec, h_idx, t_idx, r_idx, filt, directed=True, eng
     engine = engine or default_engine()
     n = h_idx.shape[0]
     dev = spec.ent0.device
-    rspec = None if spec.code == _lib.RESCAL else relation_spec(spec)   # unsupported models raise here
+    _refuse_transh_shard(spec, shard)
+    rspec = None if _dense_relations(spec) else relation_spec(spec)   # unsupported models raise here
     if isinstance(shard, EntityShard):
         _check_table(spec, shard)
         if not shard.local_storage:
@@ -870,12 +1004,11 @@ def rank_relation_prediction(spec, h_idx, t_idx, r_idx, filt, directed=True, eng
             m = r.shape[0]
             s_true = torch.empty(m, dtype=torch.float32, device=dev)
             if rspec is None:
-                # RESCAL: the candidates are the relation MATRICES: per-fact vectors h^T M_c, a dense
-                # (m, n_rel) score matrix (bilinear.py:115-121) ranked by kge_rank_dense
+                # RESCAL, TransH: a dense (m, n_rel) score matrix (_dense_rel_scores) ranked by kge_rank_dense
                 hrows, trows = hrows.reshape(m, spec.dim), trows.reshape(m, spec.dim)
-                engine.rank_dense(engine.rescal_rel_scores(spec, hrows, trows), r, f, raw, sub, true_score=s_true)
+                engine.rank_dense(_dense_rel_scores(engine, spec, hrows, trows), r, f, raw, sub, true_score=s_true)
                 if not directed:
-                    engine.rank_dense(engine.rescal_rel_scores(spec, trows, hrows), r, f, raw, sub,
+                    engine.rank_dense(_dense_rel_scores(engine, spec, trows, hrows), r, f, raw, sub,
                                       true_score_in=s_true)
                 return
             rrows = engine.gather_rows(rspec, r)
@@ -886,7 +1019,7 @@ def rank_relation_prediction(spec, h_idx, t_idx, r_idx, filt, directed=True, eng
                                              true_rows=rrows, true_score_in=s_true))
             keep.append((s_true, f))
 
-        # the dense RESCAL branch holds (chunk, n_rel) scores: at most 4096 facts per call
+        # the dense branch holds (chunk, n_rel) scores: at most 4096 facts per call
         step = min(chunk, 4096) if rspec is None else chunk
         chunks = [(lo, min(n, lo + step)) for lo in range(0, n, step)]
         if shard is None or shard.world == 1:
@@ -1028,6 +1161,9 @@ def topk_entity_inference(spec, ents, rels, side, k, mask=None, shard=None, engi
     engine = engine or default_engine()
     n = ents.shape[0]
     dev = spec.ent0.device
+    _refuse_transh_shard(spec, shard)
+    if _is_transh_spec(spec):
+        return _topk_entity_transh(spec, ents, rels, side, k, mask, engine, chunk)
     if shard is not None and shard.world > 1:
         _check_sharded_k(k, spec.n_ent)
     if isinstance(shard, EntityShard):
@@ -1063,6 +1199,41 @@ def topk_entity_inference(spec, ents, rels, side, k, mask=None, shard=None, engi
         return _topk_chunks(n, spec.n_ent, k, topk_chunk, mask, dev, chunk)
 
 
+def _topk_entity_transh(spec, ents, rels, side, k, mask, engine, chunk):
+    """topk_entity_inference for TransH: the queries grouped by relation (relation_groups), the entity table
+    projected per relation into one reused buffer and scanned as TransE-L2, as in rank_link_prediction_transh."""
+    n = ents.shape[0]
+    dev = spec.ent0.device
+    _check_k(k, spec.n_rows)
+    with _device_guard(dev):
+        order, perm, groups = relation_groups(rels, spec.n_rel)
+        ents_s, rels_s = ents[order].contiguous(), rels[order].contiguous()
+        if mask is not None:        # host CSR over the queries -> rows in sorted order
+            offs, ids = mask
+            lens = offs[1:] - offs[:-1]
+            new_offs = torch.zeros(n + 1, dtype=torch.int64)
+            new_offs[1:] = torch.cumsum(lens[perm], 0)
+            sel = torch.repeat_interleave(offs[:-1][perm], lens[perm]) + (
+                torch.arange(int(new_offs[-1])) - torch.repeat_interleave(new_offs[:-1], lens[perm]))
+            mask = (new_offs, ids[sel])
+        proj = torch.empty_like(spec.ent0)
+        pred = torch.empty((n, k), dtype=torch.int64, device=dev)
+        vals = torch.empty((n, k), dtype=torch.float32, device=dev)
+        for (rel, lo, hi), m in zip(groups, _csr_cut(mask, [(lo, hi) for _, lo, hi in groups])):
+            engine.transh_project(spec, rel, proj)
+            pspec = ModelSpec(spec.code, spec.dim, spec.n_ent, spec.n_rel, proj, None, spec.rel0, None)
+            packed = engine.pack(pspec)
+
+            def topk_chunk(a, b, mm):
+                rows = engine.gather_rows(pspec, ents_s[lo + a:lo + b])
+                return engine.topk_side(pspec, packed, side, rows, rows, rels_s[lo + a:lo + b], k, mm)
+
+            pred[lo:hi], vals[lo:hi] = _topk_chunks(hi - lo, spec.n_rows, k, topk_chunk, m, dev, chunk)
+        out_pred, out_vals = torch.empty_like(pred), torch.empty_like(vals)
+        out_pred[order], out_vals[order] = pred, vals
+        return out_pred, out_vals
+
+
 def topk_relation_inference(spec, e1, e2, k, mask=None, shard=None, engine=None, chunk=TOPK_CHUNK):
     """The k best relations completing (e1[i], ?, e2[i]), best first (RelationInference).
 
@@ -1074,14 +1245,15 @@ def topk_relation_inference(spec, e1, e2, k, mask=None, shard=None, engine=None,
     engine = engine or default_engine()
     n = e1.shape[0]
     dev = spec.ent0.device
+    _refuse_transh_shard(spec, shard)
     if isinstance(shard, QueryShard) and shard.world > 1:
         _check_sharded_k(k, spec.n_rel)
         _check_queries(shard, n)
         full, = _by_query_slices(shard, lambda a, b, m: [_pair_pack(*topk_relation_inference(
             spec, a, b, k, m, engine=engine, chunk=chunk))], (e1, e2), mask)
         return _pair_unpack(full)
-    if spec.code == _lib.RESCAL:
-        # candidates are relation matrices: dense (n, n_rel) scores, then the same selection kernels
+    if _dense_relations(spec):
+        # RESCAL, TransH: dense (n, n_rel) scores, then the same selection kernels
         rspec, packed, n_cand = None, None, spec.n_rel
     else:
         rspec = relation_spec(spec)
@@ -1090,7 +1262,7 @@ def topk_relation_inference(spec, e1, e2, k, mask=None, shard=None, engine=None,
     def local_topk(hrows, trows, m):
         if rspec is None:
             m_rows = hrows.shape[0]
-            scores = engine.rescal_rel_scores(spec, hrows.view(m_rows, spec.dim), trows.view(m_rows, spec.dim))
+            scores = _dense_rel_scores(engine, spec, hrows.view(m_rows, spec.dim), trows.view(m_rows, spec.dim))
             return engine.topk_dense(scores, k, m)
         return engine.topk_side(rspec, packed, _lib.SIDE_REL, hrows, trows, None, k, m)
 

@@ -10,8 +10,8 @@ import torch
 from . import _lib
 from .data import dict_filter_csr, filter_csr
 from .engine import (DEFAULT_CHUNK, EntityShard, ModelSpec, QueryShard, _by_query_slices, _check_table,
-                     default_engine, rank_link_prediction, rank_relation_prediction, score_triples_entity_sharded,
-                     shard_spec)
+                     default_engine, is_transh, rank_link_prediction, rank_link_prediction_transh,
+                     rank_relation_prediction, relation_groups, score_triples_entity_sharded, shard_spec)
 from .exceptions import NotYetEvaluatedError
 
 
@@ -83,6 +83,13 @@ class LinkPredictionEvaluator(object):
         t_d = tails.to(dev, non_blocking=True)
         r_d = rels.to(dev, non_blocking=True)
         stats = {"h2d_bytes": 8 * 3 * n_here, "d2h_bytes": 8 * (4 * kg.n_facts + 1)}
+        transh = is_transh(self.model)
+        if transh:
+            # TransH ranks the facts relation by relation: everything below, filter sets included, runs on
+            # the facts sorted by relation; the ranks go back to fact order at the end
+            order, order_host, groups = relation_groups(r_d, spec.n_rel)
+            heads, tails, rels = heads[order_host], tails[order_host], rels[order_host]
+            h_d, t_d, r_d = h_d[order], t_d[order], r_d[order]
 
         # Filter sets -> CSR (same per-row semantics as get_true_targets).  Built lazily: the
         # engine asks for them after the dense scans are enqueued, so host work overlaps the GPU.
@@ -121,11 +128,20 @@ class LinkPredictionEvaluator(object):
             csr_tail = from_dicts("tail", heads, rels, tails)
             csr_head = from_dicts("head", tails, rels, heads)
         engine = default_engine()
-        lazy = rank_link_prediction(spec, h_d, t_d, r_d, csr_tail, csr_head, shard=eshard,
-                                    engine=engine, chunk=DEFAULT_CHUNK, sync=False)
+        if transh:
+            lazy = rank_link_prediction_transh(spec, h_d, t_d, r_d, groups, csr_tail, csr_head, engine=engine,
+                                               chunk=DEFAULT_CHUNK, sync=False)
+        else:
+            lazy = rank_link_prediction(spec, h_d, t_d, r_d, csr_tail, csr_head, shard=eshard,
+                                        engine=engine, chunk=DEFAULT_CHUNK, sync=False)
 
         def to_host(ranks, flag):
             flag = torch.zeros(1, dtype=torch.int64, device=dev) if flag is None else flag.long().view(1)
+            if transh:         # back to fact order
+                unsorted = [torch.empty_like(x) for x in ranks]
+                for u, x in zip(unsorted, ranks):
+                    u[order] = x
+                ranks = unsorted
             if qshard is not None:
                 ranks = qshard.all_gather(ranks)
                 flag = qshard.all_reduce_sum(flag)   # every rank takes the same decision below
@@ -202,7 +218,7 @@ class RelationPredictionEvaluator(object):
 
     Parameters
     ----------
-    model: TransE (L1/L2), DistMult, RESCAL, ComplEx or Analogy model on a CUDA device.
+    model: TransE (L1/L2), TransH, DistMult, RESCAL, ComplEx or Analogy model on a CUDA device.
     knowledge_graph: object exposing ``n_facts, head_idx, tail_idx, relations, dict_of_rels``.
     directed: bool (default True).  False: both (h, ?, t) and (t, ?, h) are scored and ranked
         together against the directed true score (evaluation.py:99-107).
@@ -310,6 +326,8 @@ class TripletClassificationEvaluator(object):
 
     def __init__(self, model, kg_val, kg_test, *, shard=None):
         from .sampling import PositionalNegativeSampler
+        if shard is not None and is_transh(model):
+            raise NotImplementedError("TransHModel does not support shard= (EntityShard / QueryShard)")
         self.model = model
         self.kg_val = kg_val
         self.kg_test = kg_test

@@ -2,8 +2,8 @@
 and method signatures (torchkge/models/interfaces.py, translation.py:18-125,
 bilinear.py:14-267, 414-556), whose scoring bodies are calls into the CUDA engine.
 
-Only what lies on the hot path is here: TransE (L1 / L2), TorusE, DistMult, RESCAL, ComplEx, Analogy
-and the RotatE addition.  ``state_dict`` keys equal the reference's, so weights move freely between
+Only what lies on the hot path is here: TransE (L1 / L2), TransH, TorusE, DistMult, RESCAL, ComplEx,
+Analogy and the RotatE addition.  ``state_dict`` keys equal the reference's, so weights move freely between
 the two packages.  The pre-0.17 method names ``lp_prep_cands`` / ``lp_scoring_function``
 (docs/history.rst:37-42) are kept as aliases.
 """
@@ -263,6 +263,71 @@ class TransEModel(TranslationModel):
         h, t, r = self.ent_emb(h_idx), self.ent_emb(t_idx), self.rel_emb(r_idx)
         cands = self._expand(self.ent_emb.weight if entities else self.rel_emb.weight, b)
         return h, t, r, cands
+
+
+class TransHModel(TranslationModel):
+    """TransH (Wang et al. 2014) -- torchkge/models/translation.py:128-284: TransE-L2 between the
+    projections of h and t on a relation-specific hyperplane of normal vector ``norm_vect``.
+
+    There is no ``projected_entities`` cache: the reference fills an (n_rel, n_ent, emb_dim) tensor
+    (translation.py:179-181, 270-284), 8 GB at FB15k's size.  Link prediction and ``EntityInference``
+    project the entity table on the GPU for one relation at a time, on every call; relation prediction
+    and ``RelationInference`` project the two rows of each fact on the fly.  A reference checkpoint
+    loads here with the default ``strict=True`` (its ``projected_entities`` entry is discarded); this
+    model's ``state_dict`` loads into the reference with ``strict=False``.
+
+    ``inference_prepare_candidates`` / ``inference_scoring_function`` are not available: the
+    reference's entity candidates are a per-row (b, n_ent, emb_dim) tensor.  Use
+    ``LinkPredictionEvaluator``, ``RelationPredictionEvaluator``, ``EntityInference`` or
+    ``RelationInference``.  Out of scope: the fused training step and ``shard=``.
+    """
+
+    def __init__(self, emb_dim, n_entities, n_relations):
+        super().__init__(n_entities, n_relations, dissimilarity_type='L2')
+        self.emb_dim = emb_dim
+        self.ent_emb = init_embedding(self.n_ent, self.emb_dim)
+        self.rel_emb = init_embedding(self.n_rel, self.emb_dim)
+        self.norm_vect = init_embedding(self.n_rel, self.emb_dim)
+        self.normalize_parameters()
+        self.evaluated_projections = False
+
+    def scoring_function(self, h_idx, t_idx, r_idx):
+        """-||P(h~) + r - P(t~)||^2 with h, t and the normal vector L2-normalised (translation.py:183-198),
+        on the per-triple kernels kge_transh_score_triples_fwd / _bwd."""
+        self.evaluated_projections = False
+        from .training import score_triples_transh
+        return score_triples_transh(self, h_idx, t_idx, r_idx)
+
+    @staticmethod
+    def project(ent, norm_vect):
+        return ent - (ent * norm_vect).sum(dim=1).view(-1, 1) * norm_vect
+
+    def normalize_parameters(self):
+        self.ent_emb.weight.data = normalize(self.ent_emb.weight.data, p=2, dim=1)
+        self.norm_vect.weight.data = normalize(self.norm_vect.weight.data, p=2, dim=1)
+        self.rel_emb.weight.data = self.project(self.rel_emb.weight.data, self.norm_vect.weight.data)
+
+    def get_embeddings(self):
+        self.normalize_parameters()
+        return self.ent_emb.weight.data, self.rel_emb.weight.data, self.norm_vect.weight.data
+
+    def inference_prepare_candidates(self, h_idx, t_idx, r_idx, entities=True):
+        raise NotImplementedError(
+            "TransHModel has no inference_prepare_candidates: the reference's candidates are a per-row "
+            "(b, n_ent, emb_dim) tensor of projected entities.  Use LinkPredictionEvaluator, "
+            "RelationPredictionEvaluator, EntityInference or RelationInference, which project on the GPU.")
+
+    def inference_scoring_function(self, h, t, r):
+        raise NotImplementedError(
+            "TransHModel has no inference_scoring_function: use LinkPredictionEvaluator, "
+            "RelationPredictionEvaluator, EntityInference or RelationInference.")
+
+    def _load_from_state_dict(self, state_dict, prefix, local_metadata, strict, missing_keys, unexpected_keys,
+                              error_msgs):
+        # a reference checkpoint carries its (n_rel, n_ent, emb_dim) projection cache: not a parameter here
+        state_dict.pop(prefix + "projected_entities", None)
+        super()._load_from_state_dict(state_dict, prefix, local_metadata, strict, missing_keys, unexpected_keys,
+                                      error_msgs)
 
 
 class DistMultModel(BilinearModel):

@@ -125,6 +125,45 @@ def score_triples(model, h_idx, t_idx, r_idx):
     return _ScoreTriples.apply(code, _kernel_dim(model, code), h_idx, t_idx, r_idx, ent0, ent1, rel0, rel1)
 
 
+class _TransHScoreTriples(torch.autograd.Function):
+    """TransH's scoring_function on kge_transh_score_triples_fwd / _bwd (translation.py:183-202)."""
+
+    @staticmethod
+    def forward(ctx, dim, h, t, r, ent, rel, norm_vect):
+        tables = [x.detach().contiguous() for x in (ent, rel, norm_vect)]
+        for x in tables:
+            if x.dtype != torch.float32:
+                raise TypeError("embedding tables must be float32, got %s" % x.dtype)
+        _check_cuda(tables[0], h, t, r)
+        dev = tables[0].device
+        h, t, r = _idx(h, dev), _idx(t, dev), _idx(r, dev)
+        out = torch.empty(h.shape[0], dtype=torch.float32, device=dev)
+        _lib.check(_lib.load().kge_transh_score_triples_fwd(*(_ptr(x) for x in tables), dim, _ptr(h), _ptr(t),
+                                                            _ptr(r), h.shape[0], _ptr(out), _stream(dev)),
+                   "kge_transh_score_triples_fwd")
+        ctx.dim = dim
+        ctx.save_for_backward(h, t, r, *tables)
+        return out
+
+    @staticmethod
+    def backward(ctx, gout):
+        h, t, r, *tables = ctx.saved_tensors
+        grads = [torch.zeros_like(x) for x in tables]
+        gout = gout.contiguous().float()
+        _lib.check(_lib.load().kge_transh_score_triples_bwd(*(_ptr(x) for x in tables), *(_ptr(g) for g in grads),
+                                                            ctx.dim, _ptr(h), _ptr(t), _ptr(r), h.shape[0],
+                                                            _ptr(gout), _stream(h.device)),
+                   "kge_transh_score_triples_bwd")
+        return (None, None, None, None, *grads)
+
+
+def score_triples_transh(model, h_idx, t_idx, r_idx):
+    """TransH's ``scoring_function(h_idx, t_idx, r_idx)`` -> (n,) float scores, differentiable with respect
+    to ent_emb, rel_emb and norm_vect."""
+    return _TransHScoreTriples.apply(model.emb_dim, h_idx, t_idx, r_idx, model.ent_emb.weight,
+                                     model.rel_emb.weight, model.norm_vect.weight)
+
+
 class _MarginLoss(torch.autograd.Function):
     @staticmethod
     def forward(ctx, pos, neg, margin):
@@ -478,8 +517,16 @@ def _positional_csr(positional, n_rel, dev):
     return tuple(_idx(x, dev) for x in positional)
 
 
+def refuse_transh_fused_step(model):
+    """TransH has per-triple kernels (score_triples_transh) but no fused training step."""
+    if type(model).__name__ == "TransHModel":
+        raise NotImplementedError("TransHModel has no fused training step: train it with model(h, t, r, nh, nt), "
+                                  "a loss and backward()")
+
+
 def _fused_step(model, heads, tails, relations, loss_kind, margin, n_neg, negatives, bern_probs, seed, offset,
                 shard, rel_share=None, positional=None):
+    refuse_transh_fused_step(model)
     if negatives is not None and len(negatives) not in (2, 3):
         raise ValueError("negatives must be (neg_heads, neg_tails) or (neg_heads, neg_tails, neg_rels)")
     if positional is not None and negatives is not None:
