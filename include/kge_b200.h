@@ -326,6 +326,14 @@ int kge_rescal_rel_scores(const float* hrows, const float* trows, const float* r
  * dim <= 8192. */
 int kge_transh_rel_scores(const float* hrows, const float* trows, const float* rel, const float* norm_vect,
                           int dim, int64_t n, int64_t n_rel, float* scores, void* stream);
+/* TransD relation prediction (models/interfaces.py:261-272 with the projections of
+ * models/translation.py:645-646): scores[i][c] = -||(P_c(h_i) + r_c) - P_c(t_i)||^2, where
+ * P_c(e)[j] = fl(fl(s_e * rel_proj[c][j]) + e[j]) as kge_transd_project computes it and the norm is summed in
+ * ATen's L2-norm order.  hrows / trows: [n][rel_dim] the first rel_dim coordinates of the raw ent_emb rows,
+ * hs / ts: [n] their scalars (kge_transd_entity_scalars), rel / rel_proj: [n_rel][rel_dim] (rel_emb.weight,
+ * rel_proj_vect.weight), scores: [n][n_rel] out, for kge_rank_dense / kge_topk_dense.  rel_dim <= 8192. */
+int kge_transd_rel_scores(const float* hrows, const float* hs, const float* trows, const float* ts, const float* rel,
+                          const float* rel_proj, int rel_dim, int64_t n, int64_t n_rel, float* scores, void* stream);
 /* get_rank + filter_scores (utils/operations.py:37-61, utils/modeling.py:91-102) on a dense (n, n_cand)
  * score matrix, counters ADDED INTO as by kge_rank_side: raw_count[i] += #{c : s >= s_true};
  * filt_sub[i] += listed candidates with s >= s_true (minus the -inf quirk).  s_true = true_score_in[i]
@@ -360,6 +368,20 @@ typedef struct {
  * kge_topk_side as a KGE_TRANSE_L2 table.  dim <= 8192. */
 int kge_transh_project(const float* ent, const float* norm_row, int64_t n_rows, int dim, float* out,
                        void* stream);
+/* TransD's per-entity scalar (models/translation.py:645, evaluate_projectionss):
+ * s[e] = (ent_proj[e] * ent[e]).sum() summed over ent_dim in ATen's inner-dimension order.  ent / ent_proj:
+ * [n_rows][ent_dim] raw ent_emb.weight / ent_proj_vect.weight, s: [n_rows] out.  It does not depend on the
+ * relation: one call serves every kge_transd_project of an evaluation.  ent_dim <= 8192. */
+int kge_transd_entity_scalars(const float* ent, const float* ent_proj, int64_t n_rows, int ent_dim, float* s,
+                              void* stream);
+/* TransD's projected entity table for one relation (models/translation.py:646):
+ * out[e][j] = fl(fl(s[e] * rel_proj_row[j]) + ent[e][j]) for j < rel_dim, two roundings as in the reference.
+ * ent: [n_rows][ent_dim] raw ent_emb.weight (read with row stride ent_dim), s: [n_rows] from
+ * kge_transd_entity_scalars, rel_proj_row: [rel_dim] raw rel_proj_vect.weight row, out: [n_rows][rel_dim]
+ * (caller-provided).  The result feeds the scans as a KGE_TRANSE_L2 table of width rel_dim.
+ * rel_dim <= ent_dim <= 8192. */
+int kge_transd_project(const float* ent, int ent_dim, const float* s, const float* rel_proj_row, int64_t n_rows,
+                       int rel_dim, float* out, void* stream);
 
 /* Model.scoring_function (models/translation.py:69-81, models/bilinear.py:60-71, 188-199,
  * 460-473): scores[i] of triple (h[i], r[i], t[i]); TransE / DistMult / RESCAL L2-normalise
@@ -381,6 +403,19 @@ int kge_transh_score_triples_bwd(const float* ent, const float* rel, const float
                                  float* grad_rel, float* grad_norm_vect, int dim, const int64_t* h,
                                  const int64_t* t, const int64_t* r, int64_t n, const float* grad_scores,
                                  void* stream);
+
+/* TransD's scoring_function (models/translation.py:538-568): scores[i] = -||P(h~) + r~ - P(t~)||^2 with h~,
+ * t~, r~ and the three projection vectors L2-normalised (eps 1e-12) and P(e~)[j] = (e~ . ep~) rp~[j] + e~[j] for
+ * j < rel_dim.  Its own tables: ent / ent_proj [n_ent][ent_dim] (ent_emb.weight, ent_proj_vect.weight), rel /
+ * rel_proj [n_rel][rel_dim] (rel_emb.weight, rel_proj_vect.weight).  rel_dim <= ent_dim <= 8192. */
+int kge_transd_score_triples_fwd(const float* ent, const float* rel, const float* ent_proj, const float* rel_proj,
+                                 int ent_dim, int rel_dim, const int64_t* h, const int64_t* t, const int64_t* r,
+                                 int64_t n, float* scores, void* stream);
+/* accumulates d(sum_i grad_scores[i] * scores[i]) / d(tables) into the four gradient tables */
+int kge_transd_score_triples_bwd(const float* ent, const float* rel, const float* ent_proj, const float* rel_proj,
+                                 float* grad_ent, float* grad_rel, float* grad_ent_proj, float* grad_rel_proj,
+                                 int ent_dim, int rel_dim, const int64_t* h, const int64_t* t, const int64_t* r,
+                                 int64_t n, const float* grad_scores, void* stream);
 
 /* BernoulliNegativeSampler.corrupt_batch (sampling.py:278-327): nh/nt of length b*n_neg laid
  * out as n_neg blocks of the batch; negative j of fact i corrupts the head with probability

@@ -8,7 +8,7 @@ from .exceptions import (NotYetEvaluatedError, NotYetImplementedError, SanityErr
                          SizeMismatchError, WrongArgumentsError, WrongDimensionError)
 from .data import KnowledgeGraph  # noqa: F401
 from .models import (AnalogyModel, ComplExModel, DistMultModel, RESCALModel, RotatEModel,  # noqa: F401
-                     TorusEModel, TransEModel, TransHModel)
+                     TorusEModel, TransDModel, TransEModel, TransHModel)
 from .evaluation import (LinkPredictionEvaluator, RelationPredictionEvaluator,  # noqa: F401
                          TripletClassificationEvaluator)
 from .inference import EntityInference, RelationInference  # noqa: F401

@@ -143,6 +143,9 @@ SIGNATURES = {
     "kge_rescal_rel_scores": (_c.c_int, [_p, _p, _p, _c.c_int, _c.c_int64, _c.c_int64, _p, _p]),
     "kge_transh_rel_scores": (_c.c_int, [_p, _p, _p, _p, _c.c_int, _c.c_int64, _c.c_int64, _p, _p]),
     "kge_transh_project": (_c.c_int, [_p, _p, _c.c_int64, _c.c_int, _p, _p]),
+    "kge_transd_entity_scalars": (_c.c_int, [_p, _p, _c.c_int64, _c.c_int, _p, _p]),
+    "kge_transd_project": (_c.c_int, [_p, _c.c_int, _p, _p, _c.c_int64, _c.c_int, _p, _p]),
+    "kge_transd_rel_scores": (_c.c_int, [_p, _p, _p, _p, _p, _p, _c.c_int, _c.c_int64, _c.c_int64, _p, _p]),
     "kge_rank_dense": (_c.c_int, [_p, _c.c_int64, _c.c_int64, _p, _p, _p, _p, _p, _p, _p, _p]),
     "kge_topk_dense_workspace_bytes": (_c.c_size_t, [_c.c_int64, _c.c_int64, _c.c_int]),
     "kge_topk_dense": (_c.c_int, [_p, _c.c_int64, _c.c_int64, _c.c_int, _p, _p, _p, _p, _p, _c.c_size_t, _p]),
@@ -152,6 +155,10 @@ SIGNATURES = {
     "kge_transh_score_triples_fwd": (_c.c_int, [_p, _p, _p, _c.c_int, _p, _p, _p, _c.c_int64, _p, _p]),
     "kge_transh_score_triples_bwd": (_c.c_int, [_p, _p, _p, _p, _p, _p, _c.c_int, _p, _p, _p, _c.c_int64, _p,
                                                 _p]),
+    "kge_transd_score_triples_fwd": (_c.c_int, [_p, _p, _p, _p, _c.c_int, _c.c_int, _p, _p, _p, _c.c_int64, _p,
+                                                _p]),
+    "kge_transd_score_triples_bwd": (_c.c_int, [_p, _p, _p, _p, _p, _p, _p, _p, _c.c_int, _c.c_int, _p, _p, _p,
+                                                _c.c_int64, _p, _p]),
     "kge_corrupt_batch": (_c.c_int, [_p, _p, _p, _c.c_int64, _c.c_int32, _p, _c.c_int64,
                                      _c.c_uint64, _c.c_uint64, _p, _p, _p]),
     "kge_margin_loss_fwd": (_c.c_int, [_p, _p, _c.c_int64, _c.c_float, _p, _p]),

@@ -758,6 +758,45 @@ int kge_transh_project(const float* ent, const float* norm_row, int64_t n_rows, 
   return KGE_OK;
 }
 
+int kge_transd_entity_scalars(const float* ent, const float* ent_proj, int64_t n_rows, int ent_dim, float* s,
+                              void* stream) {
+  if (n_rows == 0) return KGE_OK;
+  if (n_rows < 0 || ent_dim < 1 || !ent || !ent_proj || !s)
+    return fail(KGE_ERR_ARG, "kge_transd_entity_scalars: bad argument");
+  if (ent_dim > kge::SCAN_MAX_DIM) return fail(KGE_ERR_UNSUPPORTED, "kge_transd_entity_scalars: ent_dim > 8192");
+  DeviceScope device_scope(s);
+  KGE_CUDA_TRY(kge::launch_transd_entity_scalars(ent, ent_proj, n_rows, ent_dim, s, static_cast<cudaStream_t>(stream)),
+               "transd_entity_scalars");
+  return KGE_OK;
+}
+
+int kge_transd_project(const float* ent, int ent_dim, const float* s, const float* rel_proj_row, int64_t n_rows,
+                       int rel_dim, float* out, void* stream) {
+  if (n_rows == 0) return KGE_OK;
+  if (n_rows < 0 || rel_dim < 1 || ent_dim < 1 || !ent || !s || !rel_proj_row || !out)
+    return fail(KGE_ERR_ARG, "kge_transd_project: bad argument");
+  if (rel_dim > ent_dim) return fail(KGE_ERR_ARG, "kge_transd_project: rel_dim > ent_dim");
+  if (ent_dim > kge::SCAN_MAX_DIM) return fail(KGE_ERR_UNSUPPORTED, "kge_transd_project: ent_dim > 8192");
+  DeviceScope device_scope(out);
+  KGE_CUDA_TRY(kge::launch_transd_project(ent, ent_dim, s, rel_proj_row, n_rows, rel_dim, out,
+                                          static_cast<cudaStream_t>(stream)),
+               "transd_project");
+  return KGE_OK;
+}
+
+int kge_transd_rel_scores(const float* hrows, const float* hs, const float* trows, const float* ts, const float* rel,
+                          const float* rel_proj, int rel_dim, int64_t n, int64_t n_rel, float* scores, void* stream) {
+  if (n == 0 || n_rel == 0) return KGE_OK;
+  if (n < 0 || n_rel < 0 || rel_dim < 1 || !hrows || !hs || !trows || !ts || !rel || !rel_proj || !scores)
+    return fail(KGE_ERR_ARG, "kge_transd_rel_scores: bad argument");
+  if (rel_dim > kge::SCAN_MAX_DIM) return fail(KGE_ERR_UNSUPPORTED, "kge_transd_rel_scores: rel_dim > 8192");
+  DeviceScope device_scope(scores);
+  KGE_CUDA_TRY(kge::launch_transd_rel_scores(hrows, hs, trows, ts, rel, rel_proj, rel_dim, n, n_rel, scores,
+                                             static_cast<cudaStream_t>(stream)),
+               "transd_rel_scores");
+  return KGE_OK;
+}
+
 int kge_rank_dense(const float* scores, int64_t n, int64_t n_cand, const int64_t* true_idx,
                    const float* true_score_in, const int64_t* filt_offs, const int64_t* filt_ids,
                    int32_t* raw_count, int32_t* filt_sub, float* true_score, void* stream) {
@@ -971,6 +1010,44 @@ int kge_transh_score_triples_bwd(const float* ent, const float* rel, const float
   KGE_CUDA_TRY(kge::launch_transh_score_bwd(ent, rel, norm_vect, grad_ent, grad_rel, grad_norm_vect, dim, h, t, r,
                                             n, grad_scores, static_cast<cudaStream_t>(stream)),
                "transh_score_triples_bwd");
+  return KGE_OK;
+}
+
+// TransD's widths: rel_dim <= ent_dim (the reference's projection fails otherwise), both within SCAN_MAX_DIM
+static int transd_widths(int ent_dim, int rel_dim, const char* fn) {
+  if (ent_dim < 1 || rel_dim < 1 || rel_dim > ent_dim) return fail(KGE_ERR_ARG, fn, "need 1 <= rel_dim <= ent_dim");
+  if (ent_dim > kge::SCAN_MAX_DIM) return fail(KGE_ERR_UNSUPPORTED, fn, "ent_dim > 8192");
+  return KGE_OK;
+}
+
+int kge_transd_score_triples_fwd(const float* ent, const float* rel, const float* ent_proj, const float* rel_proj,
+                                 int ent_dim, int rel_dim, const int64_t* h, const int64_t* t, const int64_t* r,
+                                 int64_t n, float* scores, void* stream) {
+  if (n == 0) return KGE_OK;
+  if (n < 0 || !ent || !rel || !ent_proj || !rel_proj || !h || !t || !r || !scores)
+    return fail(KGE_ERR_ARG, "kge_transd_score_triples_fwd: bad argument");
+  if (int e = transd_widths(ent_dim, rel_dim, "kge_transd_score_triples_fwd")) return e;
+  DeviceScope device_scope(ent);
+  KGE_CUDA_TRY(kge::launch_transd_score_fwd(ent, rel, ent_proj, rel_proj, ent_dim, rel_dim, h, t, r, n, scores,
+                                            static_cast<cudaStream_t>(stream)),
+               "transd_score_triples_fwd");
+  return KGE_OK;
+}
+
+int kge_transd_score_triples_bwd(const float* ent, const float* rel, const float* ent_proj, const float* rel_proj,
+                                 float* grad_ent, float* grad_rel, float* grad_ent_proj, float* grad_rel_proj,
+                                 int ent_dim, int rel_dim, const int64_t* h, const int64_t* t, const int64_t* r,
+                                 int64_t n, const float* grad_scores, void* stream) {
+  if (n == 0) return KGE_OK;
+  if (n < 0 || !ent || !rel || !ent_proj || !rel_proj || !grad_ent || !grad_rel || !grad_ent_proj ||
+      !grad_rel_proj || !h || !t || !r || !grad_scores)
+    return fail(KGE_ERR_ARG, "kge_transd_score_triples_bwd: bad argument");
+  if (int e = transd_widths(ent_dim, rel_dim, "kge_transd_score_triples_bwd")) return e;
+  DeviceScope device_scope(ent);
+  KGE_CUDA_TRY(kge::launch_transd_score_bwd(ent, rel, ent_proj, rel_proj, grad_ent, grad_rel, grad_ent_proj,
+                                            grad_rel_proj, ent_dim, rel_dim, h, t, r, n, grad_scores,
+                                            static_cast<cudaStream_t>(stream)),
+               "transd_score_triples_bwd");
   return KGE_OK;
 }
 

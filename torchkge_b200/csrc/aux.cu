@@ -401,6 +401,35 @@ __global__ void __launch_bounds__(256) transh_project_kernel(const float* __rest
   for (int k = lane; k < dim; k += 32) o[k] = transh_project_elem(e[k], nc, w[k]);
 }
 
+// TransD: s[row] = (ent_proj[row] * ent[row]).sum() in ATen's order (reduce.cuh: transd_project_elem).
+// One warp per row.
+__global__ void __launch_bounds__(256) transd_scalars_kernel(const float* __restrict__ ent,
+                                                             const float* __restrict__ ent_proj, long long n_rows,
+                                                             int dim, float* __restrict__ s) {
+  const long long row = ((long long)blockIdx.x * blockDim.x + threadIdx.x) >> 5;
+  const int lane = threadIdx.x & 31;
+  if (row >= n_rows) return;   // whole warps leave together: the shuffles below see full warps
+  const float* e = ent + (size_t)row * dim;
+  const float* p = ent_proj + (size_t)row * dim;
+  const float v = dim < 8 ? pair_score_natural<EL_DOT1>(dim, p, p, e, e)
+                          : pair_score_chains<EL_DOT1>(dim, p, p, e, e, lane);
+  if (lane == 0) s[row] = v;
+}
+
+// TransD: out[row][j] = transd_project_elem(ent[row][j], s[row], rp[j]) for j < rel_dim, the entity rows
+// read with their own stride ent_dim.  Element-wise: one thread per output element.
+__global__ void __launch_bounds__(256) transd_project_kernel(const float* __restrict__ ent, int ent_dim,
+                                                             const float* __restrict__ s,
+                                                             const float* __restrict__ rp, long long total,
+                                                             int rel_dim, float* __restrict__ out) {
+  const long long stride = (long long)gridDim.x * blockDim.x;
+  for (long long x = (long long)blockIdx.x * blockDim.x + threadIdx.x; x < total; x += stride) {
+    const long long row = x / rel_dim;
+    const int j = (int)(x - row * rel_dim);
+    out[x] = transd_project_elem(ent[(size_t)row * ent_dim + j], s[row], rp[j]);
+  }
+}
+
 inline unsigned filter_blocks(long long n_filt) {
   const long long want = (n_filt + 3) / 4;  // >= one warp per entry group; grid-stride beyond
   return (unsigned)(want < 1 ? 1 : (want > 132LL * 64 ? 132LL * 64 : want));   // 64 blocks per H100 SM
@@ -492,6 +521,23 @@ cudaError_t launch_transh_project(const float* ent, const float* w, int64_t n_ro
                                   cudaStream_t stream) {
   if (n_rows <= 0) return cudaSuccess;
   transh_project_kernel<<<blocks_for(n_rows * 32, 256), 256, 0, stream>>>(ent, w, n_rows, dim, out);
+  return cudaGetLastError();
+}
+
+cudaError_t launch_transd_entity_scalars(const float* ent, const float* ent_proj, int64_t n_rows, int ent_dim,
+                                         float* s, cudaStream_t stream) {
+  if (n_rows <= 0) return cudaSuccess;
+  transd_scalars_kernel<<<blocks_for(n_rows * 32, 256), 256, 0, stream>>>(ent, ent_proj, n_rows, ent_dim, s);
+  return cudaGetLastError();
+}
+
+cudaError_t launch_transd_project(const float* ent, int ent_dim, const float* s, const float* rel_proj_row,
+                                  int64_t n_rows, int rel_dim, float* out, cudaStream_t stream) {
+  const long long total = (long long)n_rows * rel_dim;
+  if (total <= 0) return cudaSuccess;
+  const long long want = blocks_for(total, 256);
+  const unsigned blocks = (unsigned)(want > 132LL * 16 ? 132LL * 16 : want);   // grid-stride past 16 per SM
+  transd_project_kernel<<<blocks, 256, 0, stream>>>(ent, ent_dim, s, rel_proj_row, total, rel_dim, out);
   return cudaGetLastError();
 }
 

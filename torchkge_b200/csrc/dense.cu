@@ -84,6 +84,56 @@ __global__ void transh_rel_scores_kernel(const float* __restrict__ hrows, const 
   if (lane == 0) scores[(size_t)i * n_rel + c] = s;
 }
 
+// TransD relation case (interfaces.py:261-272 with the projections of translation.py:645-646), laid out as
+// transh_rel_scores_kernel: hrows / trows hold the first dim (= rel_emb_dim) coordinates of the raw entity
+// rows and hs / ts their scalars s, so P_c(e)[j] = transd_project_elem(e[j], s_e, rel_proj[c][j]).
+__global__ void transd_rel_scores_kernel(const float* __restrict__ hrows, const float* __restrict__ hs,
+                                         const float* __restrict__ trows, const float* __restrict__ ts,
+                                         const float* __restrict__ rel, const float* __restrict__ rel_proj,
+                                         int dim, long long n, long long n_rel, float* __restrict__ scores) {
+  extern __shared__ float sm[];       // per warp: [dim] P_c(h), then [dim] P_c(t)
+  const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
+  const long long c = blockIdx.x;
+  const long long i = (long long)blockIdx.y * (blockDim.x >> 5) + warp;
+  if (i >= n) return;
+  float* ph = sm + (size_t)warp * 2 * dim;
+  float* pt = ph + dim;
+  const float* rp = rel_proj + (size_t)c * dim;
+  const float* r = rel + (size_t)c * dim;
+  const float* h = hrows + (size_t)i * dim;
+  const float* t = trows + (size_t)i * dim;
+  const float sh = hs[i], st = ts[i];
+  for (int k = lane; k < dim; k += 32) {
+    ph[k] = transd_project_elem(h[k], sh, rp[k]);
+    pt[k] = transd_project_elem(t[k], st, rp[k]);
+  }
+  __syncwarp();
+  const float s = pair_score_chains<EL_L2_HEAD>(dim, r, pt, ph, ph, lane);
+  if (lane == 0) scores[(size_t)i * n_rel + c] = s;
+}
+
+// Grid of the per-relation projection kernels above: up to 8 warps (facts) per CTA within 48 KB of shared
+// memory, one warp past dim 6144.  launch(grid, threads, smem, i_off) enqueues the facts from i_off on.
+template <auto Kernel, typename Launch>
+cudaError_t launch_projected_rel_scores(int dim, int64_t n, int64_t n_rel, Launch launch) {
+  if (n <= 0 || n_rel <= 0) return cudaSuccess;
+  const size_t per_warp = (size_t)2 * dim * sizeof(float);
+  long long warps = (long long)(48 * 1024 / per_warp);
+  warps = warps < 1 ? 1 : (warps > 8 ? 8 : warps);
+  const size_t smem = (size_t)warps * per_warp;
+  if (smem > 200 * 1024) return cudaErrorInvalidValue;
+  if (smem > 48 * 1024) {
+    const cudaError_t e = set_attribute_once<Kernel>(cudaFuncAttributeMaxDynamicSharedMemorySize, 200 * 1024);
+    if (e != cudaSuccess) return e;
+  }
+  const long long i_tiles = (n + warps - 1) / warps;
+  for (long long y0 = 0; y0 < i_tiles; y0 += 65535) {     // gridDim.y limit
+    const long long ny = i_tiles - y0 < 65535 ? i_tiles - y0 : 65535;
+    launch(dim3((unsigned)n_rel, (unsigned)ny), (unsigned)(32 * warps), smem, y0 * warps);
+  }
+  return cudaGetLastError();
+}
+
 // One warp per row of a dense (n, n_c) score matrix:
 //   raw_count[i] += #{c : s[i][c] >= s_true(i)},
 //   filt_sub[i]  += sum over the row's CSR entries of [s[i][c] >= s_true(i)] - [s_true(i) == -inf]
@@ -153,28 +203,23 @@ cudaError_t launch_rescal_rel_scores(const float* hrows, const float* trows, con
 cudaError_t launch_transh_rel_scores(const float* hrows, const float* trows, const float* rel,
                                      const float* norm_vect, int dim, int64_t n, int64_t n_rel, float* scores,
                                      cudaStream_t stream) {
-  if (n <= 0 || n_rel <= 0) return cudaSuccess;
-  // up to 8 warps (facts) per CTA within 48 KB of shared memory; one warp past dim 6144
-  const size_t per_warp = (size_t)2 * dim * sizeof(float);
-  long long warps = (long long)(48 * 1024 / per_warp);
-  warps = warps < 1 ? 1 : (warps > 8 ? 8 : warps);
-  const size_t smem = (size_t)warps * per_warp;
-  if (smem > 200 * 1024) return cudaErrorInvalidValue;
-  if (smem > 48 * 1024) {
-    const cudaError_t e =
-        set_attribute_once<transh_rel_scores_kernel>(cudaFuncAttributeMaxDynamicSharedMemorySize, 200 * 1024);
-    if (e != cudaSuccess) return e;
-  }
-  const long long i_tiles = (n + warps - 1) / warps;
-  for (long long y0 = 0; y0 < i_tiles; y0 += 65535) {     // gridDim.y limit
-    const long long ny = i_tiles - y0 < 65535 ? i_tiles - y0 : 65535;
-    dim3 grid((unsigned)n_rel, (unsigned)ny);
-    const long long i_off = y0 * warps;
-    transh_rel_scores_kernel<<<grid, (unsigned)(32 * warps), smem, stream>>>(
-        hrows + (size_t)i_off * dim, trows + (size_t)i_off * dim, rel, norm_vect, dim, n - i_off, n_rel,
-        scores + (size_t)i_off * n_rel);
-  }
-  return cudaGetLastError();
+  return launch_projected_rel_scores<transh_rel_scores_kernel>(
+      dim, n, n_rel, [&](dim3 grid, unsigned threads, size_t smem, long long i_off) {
+        transh_rel_scores_kernel<<<grid, threads, smem, stream>>>(
+            hrows + (size_t)i_off * dim, trows + (size_t)i_off * dim, rel, norm_vect, dim, n - i_off, n_rel,
+            scores + (size_t)i_off * n_rel);
+      });
+}
+
+cudaError_t launch_transd_rel_scores(const float* hrows, const float* hs, const float* trows, const float* ts,
+                                     const float* rel, const float* rel_proj, int dim, int64_t n, int64_t n_rel,
+                                     float* scores, cudaStream_t stream) {
+  return launch_projected_rel_scores<transd_rel_scores_kernel>(
+      dim, n, n_rel, [&](dim3 grid, unsigned threads, size_t smem, long long i_off) {
+        transd_rel_scores_kernel<<<grid, threads, smem, stream>>>(
+            hrows + (size_t)i_off * dim, hs + i_off, trows + (size_t)i_off * dim, ts + i_off, rel, rel_proj, dim,
+            n - i_off, n_rel, scores + (size_t)i_off * n_rel);
+      });
 }
 
 cudaError_t launch_rank_dense(const float* scores, int64_t n, int64_t n_c, const int64_t* true_idx,

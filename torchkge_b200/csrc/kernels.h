@@ -139,6 +139,13 @@ cudaError_t launch_finalize(const int32_t* raw, const int32_t* sub, int64_t n, i
 // out[row][k] = TransH projection of ent[row] on the hyperplane of normal w (reduce.cuh: transh_project_elem)
 cudaError_t launch_transh_project(const float* ent, const float* w, int64_t n_rows, int dim, float* out,
                                   cudaStream_t stream);
+// s[row] = (ent_proj[row] * ent[row]).sum() in ATen's order: TransD's per-entity scalar
+cudaError_t launch_transd_entity_scalars(const float* ent, const float* ent_proj, int64_t n_rows, int ent_dim,
+                                         float* s, cudaStream_t stream);
+// out[row][j] = TransD projection of ent[row] (row stride ent_dim) under one relation, j < rel_dim
+// (reduce.cuh: transd_project_elem)
+cudaError_t launch_transd_project(const float* ent, int ent_dim, const float* s, const float* rel_proj_row,
+                                  int64_t n_rows, int rel_dim, float* out, cudaStream_t stream);
 
 // ---- top-k selection over collected candidates (topk.cu) ----
 // best[q][k] sorted 64-bit keys (score order, then smaller id first; 0 = empty slot).
@@ -167,6 +174,11 @@ cudaError_t launch_rescal_rel_scores(const float* hrows, const float* trows, con
 cudaError_t launch_transh_rel_scores(const float* hrows, const float* trows, const float* rel,
                                      const float* norm_vect, int dim, int64_t n, int64_t n_rel, float* scores,
                                      cudaStream_t stream);
+// scores[i][c] = -||(P_c(h_i) + r_c) - P_c(t_i)||^2   TransD relation case, P_c from the first dim
+// coordinates of the rows and their scalars hs / ts
+cudaError_t launch_transd_rel_scores(const float* hrows, const float* hs, const float* trows, const float* ts,
+                                     const float* rel, const float* rel_proj, int dim, int64_t n, int64_t n_rel,
+                                     float* scores, cudaStream_t stream);
 cudaError_t launch_rank_dense(const float* scores, int64_t n, int64_t n_c, const int64_t* true_idx,
                               const float* true_score_in, const int64_t* offs, const int64_t* ids,
                               int32_t* raw_count, int32_t* filt_sub, float* true_score_out, cudaStream_t stream);

@@ -393,6 +393,14 @@ __device__ __forceinline__ float transh_project_elem(float e, float nc, float w)
   return __fsub_rn(e, __fmul_rn(nc, w));
 }
 
+// TransD's projection of entity coordinate j < rel_emb_dim under relation r (translation.py:645-646,
+// evaluate_projectionss):  P[j] = fl(fl(s * rp[j]) + e[j])  with  s = (ent_proj_vect[e] * ent_emb[e]).sum()
+// over ent_emb_dim, summed in ATen's inner-dimension order (EL_DOT1 of pair_score_natural / pair_score_chains)
+// and rp = rel_proj_vect[r].  Two roundings: the reference multiplies, then adds, and fuses nothing.
+__device__ __forceinline__ float transd_project_elem(float e, float s, float rp) {
+  return __fadd_rn(__fmul_rn(s, rp), e);
+}
+
 // Exact adjudication of the near-tie band (the list is kept as one region per CTA of the scan).
 // Chain-parallel: the independent chains of the ATen reduction are spread over the lanes of a
 // warp -- 8 lanes per pair for the L2 norm (4 pairs per warp), 32 lanes per pair for the

@@ -497,6 +497,107 @@ __global__ void transh_score_bwd_kernel(const float* __restrict__ ent, const flo
   }
 }
 
+// ---- TransD scoring_function (translation.py:538-568): with h~, t~, r~, hp~, tp~, rp~ the L2-normalised
+// head, tail, relation and their projection vectors, a = h~ . hp~, b = t~ . tp~ (over ent_dim),
+//   x[j] = (a rp~[j] + h~[j]) + r~[j] - (b rp~[j] + t~[j])  for j < rel_dim,   score = -|x|^2.
+// Its own tables (ent, rel, ent_proj, rel_proj) and two widths rather than a model code.
+struct TransDRows {
+  const float* h; const float* t; const float* hp; const float* tp;   // [ent_dim]
+  const float* r; const float* rp;                                     // [rel_dim]
+  float ih, it, ihp, itp, ir, irp;   // 1 / max(|row|, eps)
+  float a, b;                        // h~ . hp~ and t~ . tp~
+};
+
+__device__ __forceinline__ TransDRows transd_rows(const float* ent, const float* rel, const float* ep,
+                                                  const float* rpv, int ent_dim, int rel_dim, long long h,
+                                                  long long t, long long r, int lane) {
+  TransDRows p;
+  p.h = ent + (size_t)h * ent_dim; p.t = ent + (size_t)t * ent_dim;
+  p.hp = ep + (size_t)h * ent_dim; p.tp = ep + (size_t)t * ent_dim;
+  p.r = rel + (size_t)r * rel_dim; p.rp = rpv + (size_t)r * rel_dim;
+  p.ih = inv_norm_of(p.h, ent_dim, lane); p.it = inv_norm_of(p.t, ent_dim, lane);
+  p.ihp = inv_norm_of(p.hp, ent_dim, lane); p.itp = inv_norm_of(p.tp, ent_dim, lane);
+  p.ir = inv_norm_of(p.r, rel_dim, lane); p.irp = inv_norm_of(p.rp, rel_dim, lane);
+  float a = 0.f, b = 0.f;
+  for (int k = lane; k < ent_dim; k += 32) {
+    a = fmaf(p.h[k] * p.ih, p.hp[k] * p.ihp, a);
+    b = fmaf(p.t[k] * p.it, p.tp[k] * p.itp, b);
+  }
+  p.a = warp_sum(a); p.b = warp_sum(b);
+  return p;
+}
+
+__device__ __forceinline__ float transd_x(const TransDRows& p, int j) {
+  const float rpn = p.rp[j] * p.irp;
+  return (p.a * rpn + p.h[j] * p.ih) + p.r[j] * p.ir - (p.b * rpn + p.t[j] * p.it);
+}
+
+__global__ void transd_score_fwd_kernel(const float* __restrict__ ent, const float* __restrict__ rel,
+                                        const float* __restrict__ ep, const float* __restrict__ rpv, int ent_dim,
+                                        int rel_dim, const int64_t* __restrict__ h, const int64_t* __restrict__ t,
+                                        const int64_t* __restrict__ r, long long n, float* __restrict__ out) {
+  const long long w = ((long long)blockIdx.x * blockDim.x + threadIdx.x) >> 5;
+  const int lane = threadIdx.x & 31;
+  if (w >= n) return;
+  const TransDRows p = transd_rows(ent, rel, ep, rpv, ent_dim, rel_dim, h[w], t[w], r[w], lane);
+  float s = 0.f;
+  for (int j = lane; j < rel_dim; j += 32) { const float x = transd_x(p, j); s = fmaf(x, x, s); }
+  s = warp_sum(s);
+  if (lane == 0) out[w] = -s;
+}
+
+// With G = dscore/dx = -2x (rel_dim) and c = rp~ . G:
+//   dscore/dh~ = [G, 0..] + c hp~,   dscore/dhp~ = c h~,   dscore/dt~ = -[G, 0..] - c tp~,   dscore/dtp~ = -c t~,
+//   dscore/dr~ = G,   dscore/drp~ = (a - b) G,
+// each then through F.normalize:  d/dv = (G_v - v~ (v~ . G_v)) / max(|v|, eps), where
+//   h~ . G_h = h~[:rel_dim].G + c a,  hp~ . G_hp = c a,  t~ . G_t = -(t~[:rel_dim].G + c b),  tp~ . G_tp = -c b,
+//   rp~ . G_rp = (a - b) c.
+__global__ void transd_score_bwd_kernel(const float* __restrict__ ent, const float* __restrict__ rel,
+                                        const float* __restrict__ ep, const float* __restrict__ rpv,
+                                        float* __restrict__ g_ent, float* __restrict__ g_rel,
+                                        float* __restrict__ g_ep, float* __restrict__ g_rpv, int ent_dim,
+                                        int rel_dim, const int64_t* __restrict__ h, const int64_t* __restrict__ t,
+                                        const int64_t* __restrict__ r, long long n, const float* __restrict__ gout) {
+  const long long w = ((long long)blockIdx.x * blockDim.x + threadIdx.x) >> 5;
+  const int lane = threadIdx.x & 31;
+  if (w >= n) return;
+  const float g = gout[w];
+  if (g == 0.f) return;
+  const long long hi = h[w], ti = t[w], ri = r[w];
+  const TransDRows p = transd_rows(ent, rel, ep, rpv, ent_dim, rel_dim, hi, ti, ri, lane);
+  float c = 0.f, hg = 0.f, tg = 0.f, rg = 0.f;
+  for (int j = lane; j < rel_dim; j += 32) {
+    const float G = -2.f * transd_x(p, j);
+    c = fmaf(p.rp[j] * p.irp, G, c);
+    hg = fmaf(p.h[j] * p.ih, G, hg);
+    tg = fmaf(p.t[j] * p.it, G, tg);
+    rg = fmaf(p.r[j] * p.ir, G, rg);
+  }
+  c = warp_sum(c); hg = warp_sum(hg); tg = warp_sum(tg); rg = warp_sum(rg);
+  const float dot_h = hg + c * p.a, dot_hp = c * p.a, dot_t = -(tg + c * p.b), dot_tp = -c * p.b;
+  const float dot_rp = (p.a - p.b) * c;
+  float* gh = g_ent + (size_t)hi * ent_dim;
+  float* gt = g_ent + (size_t)ti * ent_dim;
+  float* ghp = g_ep + (size_t)hi * ent_dim;
+  float* gtp = g_ep + (size_t)ti * ent_dim;
+  for (int k = lane; k < ent_dim; k += 32) {
+    const float hn = p.h[k] * p.ih, tn = p.t[k] * p.it, hpn = p.hp[k] * p.ihp, tpn = p.tp[k] * p.itp;
+    const float G = k < rel_dim ? -2.f * transd_x(p, k) : 0.f;
+    atomicAdd(gh + k, g * (G + c * hpn - hn * dot_h) * p.ih);
+    atomicAdd(gt + k, g * (-G - c * tpn - tn * dot_t) * p.it);
+    atomicAdd(ghp + k, g * (c * hn - hpn * dot_hp) * p.ihp);
+    atomicAdd(gtp + k, g * (-c * tn - tpn * dot_tp) * p.itp);
+  }
+  float* gr = g_rel + (size_t)ri * rel_dim;
+  float* grp = g_rpv + (size_t)ri * rel_dim;
+  for (int j = lane; j < rel_dim; j += 32) {
+    const float rn = p.r[j] * p.ir, rpn = p.rp[j] * p.irp;
+    const float G = -2.f * transd_x(p, j);
+    atomicAdd(gr + j, g * (G - rn * rg) * p.ir);
+    atomicAdd(grp + j, g * ((p.a - p.b) * G - rpn * dot_rp) * p.irp);
+  }
+}
+
 // ------------------------------------------------------------------------------------------
 __global__ void score_triples_fwd_kernel(int model, int dim, TrainTables tb,
                                          const int64_t* __restrict__ h,
@@ -1660,6 +1761,25 @@ cudaError_t launch_transh_score_bwd(const float* ent, const float* rel, const fl
   if (n <= 0) return cudaSuccess;
   transh_score_bwd_kernel<<<blocks_for_warps(n), WARPS_PER_BLOCK * 32, 0, st>>>(
       ent, rel, norm_vect, g_ent, g_rel, g_norm_vect, dim, h, t, r, n, gout);
+  return cudaGetLastError();
+}
+
+cudaError_t launch_transd_score_fwd(const float* ent, const float* rel, const float* ent_proj,
+                                    const float* rel_proj, int ent_dim, int rel_dim, const int64_t* h,
+                                    const int64_t* t, const int64_t* r, int64_t n, float* out, cudaStream_t st) {
+  if (n <= 0) return cudaSuccess;
+  transd_score_fwd_kernel<<<blocks_for_warps(n), WARPS_PER_BLOCK * 32, 0, st>>>(ent, rel, ent_proj, rel_proj, ent_dim,
+                                                                                rel_dim, h, t, r, n, out);
+  return cudaGetLastError();
+}
+
+cudaError_t launch_transd_score_bwd(const float* ent, const float* rel, const float* ent_proj,
+                                    const float* rel_proj, float* g_ent, float* g_rel, float* g_ent_proj,
+                                    float* g_rel_proj, int ent_dim, int rel_dim, const int64_t* h, const int64_t* t,
+                                    const int64_t* r, int64_t n, const float* gout, cudaStream_t st) {
+  if (n <= 0) return cudaSuccess;
+  transd_score_bwd_kernel<<<blocks_for_warps(n), WARPS_PER_BLOCK * 32, 0, st>>>(
+      ent, rel, ent_proj, rel_proj, g_ent, g_rel, g_ent_proj, g_rel_proj, ent_dim, rel_dim, h, t, r, n, gout);
   return cudaGetLastError();
 }
 

@@ -84,6 +84,14 @@ cudaError_t launch_transh_score_fwd(const float* ent, const float* rel, const fl
 cudaError_t launch_transh_score_bwd(const float* ent, const float* rel, const float* norm_vect, float* g_ent,
                                     float* g_rel, float* g_norm_vect, int dim, const int64_t* h, const int64_t* t,
                                     const int64_t* r, int64_t n, const float* gout, cudaStream_t st);
+// TransD scoring_function (translation.py:538-568) on its own tables, forward and backward
+cudaError_t launch_transd_score_fwd(const float* ent, const float* rel, const float* ent_proj,
+                                    const float* rel_proj, int ent_dim, int rel_dim, const int64_t* h,
+                                    const int64_t* t, const int64_t* r, int64_t n, float* out, cudaStream_t st);
+cudaError_t launch_transd_score_bwd(const float* ent, const float* rel, const float* ent_proj,
+                                    const float* rel_proj, float* g_ent, float* g_rel, float* g_ent_proj,
+                                    float* g_rel_proj, int ent_dim, int rel_dim, const int64_t* h, const int64_t* t,
+                                    const int64_t* r, int64_t n, const float* gout, cudaStream_t st);
 cudaError_t launch_corrupt_batch(const int64_t* h, const int64_t* t, const int64_t* r, int64_t b,
                                  int n_neg, const float* probs, int64_t n_ent, uint64_t seed,
                                  uint64_t offset, int64_t* nh, int64_t* nt, cudaStream_t st);

@@ -42,7 +42,10 @@ class ModelSpec:
         self.ent2, self.rel2 = ent2, rel2
         self.ent_lo = int(ent_lo)    # global id of row 0 of ent0/ent1
         self.n_rows = int(ent0.shape[0])
-        #: TransH only (transh_spec): the raw norm_vect table; ent0 / rel0 are then ent_emb / rel_emb
+        #: TransH / TransD only (transh_spec, transd_spec): the model's class name.  ent0 is then ranked only
+        #: after a per-relation projection (project_relation) and relation prediction is dense (_dense_rel_scores)
+        self.projection = None
+        #: TransH only: the raw norm_vect table; ent0 / rel0 are then ent_emb / rel_emb
         self.norm_vect = None
         if code == _lib.ANALOGY:
             for name, planes in (("entity", (ent0, ent1, ent2)), ("relation", (rel0, rel1, rel2))):
@@ -135,14 +138,29 @@ class ModelSpec:
                 "TransHModel is supported by the unsharded LinkPredictionEvaluator, RelationPredictionEvaluator, "
                 "TripletClassificationEvaluator, EntityInference, RelationInference and scoring_function only "
                 "(not by the fused training step or shard=)")
+        if name == "TransDModel":
+            # as TransH: the entry points that support TransD build its spec with transd_spec
+            raise NotImplementedError(
+                "TransDModel is supported by the unsharded LinkPredictionEvaluator, RelationPredictionEvaluator, "
+                "TripletClassificationEvaluator, EntityInference, RelationInference and scoring_function only "
+                "(not by the fused training step or shard=)")
         raise NotImplementedError(
-            "%s has no CUDA link-prediction path (supported: TransE L1/L2, TransH, TorusE torus_L1/torus_L2, "
-            "DistMult, RESCAL, ComplEx, Analogy, RotatE)" % name)
+            "%s has no CUDA link-prediction path (supported: TransE L1/L2, TransH, TransD, TorusE "
+            "torus_L1/torus_L2, DistMult, RESCAL, ComplEx, Analogy, RotatE)" % name)
 
 
-def is_transh(model):
-    """TransHModel of this package or (duck-typed, by class name) of the reference."""
-    return type(model).__name__ == "TransHModel"
+#: the models ranked on per-relation projected entity tables, by class name
+PROJECTED_MODELS = ("TransHModel", "TransDModel")
+
+#: widest embedding the kernels take (csrc/kernels.h: SCAN_MAX_DIM)
+MAX_DIM = 8192
+
+
+def projected_model(model):
+    """The class name of a TransH or TransD model of this package or (duck-typed, by class name) of the
+    reference, else None."""
+    name = type(model).__name__
+    return name if name in PROJECTED_MODELS else None
 
 
 def transh_spec(model):
@@ -152,18 +170,57 @@ def transh_spec(model):
     f = ModelSpec._f32
     spec = ModelSpec(_lib.TRANSE_L2, model.emb_dim, model.n_ent, model.n_rel, f(model.ent_emb.weight), None,
                      f(model.rel_emb.weight), None)
+    spec.projection = "TransHModel"
     spec.norm_vect = f(model.norm_vect.weight)
     return spec
 
 
-def _is_transh_spec(spec):
-    return getattr(spec, "norm_vect", None) is not None
+def check_transd_widths(ent_dim, rel_dim):
+    """TransD's widths, checked before any device work: the reference's projection adds a rel_emb_dim vector to
+    ent[:rel_emb_dim] (translation.py:568, 646) and fails on a broadcast when rel_emb_dim > ent_emb_dim."""
+    if not 1 <= rel_dim <= ent_dim:
+        raise ValueError("TransDModel needs 1 <= rel_emb_dim <= ent_emb_dim (got rel_emb_dim = %d, ent_emb_dim = %d)"
+                         % (rel_dim, ent_dim))
+    if ent_dim > MAX_DIM:
+        raise ValueError("TransDModel: ent_emb_dim = %d exceeds %d" % (ent_dim, MAX_DIM))
 
 
-def _refuse_transh_shard(spec, shard):
-    """Sharded TransH calls are not supported: raised on every rank, before any collective."""
-    if _is_transh_spec(spec) and shard is not None:
-        raise NotImplementedError("TransHModel does not support shard= (EntityShard / QueryShard)")
+def transd_spec(model, engine=None):
+    """The spec of a TransD model (translation.py:518-536), read at width rel_emb_dim: ent0 holds the first
+    rel_emb_dim coordinates of the raw ent_emb rows (the rows relation prediction projects on the fly), rel0
+    the raw rel_emb table.  It also carries the raw ent_emb table (``ent_full``, its width ``ent_dim``), the
+    raw rel_proj_vect table (``rel_proj``) and every entity's scalar s_e = (ent_proj_vect[e] * ent_emb[e]).sum()
+    (``scalars``), computed once here: it does not depend on the relation.  Every TransD path projects the
+    entity rows per relation first (rank_link_prediction_transh, topk_entity_inference, transd_rel_scores)."""
+    check_transd_widths(model.ent_emb_dim, model.rel_emb_dim)
+    f = ModelSpec._f32
+    ent, rel_dim = f(model.ent_emb.weight), model.rel_emb_dim
+    spec = ModelSpec(_lib.TRANSE_L2, rel_dim, model.n_ent, model.n_rel, ent[:, :rel_dim].contiguous(), None,
+                     f(model.rel_emb.weight), None)
+    spec.projection = "TransDModel"
+    spec.ent_full, spec.ent_dim = ent, model.ent_emb_dim
+    spec.rel_proj = f(model.rel_proj_vect.weight)
+    spec.scalars = None
+    if ent.is_cuda:      # a model on the host is refused by shard_spec, next
+        spec.scalars = (engine or default_engine()).transd_entity_scalars(ent, f(model.ent_proj_vect.weight))
+    return spec
+
+
+def _is_projected_spec(spec):
+    return getattr(spec, "projection", None) is not None
+
+
+def _refuse_projected_shard(spec, shard):
+    """Sharded TransH / TransD calls are not supported: raised on every rank, before any collective."""
+    if _is_projected_spec(spec) and shard is not None:
+        raise NotImplementedError("%s does not support shard= (EntityShard / QueryShard)" % spec.projection)
+
+
+def project_relation(engine, spec, rel, out):
+    """out (n_rows, spec.dim) <- the entity rows of a TransH / TransD spec projected for relation ``rel``."""
+    if spec.projection == "TransDModel":
+        return engine.transd_project(spec, rel, out)
+    return engine.transh_project(spec, rel, out)
 
 
 def _ptr(t):
@@ -450,6 +507,38 @@ class CudaEngine:
         self.launches += 1
         return scores
 
+    def transd_entity_scalars(self, ent, ent_proj):
+        """(n_rows,) s_e = (ent_proj[e] * ent[e]).sum() of TransD's raw ent_emb / ent_proj_vect tables, in ATen's
+        order (kge_transd_entity_scalars, translation.py:645)."""
+        _need_cuda(ent, ent_proj)
+        n, dim = ent.shape
+        s = torch.empty(n, dtype=torch.float32, device=ent.device)
+        _lib.check(self.lib.kge_transd_entity_scalars(_ptr(ent), _ptr(ent_proj), n, dim, _ptr(s),
+                                                      _stream(ent.device)), "kge_transd_entity_scalars")
+        self.launches += 1
+        return s
+
+    def transd_project(self, spec, rel, out):
+        """out (n_rows, rel_dim) <- the entity rows of ``spec`` (transd_spec) projected for relation ``rel``
+        (kge_transd_project, translation.py:646)."""
+        _need_cuda(spec.ent_full, out)
+        _lib.check(self.lib.kge_transd_project(_ptr(spec.ent_full), spec.ent_dim, _ptr(spec.scalars),
+                                               _ptr(spec.rel_proj[rel]), spec.n_rows, spec.dim, _ptr(out),
+                                               _stream(out.device)), "kge_transd_project")
+        self.launches += 1
+        return out
+
+    def transd_rel_scores(self, spec, hrows, trows, hs, ts):
+        """(n, n_rel) scores -||(P_c(h) + r_c) - P_c(t)||^2 of every relation c: TransD's relation case
+        (interfaces.py:261-272), dense like TransH's; hrows / trows (n, rel_dim), hs / ts (n,) their scalars."""
+        n, dev = hrows.shape[0], hrows.device
+        scores = torch.empty((n, spec.n_rel), dtype=torch.float32, device=dev)
+        _lib.check(self.lib.kge_transd_rel_scores(_ptr(hrows), _ptr(hs), _ptr(trows), _ptr(ts), _ptr(spec.rel0),
+                                                  _ptr(spec.rel_proj), spec.dim, n, spec.n_rel, _ptr(scores),
+                                                  _stream(dev)), "kge_transd_rel_scores")
+        self.launches += 1
+        return scores
+
     def rank_dense(self, scores, true_idx, filt, raw_count, filt_sub, true_score=None, true_score_in=None):
         """get_rank + filter_scores on a dense (n, n_cand) matrix, counters added into."""
         n, n_c = scores.shape
@@ -723,11 +812,13 @@ def shard_spec(model, shard=None, who="evaluate", n=None, build=ModelSpec.from_m
     """The ModelSpec the engine reads for ``model`` (``build(model)``) under ``shard``, after the shard's
     argument checks: under an EntityShard with local storage the model holds entity rows [lo, hi) and its
     row 0 is entity lo (_check_table); a QueryShard must cover ``n`` facts, when ``n`` is given.  The
-    checks come first, then the model must be on a CUDA device.  TransH: no shard, and transh_spec."""
-    if is_transh(model):
+    checks come first, then the model must be on a CUDA device.  TransH / TransD: no shard, and transh_spec /
+    transd_spec."""
+    name = projected_model(model)
+    if name is not None:
         if shard is not None:
-            raise NotImplementedError("TransHModel does not support shard= (EntityShard / QueryShard)")
-        build = transh_spec
+            raise NotImplementedError("%s does not support shard= (EntityShard / QueryShard)" % name)
+        build = transh_spec if name == "TransHModel" else transd_spec
     spec = build(model)
     if isinstance(shard, EntityShard):
         if shard.local_storage:
@@ -789,8 +880,8 @@ def rank_link_prediction(spec, h_idx, t_idx, r_idx, filt_tail, filt_head, shard=
     """
     engine = engine or default_engine()
     n = h_idx.shape[0]
-    if _is_transh_spec(spec):
-        raise ValueError("a TransH spec is ranked by rank_link_prediction_transh")
+    if _is_projected_spec(spec):
+        raise ValueError("a %s spec is ranked by rank_link_prediction_transh" % spec.projection[:-len("Model")])
     table = spec
     if shard is not None:
         _check_table(spec, shard)
@@ -896,25 +987,25 @@ def relation_groups(r_idx, n_rel):
 
 def rank_link_prediction_transh(spec, h_idx, t_idx, r_idx, groups, filt_tail, filt_head, engine=None,
                                 chunk=DEFAULT_CHUNK, exact=False, sync=True):
-    """rank_link_prediction for TransH (transh_spec): the facts come sorted by relation, ``groups`` the
-    (relation, lo, hi) of relation_groups.  Per relation, the entity table is projected on its hyperplane into
-    one reused buffer (kge_transh_project) and the group is ranked on it as TransE-L2 -- tail queries
-    fl(P_r(h) + r) against the projected candidates, head candidates (P_r(c) + r) - P_r(t), exactly the
-    reference's arithmetic on its projected_entities (interfaces.py:249-260) -- with the filter CSR rows of
-    the group.  The tensor-core image of the buffer is rebuilt per relation, without the cache.
-    Arguments and result as rank_link_prediction's (no shard)."""
+    """rank_link_prediction for TransH and TransD (transh_spec, transd_spec): the facts come sorted by relation,
+    ``groups`` the (relation, lo, hi) of relation_groups.  Per relation, the entity table is projected into one
+    reused (n_rows, spec.dim) buffer (project_relation: kge_transh_project or kge_transd_project) and the group
+    is ranked on it as TransE-L2 -- tail queries fl(P_r(h) + r) against the projected candidates, head
+    candidates (P_r(c) + r) - P_r(t), exactly the reference's arithmetic on its projected_entities
+    (interfaces.py:249-260) -- with the filter CSR rows of the group.  The tensor-core image of the buffer is
+    rebuilt per relation, without the cache.  Arguments and result as rank_link_prediction's (no shard)."""
     engine = engine or default_engine()
     n = h_idx.shape[0]
     dev = spec.ent0.device
     with _device_guard(dev):
-        proj = torch.empty_like(spec.ent0)
+        proj = torch.empty((spec.n_rows, spec.dim), dtype=torch.float32, device=dev)
         ranks = [torch.empty(n, dtype=torch.int64, device=dev) for _ in range(4)]
         filts = [f() if callable(f) else f for f in (filt_tail, filt_head)]
         ranges = [(lo, hi) for _, lo, hi in groups]
         parts = [_csr_cut(f, ranges) for f in filts]    # one device -> host read per CSR
         flags = []
         for (rel, lo, hi), ft, fh in zip(groups, parts[0], parts[1]):
-            engine.transh_project(spec, rel, proj)
+            project_relation(engine, spec, rel, proj)
             pspec = ModelSpec(spec.code, spec.dim, spec.n_ent, spec.n_rel, proj, None, spec.rel0, None)
             lazy = rank_link_prediction(pspec, h_idx[lo:hi], t_idx[lo:hi], r_idx[lo:hi], ft, fh, engine=engine,
                                         chunk=chunk, exact=exact, sync=False, tc_cache=False)
@@ -952,14 +1043,18 @@ def relation_spec(spec):
 
 def _dense_relations(spec):
     """Models whose relation case is a dense (n, n_rel) score matrix rather than a scan over a candidate table:
-    RESCAL (per-fact vectors h^T M_c, bilinear.py:115-121) and TransH (rows projected per relation,
+    RESCAL (per-fact vectors h^T M_c, bilinear.py:115-121), TransH and TransD (rows projected per relation,
     interfaces.py:261-272)."""
-    return spec.code == _lib.RESCAL or _is_transh_spec(spec)
+    return spec.code == _lib.RESCAL or _is_projected_spec(spec)
 
 
-def _dense_rel_scores(engine, spec, hrows, trows):
-    """(n, n_rel) relation scores of the facts (hrows, ?, trows), hrows / trows (n, dim), for _dense_relations."""
-    if _is_transh_spec(spec):
+def _dense_rel_scores(engine, spec, hrows, trows, h_idx=None, t_idx=None):
+    """(n, n_rel) relation scores of the facts (hrows, ?, trows), hrows / trows (n, dim), for _dense_relations.
+    TransD also reads the scalars of the facts' entities h_idx / t_idx (unsharded calls only)."""
+    projection = getattr(spec, "projection", None)
+    if projection == "TransDModel":
+        return engine.transd_rel_scores(spec, hrows, trows, spec.scalars[h_idx], spec.scalars[t_idx])
+    if projection == "TransHModel":
         return engine.transh_rel_scores(spec, hrows, trows)
     return engine.rescal_rel_scores(spec, hrows, trows)
 
@@ -985,7 +1080,7 @@ def rank_relation_prediction(spec, h_idx, t_idx, r_idx, filt, directed=True, eng
     engine = engine or default_engine()
     n = h_idx.shape[0]
     dev = spec.ent0.device
-    _refuse_transh_shard(spec, shard)
+    _refuse_projected_shard(spec, shard)
     rspec = None if _dense_relations(spec) else relation_spec(spec)   # unsupported models raise here
     if isinstance(shard, EntityShard):
         _check_table(spec, shard)
@@ -999,16 +1094,19 @@ def rank_relation_prediction(spec, h_idx, t_idx, r_idx, filt, directed=True, eng
         packed = None if rspec is None else engine.pack(rspec)
         keep = []
 
-        def rank_rows(hrows, trows, r, f, raw, sub):
-            """Adds the counts of facts (hrows, ?, trows) with true relations r into raw / sub."""
+        def rank_rows(hrows, trows, r, f, raw, sub, h=None, t=None):
+            """Adds the counts of facts (hrows, ?, trows) with true relations r into raw / sub; h / t: the
+            facts' entities (unsharded calls)."""
             m = r.shape[0]
             s_true = torch.empty(m, dtype=torch.float32, device=dev)
             if rspec is None:
-                # RESCAL, TransH: a dense (m, n_rel) score matrix (_dense_rel_scores) ranked by kge_rank_dense
+                # RESCAL, TransH, TransD: a dense (m, n_rel) score matrix (_dense_rel_scores) ranked by
+                # kge_rank_dense
                 hrows, trows = hrows.reshape(m, spec.dim), trows.reshape(m, spec.dim)
-                engine.rank_dense(_dense_rel_scores(engine, spec, hrows, trows), r, f, raw, sub, true_score=s_true)
+                engine.rank_dense(_dense_rel_scores(engine, spec, hrows, trows, h, t), r, f, raw, sub,
+                                  true_score=s_true)
                 if not directed:
-                    engine.rank_dense(_dense_rel_scores(engine, spec, trows, hrows), r, f, raw, sub,
+                    engine.rank_dense(_dense_rel_scores(engine, spec, trows, hrows, t, h), r, f, raw, sub,
                                       true_score_in=s_true)
                 return
             rrows = engine.gather_rows(rspec, r)
@@ -1027,7 +1125,7 @@ def rank_relation_prediction(spec, h_idx, t_idx, r_idx, filt, directed=True, eng
             for (lo, hi), f in zip(chunks, _csr_cut(filt, chunks)):
                 h, t, r = h_idx[lo:hi], t_idx[lo:hi], r_idx[lo:hi].contiguous()
                 rank_rows(engine.gather_rows(spec, h), engine.gather_rows(spec, t), r, f,
-                          counters[0][lo:hi], counters[1][lo:hi])
+                          counters[0][lo:hi], counters[1][lo:hi], h, t)
             ranks, filt_ranks = engine.finalize(counters[0], counters[1])
             del keep
             return ranks, filt_ranks
@@ -1161,8 +1259,8 @@ def topk_entity_inference(spec, ents, rels, side, k, mask=None, shard=None, engi
     engine = engine or default_engine()
     n = ents.shape[0]
     dev = spec.ent0.device
-    _refuse_transh_shard(spec, shard)
-    if _is_transh_spec(spec):
+    _refuse_projected_shard(spec, shard)
+    if _is_projected_spec(spec):
         return _topk_entity_transh(spec, ents, rels, side, k, mask, engine, chunk)
     if shard is not None and shard.world > 1:
         _check_sharded_k(k, spec.n_ent)
@@ -1200,8 +1298,9 @@ def topk_entity_inference(spec, ents, rels, side, k, mask=None, shard=None, engi
 
 
 def _topk_entity_transh(spec, ents, rels, side, k, mask, engine, chunk):
-    """topk_entity_inference for TransH: the queries grouped by relation (relation_groups), the entity table
-    projected per relation into one reused buffer and scanned as TransE-L2, as in rank_link_prediction_transh."""
+    """topk_entity_inference for TransH and TransD: the queries grouped by relation (relation_groups), the entity
+    table projected per relation into one reused buffer and scanned as TransE-L2, as in
+    rank_link_prediction_transh."""
     n = ents.shape[0]
     dev = spec.ent0.device
     _check_k(k, spec.n_rows)
@@ -1216,11 +1315,11 @@ def _topk_entity_transh(spec, ents, rels, side, k, mask, engine, chunk):
             sel = torch.repeat_interleave(offs[:-1][perm], lens[perm]) + (
                 torch.arange(int(new_offs[-1])) - torch.repeat_interleave(new_offs[:-1], lens[perm]))
             mask = (new_offs, ids[sel])
-        proj = torch.empty_like(spec.ent0)
+        proj = torch.empty((spec.n_rows, spec.dim), dtype=torch.float32, device=dev)
         pred = torch.empty((n, k), dtype=torch.int64, device=dev)
         vals = torch.empty((n, k), dtype=torch.float32, device=dev)
         for (rel, lo, hi), m in zip(groups, _csr_cut(mask, [(lo, hi) for _, lo, hi in groups])):
-            engine.transh_project(spec, rel, proj)
+            project_relation(engine, spec, rel, proj)
             pspec = ModelSpec(spec.code, spec.dim, spec.n_ent, spec.n_rel, proj, None, spec.rel0, None)
             packed = engine.pack(pspec)
 
@@ -1245,7 +1344,7 @@ def topk_relation_inference(spec, e1, e2, k, mask=None, shard=None, engine=None,
     engine = engine or default_engine()
     n = e1.shape[0]
     dev = spec.ent0.device
-    _refuse_transh_shard(spec, shard)
+    _refuse_projected_shard(spec, shard)
     if isinstance(shard, QueryShard) and shard.world > 1:
         _check_sharded_k(k, spec.n_rel)
         _check_queries(shard, n)
@@ -1253,16 +1352,16 @@ def topk_relation_inference(spec, e1, e2, k, mask=None, shard=None, engine=None,
             spec, a, b, k, m, engine=engine, chunk=chunk))], (e1, e2), mask)
         return _pair_unpack(full)
     if _dense_relations(spec):
-        # RESCAL, TransH: dense (n, n_rel) scores, then the same selection kernels
+        # RESCAL, TransH, TransD: dense (n, n_rel) scores, then the same selection kernels
         rspec, packed, n_cand = None, None, spec.n_rel
     else:
         rspec = relation_spec(spec)
         packed, n_cand = engine.pack(rspec), rspec.n_rows
 
-    def local_topk(hrows, trows, m):
+    def local_topk(hrows, trows, m, a=None, b=None):
         if rspec is None:
             m_rows = hrows.shape[0]
-            scores = _dense_rel_scores(engine, spec, hrows.view(m_rows, spec.dim), trows.view(m_rows, spec.dim))
+            scores = _dense_rel_scores(engine, spec, hrows.view(m_rows, spec.dim), trows.view(m_rows, spec.dim), a, b)
             return engine.topk_dense(scores, k, m)
         return engine.topk_side(rspec, packed, _lib.SIDE_REL, hrows, trows, None, k, m)
 
@@ -1273,7 +1372,8 @@ def topk_relation_inference(spec, e1, e2, k, mask=None, shard=None, engine=None,
     with _device_guard(dev):
         if shard is None or shard.world == 1:
             def topk_chunk(lo, hi, m):
-                return local_topk(engine.gather_rows(spec, e1[lo:hi]), engine.gather_rows(spec, e2[lo:hi]), m)
+                a, b = e1[lo:hi], e2[lo:hi]
+                return local_topk(engine.gather_rows(spec, a), engine.gather_rows(spec, b), m, a, b)
 
             return _topk_chunks(n, n_cand, k, topk_chunk, mask, dev, chunk)
 

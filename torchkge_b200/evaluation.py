@@ -10,7 +10,7 @@ import torch
 from . import _lib
 from .data import dict_filter_csr, filter_csr
 from .engine import (DEFAULT_CHUNK, EntityShard, ModelSpec, QueryShard, _by_query_slices, _check_table,
-                     default_engine, is_transh, rank_link_prediction, rank_link_prediction_transh,
+                     default_engine, projected_model, rank_link_prediction, rank_link_prediction_transh,
                      rank_relation_prediction, relation_groups, score_triples_entity_sharded, shard_spec)
 from .exceptions import NotYetEvaluatedError
 
@@ -83,9 +83,9 @@ class LinkPredictionEvaluator(object):
         t_d = tails.to(dev, non_blocking=True)
         r_d = rels.to(dev, non_blocking=True)
         stats = {"h2d_bytes": 8 * 3 * n_here, "d2h_bytes": 8 * (4 * kg.n_facts + 1)}
-        transh = is_transh(self.model)
+        transh = projected_model(self.model) is not None
         if transh:
-            # TransH ranks the facts relation by relation: everything below, filter sets included, runs on
+            # TransH and TransD rank the facts relation by relation: everything below, filter sets included, runs on
             # the facts sorted by relation; the ranks go back to fact order at the end
             order, order_host, groups = relation_groups(r_d, spec.n_rel)
             heads, tails, rels = heads[order_host], tails[order_host], rels[order_host]
@@ -218,7 +218,7 @@ class RelationPredictionEvaluator(object):
 
     Parameters
     ----------
-    model: TransE (L1/L2), TransH, DistMult, RESCAL, ComplEx or Analogy model on a CUDA device.
+    model: TransE (L1/L2), TransH, TransD, DistMult, RESCAL, ComplEx or Analogy model on a CUDA device.
     knowledge_graph: object exposing ``n_facts, head_idx, tail_idx, relations, dict_of_rels``.
     directed: bool (default True).  False: both (h, ?, t) and (t, ?, h) are scored and ranked
         together against the directed true score (evaluation.py:99-107).
@@ -326,8 +326,8 @@ class TripletClassificationEvaluator(object):
 
     def __init__(self, model, kg_val, kg_test, *, shard=None):
         from .sampling import PositionalNegativeSampler
-        if shard is not None and is_transh(model):
-            raise NotImplementedError("TransHModel does not support shard= (EntityShard / QueryShard)")
+        if shard is not None and projected_model(model) is not None:
+            raise NotImplementedError("%s does not support shard= (EntityShard / QueryShard)" % projected_model(model))
         self.model = model
         self.kg_val = kg_val
         self.kg_test = kg_test

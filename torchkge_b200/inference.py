@@ -47,7 +47,7 @@ class EntityInference(object):
 
     Parameters (torchkge/inference.py:183-201)
     ----------
-    model: TransE / TransH / DistMult / RESCAL / ComplEx / RotatE model on a CUDA device.
+    model: TransE / TransH / TransD / DistMult / RESCAL / ComplEx / RotatE model on a CUDA device.
     known_entities, known_relations: torch.LongTensor (n_facts,)
     top_k: int
     missing: 'tails' (complete (h, r, ?)) or 'heads' (complete (?, r, t))
@@ -97,7 +97,7 @@ class EntityInference(object):
 class RelationInference(object):
     """Infer the missing relation of (entity 1, entity 2) pairs (torchkge/inference.py:78-155).
 
-    model: TransE (L1/L2), TransH, DistMult or ComplEx model on a CUDA device.  dictionary: optional
+    model: TransE (L1/L2), TransH, TransD, DistMult or ComplEx model on a CUDA device.  dictionary: optional
     mapping (entity 1, entity 2) -> set of known relations (``kg.dict_of_rels``), excluded from
     the predictions.  Attributes: ``predictions`` (n_facts, top_k) long, ``scores`` float.
     shard: ``EntityShard`` or ``QueryShard``, optional, keyword only (extension).  The candidates

@@ -2,8 +2,8 @@
 and method signatures (torchkge/models/interfaces.py, translation.py:18-125,
 bilinear.py:14-267, 414-556), whose scoring bodies are calls into the CUDA engine.
 
-Only what lies on the hot path is here: TransE (L1 / L2), TransH, TorusE, DistMult, RESCAL, ComplEx,
-Analogy and the RotatE addition.  ``state_dict`` keys equal the reference's, so weights move freely between
+Only what lies on the hot path is here: TransE (L1 / L2), TransH, TransD, TorusE, DistMult, RESCAL,
+ComplEx, Analogy and the RotatE addition.  ``state_dict`` keys equal the reference's, so weights move freely between
 the two packages.  The pre-0.17 method names ``lp_prep_cands`` / ``lp_scoring_function``
 (docs/history.rst:37-42) are kept as aliases.
 """
@@ -325,6 +325,80 @@ class TransHModel(TranslationModel):
     def _load_from_state_dict(self, state_dict, prefix, local_metadata, strict, missing_keys, unexpected_keys,
                               error_msgs):
         # a reference checkpoint carries its (n_rel, n_ent, emb_dim) projection cache: not a parameter here
+        state_dict.pop(prefix + "projected_entities", None)
+        super()._load_from_state_dict(state_dict, prefix, local_metadata, strict, missing_keys, unexpected_keys,
+                                      error_msgs)
+
+
+class TransDModel(TranslationModel):
+    """TransD (Ji et al. 2015) -- torchkge/models/translation.py:461-652: TransE-L2 between the projections
+    P_r(e) = (e . e_p) r_p + e[:rel_emb_dim] of h and t, with an entity projection vector e_p
+    (``ent_proj_vect``, ent_emb_dim) and a relation projection vector r_p (``rel_proj_vect``, rel_emb_dim).
+
+    There is no ``projected_entities`` cache: the reference fills an (n_rel, n_ent, rel_emb_dim) tensor
+    (translation.py:533-536, 629-652), 8 GB at FB15k's size.  Link prediction and ``EntityInference``
+    compute every entity's scalar e . e_p once per call and project the entity table on the GPU for one
+    relation at a time; relation prediction and ``RelationInference`` project the two rows of each fact on
+    the fly.  Unlike the reference, which ranks on projections cached until the next ``scoring_function``
+    call, every call projects the current weights.  A reference checkpoint loads here with the default
+    ``strict=True`` (its ``projected_entities`` entry is discarded); this model's ``state_dict`` loads into
+    the reference with ``strict=False``.  ``rel_emb_dim`` may not exceed ``ent_emb_dim``.
+
+    ``inference_prepare_candidates`` / ``inference_scoring_function`` are not available: the
+    reference's entity candidates are a per-row (b, n_ent, rel_emb_dim) tensor.  Use
+    ``LinkPredictionEvaluator``, ``RelationPredictionEvaluator``, ``EntityInference`` or
+    ``RelationInference``.  Out of scope: the fused training step and ``shard=``.
+    """
+
+    def __init__(self, ent_emb_dim, rel_emb_dim, n_entities, n_relations):
+        super().__init__(n_entities, n_relations, dissimilarity_type='L2')
+        self.ent_emb_dim = ent_emb_dim
+        self.rel_emb_dim = rel_emb_dim
+        self.ent_emb = init_embedding(self.n_ent, self.ent_emb_dim)
+        self.rel_emb = init_embedding(self.n_rel, self.rel_emb_dim)
+        self.ent_proj_vect = init_embedding(self.n_ent, self.ent_emb_dim)
+        self.rel_proj_vect = init_embedding(self.n_rel, self.rel_emb_dim)
+        self.normalize_parameters()
+        self.evaluated_projections = False
+
+    def scoring_function(self, h_idx, t_idx, r_idx):
+        """-||P(h~) + r~ - P(t~)||^2 with h, t, r and the three projection vectors L2-normalised
+        (translation.py:538-556), on the per-triple kernels kge_transd_score_triples_fwd / _bwd."""
+        self.evaluated_projections = False
+        from .training import score_triples_transd
+        return score_triples_transd(self, h_idx, t_idx, r_idx)
+
+    def project(self, ent, e_proj_vect, r_proj_vect):
+        b_size = ent.shape[0]
+        scalar_product = (ent * e_proj_vect).sum(dim=1)
+        proj_e = (r_proj_vect * scalar_product.view(b_size, 1))
+        return proj_e + ent[:, :self.rel_emb_dim]
+
+    def normalize_parameters(self):
+        self.ent_emb.weight.data = normalize(self.ent_emb.weight.data, p=2, dim=1)
+        self.rel_emb.weight.data = normalize(self.rel_emb.weight.data, p=2, dim=1)
+        self.ent_proj_vect.weight.data = normalize(self.ent_proj_vect.weight.data, p=2, dim=1)
+        self.rel_proj_vect.weight.data = normalize(self.rel_proj_vect.weight.data, p=2, dim=1)
+
+    def get_embeddings(self):
+        self.normalize_parameters()
+        return self.ent_emb.weight.data, self.rel_emb.weight.data, \
+            self.ent_proj_vect.weight.data, self.rel_proj_vect.weight.data
+
+    def inference_prepare_candidates(self, h_idx, t_idx, r_idx, entities=True):
+        raise NotImplementedError(
+            "TransDModel has no inference_prepare_candidates: the reference's candidates are a per-row "
+            "(b, n_ent, rel_emb_dim) tensor of projected entities.  Use LinkPredictionEvaluator, "
+            "RelationPredictionEvaluator, EntityInference or RelationInference, which project on the GPU.")
+
+    def inference_scoring_function(self, h, t, r):
+        raise NotImplementedError(
+            "TransDModel has no inference_scoring_function: use LinkPredictionEvaluator, "
+            "RelationPredictionEvaluator, EntityInference or RelationInference.")
+
+    def _load_from_state_dict(self, state_dict, prefix, local_metadata, strict, missing_keys, unexpected_keys,
+                              error_msgs):
+        # a reference checkpoint carries its (n_rel, n_ent, rel_emb_dim) projection cache: not a parameter here
         state_dict.pop(prefix + "projected_entities", None)
         super()._load_from_state_dict(state_dict, prefix, local_metadata, strict, missing_keys, unexpected_keys,
                                       error_msgs)

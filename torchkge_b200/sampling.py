@@ -10,7 +10,7 @@ import torch
 
 from . import _lib
 from .engine import _ptr, _stream
-from .training import fused_loss_step, fused_margin_step, loss_kind_of, refuse_transh_fused_step
+from .training import fused_loss_step, fused_margin_step, loss_kind_of, refuse_projected_fused_step
 
 
 def get_bernoulli_probs(kg):
@@ -175,7 +175,7 @@ def _sampler_fused_step(sampler, model, heads, tails, relations, margin, n_neg, 
     """fused_step of the samplers: their argument checks, then the fused step at the sampler's next call count
     with head probabilities ``probs`` (rel_share: the relation-corrupting step; positional: the positional
     step's CSR)."""
-    refuse_transh_fused_step(model)
+    refuse_projected_fused_step(model)
     if (margin is None) == (criterion is None):
         raise ValueError("fused_step takes exactly one of margin and criterion")
     if criterion is not None:

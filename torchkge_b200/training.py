@@ -11,7 +11,7 @@ import torch
 
 from . import _lib
 from .engine import (EntityShard, ModelSpec, QueryShard, _check_table, _device_guard, _exchanged_rows, _plane_ptrs,
-                     _ptr, _stream, default_engine)
+                     _ptr, _stream, check_transd_widths, default_engine, projected_model)
 
 
 def _param_tensors(model, code):
@@ -162,6 +162,46 @@ def score_triples_transh(model, h_idx, t_idx, r_idx):
     to ent_emb, rel_emb and norm_vect."""
     return _TransHScoreTriples.apply(model.emb_dim, h_idx, t_idx, r_idx, model.ent_emb.weight,
                                      model.rel_emb.weight, model.norm_vect.weight)
+
+
+class _TransDScoreTriples(torch.autograd.Function):
+    """TransD's scoring_function on kge_transd_score_triples_fwd / _bwd (translation.py:538-568)."""
+
+    @staticmethod
+    def forward(ctx, ent_dim, rel_dim, h, t, r, ent, rel, ent_proj, rel_proj):
+        tables = [x.detach().contiguous() for x in (ent, rel, ent_proj, rel_proj)]
+        for x in tables:
+            if x.dtype != torch.float32:
+                raise TypeError("embedding tables must be float32, got %s" % x.dtype)
+        _check_cuda(tables[0], h, t, r)
+        dev = tables[0].device
+        h, t, r = _idx(h, dev), _idx(t, dev), _idx(r, dev)
+        out = torch.empty(h.shape[0], dtype=torch.float32, device=dev)
+        _lib.check(_lib.load().kge_transd_score_triples_fwd(*(_ptr(x) for x in tables), ent_dim, rel_dim, _ptr(h),
+                                                            _ptr(t), _ptr(r), h.shape[0], _ptr(out), _stream(dev)),
+                   "kge_transd_score_triples_fwd")
+        ctx.dims = (ent_dim, rel_dim)
+        ctx.save_for_backward(h, t, r, *tables)
+        return out
+
+    @staticmethod
+    def backward(ctx, gout):
+        h, t, r, *tables = ctx.saved_tensors
+        grads = [torch.zeros_like(x) for x in tables]
+        gout = gout.contiguous().float()
+        _lib.check(_lib.load().kge_transd_score_triples_bwd(*(_ptr(x) for x in tables), *(_ptr(g) for g in grads),
+                                                            *ctx.dims, _ptr(h), _ptr(t), _ptr(r), h.shape[0],
+                                                            _ptr(gout), _stream(h.device)),
+                   "kge_transd_score_triples_bwd")
+        return (None, None, None, None, None, *grads)
+
+
+def score_triples_transd(model, h_idx, t_idx, r_idx):
+    """TransD's ``scoring_function(h_idx, t_idx, r_idx)`` -> (n,) float scores, differentiable with respect
+    to ent_emb, rel_emb, ent_proj_vect and rel_proj_vect."""
+    check_transd_widths(model.ent_emb_dim, model.rel_emb_dim)
+    return _TransDScoreTriples.apply(model.ent_emb_dim, model.rel_emb_dim, h_idx, t_idx, r_idx, model.ent_emb.weight,
+                                     model.rel_emb.weight, model.ent_proj_vect.weight, model.rel_proj_vect.weight)
 
 
 class _MarginLoss(torch.autograd.Function):
@@ -517,16 +557,17 @@ def _positional_csr(positional, n_rel, dev):
     return tuple(_idx(x, dev) for x in positional)
 
 
-def refuse_transh_fused_step(model):
-    """TransH has per-triple kernels (score_triples_transh) but no fused training step."""
-    if type(model).__name__ == "TransHModel":
-        raise NotImplementedError("TransHModel has no fused training step: train it with model(h, t, r, nh, nt), "
-                                  "a loss and backward()")
+def refuse_projected_fused_step(model):
+    """TransH and TransD have per-triple kernels (score_triples_transh / _transd) but no fused training step."""
+    name = projected_model(model)
+    if name is not None:
+        raise NotImplementedError("%s has no fused training step: train it with model(h, t, r, nh, nt), "
+                                  "a loss and backward()" % name)
 
 
 def _fused_step(model, heads, tails, relations, loss_kind, margin, n_neg, negatives, bern_probs, seed, offset,
                 shard, rel_share=None, positional=None):
-    refuse_transh_fused_step(model)
+    refuse_projected_fused_step(model)
     if negatives is not None and len(negatives) not in (2, 3):
         raise ValueError("negatives must be (neg_heads, neg_tails) or (neg_heads, neg_tails, neg_rels)")
     if positional is not None and negatives is not None:
