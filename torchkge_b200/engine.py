@@ -6,7 +6,8 @@ may substitute an object with the same methods (``pack``, ``gather_rows``, ``ran
 ``score_all``; ``topk_side`` / ``topk_merge`` for top-k inference; ``margin_step_fwd`` /
 ``margin_step_bwd`` / ``scatter_rows_add`` for the sharded training step; ``finalize`` /
 ``rescal_rel_scores`` / ``rank_dense`` for relation prediction; ``score_triples`` for triplet
-classification) to exercise the sharding logic on CPU.
+classification; ``transh_project`` / ``transd_project`` for the relation-grouped loops of TransH and
+TransD) to exercise the sharding and grouping logic on CPU.
 """
 import ctypes
 import os
@@ -42,11 +43,6 @@ class ModelSpec:
         self.ent2, self.rel2 = ent2, rel2
         self.ent_lo = int(ent_lo)    # global id of row 0 of ent0/ent1
         self.n_rows = int(ent0.shape[0])
-        #: TransH / TransD only (transh_spec, transd_spec): the model's class name.  ent0 is then ranked only
-        #: after a per-relation projection (project_relation) and relation prediction is dense (_dense_rel_scores)
-        self.projection = None
-        #: TransH only: the raw norm_vect table; ent0 / rel0 are then ent_emb / rel_emb
-        self.norm_vect = None
         if code == _lib.ANALOGY:
             for name, planes in (("entity", (ent0, ent1, ent2)), ("relation", (rel0, rel1, rel2))):
                 if planes[0] is None and name == "relation":
@@ -131,48 +127,48 @@ class ModelSpec:
             r = cls.stacked([model.sc_rel_emb.weight, model.re_rel_emb.weight, model.im_rel_emb.weight])
             return cls(_lib.ANALOGY, model.scalar_dim, model.n_ent, model.n_rel, e[0], e[1], r[0], r[1],
                        ent2=e[2], rel2=r[2])
-        if name == "TransHModel":
-            # every entry point that supports TransH builds its spec with transh_spec; the others (the
-            # fused training step, sharded calls, inference_scoring_function) end here
+        if name in PROJECTED_SPECS:
+            # every entry point that supports TransH / TransD builds its spec from PROJECTED_SPECS; the others
+            # (the fused training step, sharded calls) end here
             raise NotImplementedError(
-                "TransHModel is supported by the unsharded LinkPredictionEvaluator, RelationPredictionEvaluator, "
+                "%s is supported by the unsharded LinkPredictionEvaluator, RelationPredictionEvaluator, "
                 "TripletClassificationEvaluator, EntityInference, RelationInference and scoring_function only "
-                "(not by the fused training step or shard=)")
-        if name == "TransDModel":
-            # as TransH: the entry points that support TransD build its spec with transd_spec
-            raise NotImplementedError(
-                "TransDModel is supported by the unsharded LinkPredictionEvaluator, RelationPredictionEvaluator, "
-                "TripletClassificationEvaluator, EntityInference, RelationInference and scoring_function only "
-                "(not by the fused training step or shard=)")
+                "(not by the fused training step or shard=)" % name)
         raise NotImplementedError(
             "%s has no CUDA link-prediction path (supported: TransE L1/L2, TransH, TransD, TorusE "
             "torus_L1/torus_L2, DistMult, RESCAL, ComplEx, Analogy, RotatE)" % name)
 
 
-#: the models ranked on per-relation projected entity tables, by class name
-PROJECTED_MODELS = ("TransHModel", "TransDModel")
-
 #: widest embedding the kernels take (csrc/kernels.h: SCAN_MAX_DIM)
 MAX_DIM = 8192
 
 
-def projected_model(model):
-    """The class name of a TransH or TransD model of this package or (duck-typed, by class name) of the
-    reference, else None."""
-    name = type(model).__name__
-    return name if name in PROJECTED_MODELS else None
+class ProjectedSpec(ModelSpec):
+    """A TransH or TransD model read as TransE-L2, whose entity rows are ranked only after a per-relation
+    projection: ``project(engine, rel, out)`` writes the (n_rows, dim) table of relation ``rel`` into ``out``
+    (the relation-grouped loops of rank_link_prediction_projected and topk_entity_inference), and
+    ``rel_scores(engine, hrows, trows, h_idx, t_idx)`` gives the dense (n, n_rel) relation scores of the facts
+    (_dense_rel_scores).  ``name``: the model's class name, for error messages."""
+
+    def __init__(self, model, dim, ent0, rel0):
+        super().__init__(_lib.TRANSE_L2, dim, model.n_ent, model.n_rel, ent0, None, rel0, None)
+        self.name = type(model).__name__
 
 
-def transh_spec(model):
-    """The spec of a TransH model (translation.py:168-181): the entity and relation tables read as a
-    TransE-L2 model's, plus the raw normal vectors.  The scans never see ent_emb itself: every TransH path
-    projects it per relation first (rank_link_prediction_transh, topk_entity_inference, transh_rel_scores)."""
-    f = ModelSpec._f32
-    spec = ModelSpec(_lib.TRANSE_L2, model.emb_dim, model.n_ent, model.n_rel, f(model.ent_emb.weight), None,
-                     f(model.rel_emb.weight), None)
-    spec.projection = "TransHModel"
-    spec.norm_vect = f(model.norm_vect.weight)
-    return spec
+class TransHSpec(ProjectedSpec):
+    """TransH (translation.py:168-181): ent_emb and rel_emb read as a TransE-L2 model's, plus the raw normal
+    vectors (``norm_vect``)."""
+
+    def __init__(self, model):
+        f = ModelSpec._f32
+        super().__init__(model, model.emb_dim, f(model.ent_emb.weight), f(model.rel_emb.weight))
+        self.norm_vect = f(model.norm_vect.weight)
+
+    def project(self, engine, rel, out):
+        return engine.transh_project(self, rel, out)
+
+    def rel_scores(self, engine, hrows, trows, h_idx, t_idx):
+        return engine.transh_rel_scores(self, hrows, trows)
 
 
 def check_transd_widths(ent_dim, rel_dim):
@@ -185,42 +181,41 @@ def check_transd_widths(ent_dim, rel_dim):
         raise ValueError("TransDModel: ent_emb_dim = %d exceeds %d" % (ent_dim, MAX_DIM))
 
 
-def transd_spec(model, engine=None):
-    """The spec of a TransD model (translation.py:518-536), read at width rel_emb_dim: ent0 holds the first
-    rel_emb_dim coordinates of the raw ent_emb rows (the rows relation prediction projects on the fly), rel0
-    the raw rel_emb table.  It also carries the raw ent_emb table (``ent_full``, its width ``ent_dim``), the
-    raw rel_proj_vect table (``rel_proj``) and every entity's scalar s_e = (ent_proj_vect[e] * ent_emb[e]).sum()
-    (``scalars``), computed once here: it does not depend on the relation.  Every TransD path projects the
-    entity rows per relation first (rank_link_prediction_transh, topk_entity_inference, transd_rel_scores)."""
-    check_transd_widths(model.ent_emb_dim, model.rel_emb_dim)
-    f = ModelSpec._f32
-    ent, rel_dim = f(model.ent_emb.weight), model.rel_emb_dim
-    spec = ModelSpec(_lib.TRANSE_L2, rel_dim, model.n_ent, model.n_rel, ent[:, :rel_dim].contiguous(), None,
-                     f(model.rel_emb.weight), None)
-    spec.projection = "TransDModel"
-    spec.ent_full, spec.ent_dim = ent, model.ent_emb_dim
-    spec.rel_proj = f(model.rel_proj_vect.weight)
-    spec.scalars = None
-    if ent.is_cuda:      # a model on the host is refused by shard_spec, next
-        spec.scalars = (engine or default_engine()).transd_entity_scalars(ent, f(model.ent_proj_vect.weight))
-    return spec
+class TransDSpec(ProjectedSpec):
+    """TransD (translation.py:518-536), read at width rel_emb_dim: ent0 holds the first rel_emb_dim coordinates
+    of the raw ent_emb rows (the rows relation prediction projects on the fly), rel0 the raw rel_emb table.  It
+    also holds the raw ent_emb table (``ent_full``, its width ``ent_dim``), the raw rel_proj_vect table
+    (``rel_proj``) and every entity's scalar s_e = (ent_proj_vect[e] * ent_emb[e]).sum() (``scalars``), computed
+    once here: it does not depend on the relation."""
+
+    def __init__(self, model):
+        check_transd_widths(model.ent_emb_dim, model.rel_emb_dim)
+        f = ModelSpec._f32
+        ent, rel_dim = f(model.ent_emb.weight), model.rel_emb_dim
+        super().__init__(model, rel_dim, ent[:, :rel_dim].contiguous(), f(model.rel_emb.weight))
+        self.ent_full, self.ent_dim = ent, model.ent_emb_dim
+        self.rel_proj = f(model.rel_proj_vect.weight)
+        # a model on the host has none: shard_spec refuses it next
+        self.scalars = (default_engine().transd_entity_scalars(ent, f(model.ent_proj_vect.weight))
+                        if ent.is_cuda else None)
+
+    def project(self, engine, rel, out):
+        return engine.transd_project(self, rel, out)
+
+    def rel_scores(self, engine, hrows, trows, h_idx, t_idx):
+        return engine.transd_rel_scores(self, hrows, trows, self.scalars[h_idx], self.scalars[t_idx])
 
 
-def _is_projected_spec(spec):
-    return getattr(spec, "projection", None) is not None
+#: the models ranked on per-relation projected entity tables: class name (this package's or, duck-typed, the
+#: reference's) -> spec
+PROJECTED_SPECS = {"TransHModel": TransHSpec, "TransDModel": TransDSpec}
 
 
-def _refuse_projected_shard(spec, shard):
-    """Sharded TransH / TransD calls are not supported: raised on every rank, before any collective."""
-    if _is_projected_spec(spec) and shard is not None:
-        raise NotImplementedError("%s does not support shard= (EntityShard / QueryShard)" % spec.projection)
-
-
-def project_relation(engine, spec, rel, out):
-    """out (n_rows, spec.dim) <- the entity rows of a TransH / TransD spec projected for relation ``rel``."""
-    if spec.projection == "TransDModel":
-        return engine.transd_project(spec, rel, out)
-    return engine.transh_project(spec, rel, out)
+def refuse_projected_shard(name, shard):
+    """A TransH / TransD model (``name``: its class name) takes no shard=: raised on every rank, before any
+    device work or collective."""
+    if shard is not None and name in PROJECTED_SPECS:
+        raise NotImplementedError("%s does not support shard= (EntityShard / QueryShard)" % name)
 
 
 def _ptr(t):
@@ -488,7 +483,7 @@ class CudaEngine:
         return scores
 
     def transh_project(self, spec, rel, out):
-        """out (n_rows, dim) <- the entity rows of ``spec`` (transh_spec) projected on the hyperplane of
+        """out (n_rows, dim) <- the entity rows of ``spec`` (TransHSpec) projected on the hyperplane of
         relation ``rel`` (kge_transh_project, translation.py:279-281)."""
         _need_cuda(spec.ent0, out)
         _lib.check(self.lib.kge_transh_project(_ptr(spec.ent0), _ptr(spec.norm_vect[rel]), spec.n_rows, spec.dim,
@@ -519,7 +514,7 @@ class CudaEngine:
         return s
 
     def transd_project(self, spec, rel, out):
-        """out (n_rows, rel_dim) <- the entity rows of ``spec`` (transd_spec) projected for relation ``rel``
+        """out (n_rows, rel_dim) <- the entity rows of ``spec`` (TransDSpec) projected for relation ``rel``
         (kge_transd_project, translation.py:646)."""
         _need_cuda(spec.ent_full, out)
         _lib.check(self.lib.kge_transd_project(_ptr(spec.ent_full), spec.ent_dim, _ptr(spec.scalars),
@@ -812,14 +807,11 @@ def shard_spec(model, shard=None, who="evaluate", n=None, build=ModelSpec.from_m
     """The ModelSpec the engine reads for ``model`` (``build(model)``) under ``shard``, after the shard's
     argument checks: under an EntityShard with local storage the model holds entity rows [lo, hi) and its
     row 0 is entity lo (_check_table); a QueryShard must cover ``n`` facts, when ``n`` is given.  The
-    checks come first, then the model must be on a CUDA device.  TransH / TransD: no shard, and transh_spec /
-    transd_spec."""
-    name = projected_model(model)
-    if name is not None:
-        if shard is not None:
-            raise NotImplementedError("%s does not support shard= (EntityShard / QueryShard)" % name)
-        build = transh_spec if name == "TransHModel" else transd_spec
-    spec = build(model)
+    checks come first, then the model must be on a CUDA device.  TransH / TransD: no shard, and the spec of
+    PROJECTED_SPECS."""
+    name = type(model).__name__
+    refuse_projected_shard(name, shard)
+    spec = PROJECTED_SPECS.get(name, build)(model)
     if isinstance(shard, EntityShard):
         if shard.local_storage:
             spec = ModelSpec(spec.code, spec.dim, shard.n_ent, spec.n_rel, spec.ent0, spec.ent1, spec.rel0,
@@ -880,8 +872,8 @@ def rank_link_prediction(spec, h_idx, t_idx, r_idx, filt_tail, filt_head, shard=
     """
     engine = engine or default_engine()
     n = h_idx.shape[0]
-    if _is_projected_spec(spec):
-        raise ValueError("a %s spec is ranked by rank_link_prediction_transh" % spec.projection[:-len("Model")])
+    if isinstance(spec, ProjectedSpec):
+        raise ValueError("a %s spec is ranked by rank_link_prediction_projected" % spec.name[:-len("Model")])
     table = spec
     if shard is not None:
         _check_table(spec, shard)
@@ -985,29 +977,36 @@ def relation_groups(r_idx, n_rel):
     return order, order_host, groups
 
 
-def rank_link_prediction_transh(spec, h_idx, t_idx, r_idx, groups, filt_tail, filt_head, engine=None,
-                                chunk=DEFAULT_CHUNK, exact=False, sync=True):
-    """rank_link_prediction for TransH and TransD (transh_spec, transd_spec): the facts come sorted by relation,
-    ``groups`` the (relation, lo, hi) of relation_groups.  Per relation, the entity table is projected into one
-    reused (n_rows, spec.dim) buffer (project_relation: kge_transh_project or kge_transd_project) and the group
-    is ranked on it as TransE-L2 -- tail queries fl(P_r(h) + r) against the projected candidates, head
-    candidates (P_r(c) + r) - P_r(t), exactly the reference's arithmetic on its projected_entities
+def _projected_groups(spec, groups, engine):
+    """The relation-grouped loop of a ProjectedSpec: for every (relation, lo, hi) of ``groups`` (relation_groups),
+    the entity table projected for the relation (``spec.project``) into one (n_rows, dim) buffer, allocated once,
+    then (relation, lo, hi, the buffer's TransE-L2 spec)."""
+    proj = torch.empty((spec.n_rows, spec.dim), dtype=torch.float32, device=spec.ent0.device)
+    table = ModelSpec(spec.code, spec.dim, spec.n_ent, spec.n_rel, proj, None, spec.rel0, None)
+    for rel, lo, hi in groups:
+        spec.project(engine, rel, proj)
+        yield rel, lo, hi, table
+
+
+def rank_link_prediction_projected(spec, h_idx, t_idx, r_idx, groups, filt_tail, filt_head, engine=None,
+                                   chunk=DEFAULT_CHUNK, exact=False, sync=True):
+    """rank_link_prediction for TransH and TransD (ProjectedSpec): the facts come sorted by relation, ``groups``
+    the (relation, lo, hi) of relation_groups.  Per relation, the entity table is projected (_projected_groups)
+    and the group is ranked on it as TransE-L2 -- tail queries fl(P_r(h) + r) against the projected candidates,
+    head candidates (P_r(c) + r) - P_r(t), exactly the reference's arithmetic on its projected_entities
     (interfaces.py:249-260) -- with the filter CSR rows of the group.  The tensor-core image of the buffer is
     rebuilt per relation, without the cache.  Arguments and result as rank_link_prediction's (no shard)."""
     engine = engine or default_engine()
     n = h_idx.shape[0]
     dev = spec.ent0.device
     with _device_guard(dev):
-        proj = torch.empty((spec.n_rows, spec.dim), dtype=torch.float32, device=dev)
         ranks = [torch.empty(n, dtype=torch.int64, device=dev) for _ in range(4)]
         filts = [f() if callable(f) else f for f in (filt_tail, filt_head)]
         ranges = [(lo, hi) for _, lo, hi in groups]
         parts = [_csr_cut(f, ranges) for f in filts]    # one device -> host read per CSR
         flags = []
-        for (rel, lo, hi), ft, fh in zip(groups, parts[0], parts[1]):
-            project_relation(engine, spec, rel, proj)
-            pspec = ModelSpec(spec.code, spec.dim, spec.n_ent, spec.n_rel, proj, None, spec.rel0, None)
-            lazy = rank_link_prediction(pspec, h_idx[lo:hi], t_idx[lo:hi], r_idx[lo:hi], ft, fh, engine=engine,
+        for (_, lo, hi, table), ft, fh in zip(_projected_groups(spec, groups, engine), parts[0], parts[1]):
+            lazy = rank_link_prediction(table, h_idx[lo:hi], t_idx[lo:hi], r_idx[lo:hi], ft, fh, engine=engine,
                                         chunk=chunk, exact=exact, sync=False, tc_cache=False)
             for out, x in zip(ranks, lazy.ranks):
                 out[lo:hi] = x
@@ -1016,8 +1015,8 @@ def rank_link_prediction_transh(spec, h_idx, t_idx, r_idx, groups, filt_tail, fi
         overflow = torch.cat(flags).sum() if flags else None
 
     def redo():
-        return rank_link_prediction_transh(spec, h_idx, t_idx, r_idx, groups, filts[0], filts[1], engine=engine,
-                                           chunk=chunk, exact=True)
+        return rank_link_prediction_projected(spec, h_idx, t_idx, r_idx, groups, filts[0], filts[1], engine=engine,
+                                              chunk=chunk, exact=True)
 
     lazy = LazyRanks(tuple(ranks), overflow, redo)
     return lazy.get() if sync else lazy
@@ -1045,17 +1044,14 @@ def _dense_relations(spec):
     """Models whose relation case is a dense (n, n_rel) score matrix rather than a scan over a candidate table:
     RESCAL (per-fact vectors h^T M_c, bilinear.py:115-121), TransH and TransD (rows projected per relation,
     interfaces.py:261-272)."""
-    return spec.code == _lib.RESCAL or _is_projected_spec(spec)
+    return spec.code == _lib.RESCAL or isinstance(spec, ProjectedSpec)
 
 
 def _dense_rel_scores(engine, spec, hrows, trows, h_idx=None, t_idx=None):
     """(n, n_rel) relation scores of the facts (hrows, ?, trows), hrows / trows (n, dim), for _dense_relations.
     TransD also reads the scalars of the facts' entities h_idx / t_idx (unsharded calls only)."""
-    projection = getattr(spec, "projection", None)
-    if projection == "TransDModel":
-        return engine.transd_rel_scores(spec, hrows, trows, spec.scalars[h_idx], spec.scalars[t_idx])
-    if projection == "TransHModel":
-        return engine.transh_rel_scores(spec, hrows, trows)
+    if isinstance(spec, ProjectedSpec):
+        return spec.rel_scores(engine, hrows, trows, h_idx, t_idx)
     return engine.rescal_rel_scores(spec, hrows, trows)
 
 
@@ -1080,7 +1076,8 @@ def rank_relation_prediction(spec, h_idx, t_idx, r_idx, filt, directed=True, eng
     engine = engine or default_engine()
     n = h_idx.shape[0]
     dev = spec.ent0.device
-    _refuse_projected_shard(spec, shard)
+    if isinstance(spec, ProjectedSpec):
+        refuse_projected_shard(spec.name, shard)
     rspec = None if _dense_relations(spec) else relation_spec(spec)   # unsupported models raise here
     if isinstance(shard, EntityShard):
         _check_table(spec, shard)
@@ -1259,9 +1256,9 @@ def topk_entity_inference(spec, ents, rels, side, k, mask=None, shard=None, engi
     engine = engine or default_engine()
     n = ents.shape[0]
     dev = spec.ent0.device
-    _refuse_projected_shard(spec, shard)
-    if _is_projected_spec(spec):
-        return _topk_entity_transh(spec, ents, rels, side, k, mask, engine, chunk)
+    if isinstance(spec, ProjectedSpec):
+        refuse_projected_shard(spec.name, shard)
+        return _topk_entity_projected(spec, ents, rels, side, k, mask, engine, chunk)
     if shard is not None and shard.world > 1:
         _check_sharded_k(k, spec.n_ent)
     if isinstance(shard, EntityShard):
@@ -1297,10 +1294,10 @@ def topk_entity_inference(spec, ents, rels, side, k, mask=None, shard=None, engi
         return _topk_chunks(n, spec.n_ent, k, topk_chunk, mask, dev, chunk)
 
 
-def _topk_entity_transh(spec, ents, rels, side, k, mask, engine, chunk):
+def _topk_entity_projected(spec, ents, rels, side, k, mask, engine, chunk):
     """topk_entity_inference for TransH and TransD: the queries grouped by relation (relation_groups), the entity
-    table projected per relation into one reused buffer and scanned as TransE-L2, as in
-    rank_link_prediction_transh."""
+    table projected per relation (_projected_groups) and scanned as TransE-L2, as in
+    rank_link_prediction_projected."""
     n = ents.shape[0]
     dev = spec.ent0.device
     _check_k(k, spec.n_rows)
@@ -1315,17 +1312,15 @@ def _topk_entity_transh(spec, ents, rels, side, k, mask, engine, chunk):
             sel = torch.repeat_interleave(offs[:-1][perm], lens[perm]) + (
                 torch.arange(int(new_offs[-1])) - torch.repeat_interleave(new_offs[:-1], lens[perm]))
             mask = (new_offs, ids[sel])
-        proj = torch.empty((spec.n_rows, spec.dim), dtype=torch.float32, device=dev)
         pred = torch.empty((n, k), dtype=torch.int64, device=dev)
         vals = torch.empty((n, k), dtype=torch.float32, device=dev)
-        for (rel, lo, hi), m in zip(groups, _csr_cut(mask, [(lo, hi) for _, lo, hi in groups])):
-            project_relation(engine, spec, rel, proj)
-            pspec = ModelSpec(spec.code, spec.dim, spec.n_ent, spec.n_rel, proj, None, spec.rel0, None)
-            packed = engine.pack(pspec)
+        masks = _csr_cut(mask, [(lo, hi) for _, lo, hi in groups])
+        for (_, lo, hi, table), m in zip(_projected_groups(spec, groups, engine), masks):
+            packed = engine.pack(table)
 
             def topk_chunk(a, b, mm):
-                rows = engine.gather_rows(pspec, ents_s[lo + a:lo + b])
-                return engine.topk_side(pspec, packed, side, rows, rows, rels_s[lo + a:lo + b], k, mm)
+                rows = engine.gather_rows(table, ents_s[lo + a:lo + b])
+                return engine.topk_side(table, packed, side, rows, rows, rels_s[lo + a:lo + b], k, mm)
 
             pred[lo:hi], vals[lo:hi] = _topk_chunks(hi - lo, spec.n_rows, k, topk_chunk, m, dev, chunk)
         out_pred, out_vals = torch.empty_like(pred), torch.empty_like(vals)
@@ -1344,7 +1339,8 @@ def topk_relation_inference(spec, e1, e2, k, mask=None, shard=None, engine=None,
     engine = engine or default_engine()
     n = e1.shape[0]
     dev = spec.ent0.device
-    _refuse_projected_shard(spec, shard)
+    if isinstance(spec, ProjectedSpec):
+        refuse_projected_shard(spec.name, shard)
     if isinstance(shard, QueryShard) and shard.world > 1:
         _check_sharded_k(k, spec.n_rel)
         _check_queries(shard, n)

@@ -9,9 +9,10 @@ import torch
 
 from . import _lib
 from .data import dict_filter_csr, filter_csr
-from .engine import (DEFAULT_CHUNK, EntityShard, ModelSpec, QueryShard, _by_query_slices, _check_table,
-                     default_engine, projected_model, rank_link_prediction, rank_link_prediction_transh,
-                     rank_relation_prediction, relation_groups, score_triples_entity_sharded, shard_spec)
+from .engine import (DEFAULT_CHUNK, EntityShard, ModelSpec, ProjectedSpec, QueryShard, _by_query_slices,
+                     _check_table, default_engine, rank_link_prediction, rank_link_prediction_projected,
+                     rank_relation_prediction, refuse_projected_shard, relation_groups, score_triples_entity_sharded,
+                     shard_spec)
 from .exceptions import NotYetEvaluatedError
 
 
@@ -83,8 +84,8 @@ class LinkPredictionEvaluator(object):
         t_d = tails.to(dev, non_blocking=True)
         r_d = rels.to(dev, non_blocking=True)
         stats = {"h2d_bytes": 8 * 3 * n_here, "d2h_bytes": 8 * (4 * kg.n_facts + 1)}
-        transh = projected_model(self.model) is not None
-        if transh:
+        projected = isinstance(spec, ProjectedSpec)
+        if projected:
             # TransH and TransD rank the facts relation by relation: everything below, filter sets included, runs on
             # the facts sorted by relation; the ranks go back to fact order at the end
             order, order_host, groups = relation_groups(r_d, spec.n_rel)
@@ -128,16 +129,16 @@ class LinkPredictionEvaluator(object):
             csr_tail = from_dicts("tail", heads, rels, tails)
             csr_head = from_dicts("head", tails, rels, heads)
         engine = default_engine()
-        if transh:
-            lazy = rank_link_prediction_transh(spec, h_d, t_d, r_d, groups, csr_tail, csr_head, engine=engine,
-                                               chunk=DEFAULT_CHUNK, sync=False)
+        if projected:
+            lazy = rank_link_prediction_projected(spec, h_d, t_d, r_d, groups, csr_tail, csr_head, engine=engine,
+                                                  chunk=DEFAULT_CHUNK, sync=False)
         else:
             lazy = rank_link_prediction(spec, h_d, t_d, r_d, csr_tail, csr_head, shard=eshard,
                                         engine=engine, chunk=DEFAULT_CHUNK, sync=False)
 
         def to_host(ranks, flag):
             flag = torch.zeros(1, dtype=torch.int64, device=dev) if flag is None else flag.long().view(1)
-            if transh:         # back to fact order
+            if projected:      # back to fact order
                 unsorted = [torch.empty_like(x) for x in ranks]
                 for u, x in zip(unsorted, ranks):
                     u[order] = x
@@ -326,8 +327,7 @@ class TripletClassificationEvaluator(object):
 
     def __init__(self, model, kg_val, kg_test, *, shard=None):
         from .sampling import PositionalNegativeSampler
-        if shard is not None and projected_model(model) is not None:
-            raise NotImplementedError("%s does not support shard= (EntityShard / QueryShard)" % projected_model(model))
+        refuse_projected_shard(type(model).__name__, shard)
         self.model = model
         self.kg_val = kg_val
         self.kg_test = kg_test

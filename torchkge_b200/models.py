@@ -265,7 +265,32 @@ class TransEModel(TranslationModel):
         return h, t, r, cands
 
 
-class TransHModel(TranslationModel):
+class ProjectedTranslationModel(TranslationModel):
+    """TransH and TransD: TransE-L2 between per-relation projections of h and t, ranked here without the
+    reference's (n_rel, n_ent, width) ``projected_entities`` cache.  A subclass names that width in
+    ``cand_width``, for the error messages."""
+
+    def inference_prepare_candidates(self, h_idx, t_idx, r_idx, entities=True):
+        raise NotImplementedError(
+            "%s has no inference_prepare_candidates: the reference's candidates are a per-row "
+            "(b, n_ent, %s) tensor of projected entities.  Use LinkPredictionEvaluator, "
+            "RelationPredictionEvaluator, EntityInference or RelationInference, which project on the GPU."
+            % (type(self).__name__, self.cand_width))
+
+    def inference_scoring_function(self, h, t, r):
+        raise NotImplementedError(
+            "%s has no inference_scoring_function: use LinkPredictionEvaluator, "
+            "RelationPredictionEvaluator, EntityInference or RelationInference." % type(self).__name__)
+
+    def _load_from_state_dict(self, state_dict, prefix, local_metadata, strict, missing_keys, unexpected_keys,
+                              error_msgs):
+        # a reference checkpoint carries its projection cache: not a parameter here
+        state_dict.pop(prefix + "projected_entities", None)
+        super()._load_from_state_dict(state_dict, prefix, local_metadata, strict, missing_keys, unexpected_keys,
+                                      error_msgs)
+
+
+class TransHModel(ProjectedTranslationModel):
     """TransH (Wang et al. 2014) -- torchkge/models/translation.py:128-284: TransE-L2 between the
     projections of h and t on a relation-specific hyperplane of normal vector ``norm_vect``.
 
@@ -281,6 +306,8 @@ class TransHModel(TranslationModel):
     ``LinkPredictionEvaluator``, ``RelationPredictionEvaluator``, ``EntityInference`` or
     ``RelationInference``.  Out of scope: the fused training step and ``shard=``.
     """
+
+    cand_width = "emb_dim"
 
     def __init__(self, emb_dim, n_entities, n_relations):
         super().__init__(n_entities, n_relations, dissimilarity_type='L2')
@@ -311,26 +338,8 @@ class TransHModel(TranslationModel):
         self.normalize_parameters()
         return self.ent_emb.weight.data, self.rel_emb.weight.data, self.norm_vect.weight.data
 
-    def inference_prepare_candidates(self, h_idx, t_idx, r_idx, entities=True):
-        raise NotImplementedError(
-            "TransHModel has no inference_prepare_candidates: the reference's candidates are a per-row "
-            "(b, n_ent, emb_dim) tensor of projected entities.  Use LinkPredictionEvaluator, "
-            "RelationPredictionEvaluator, EntityInference or RelationInference, which project on the GPU.")
 
-    def inference_scoring_function(self, h, t, r):
-        raise NotImplementedError(
-            "TransHModel has no inference_scoring_function: use LinkPredictionEvaluator, "
-            "RelationPredictionEvaluator, EntityInference or RelationInference.")
-
-    def _load_from_state_dict(self, state_dict, prefix, local_metadata, strict, missing_keys, unexpected_keys,
-                              error_msgs):
-        # a reference checkpoint carries its (n_rel, n_ent, emb_dim) projection cache: not a parameter here
-        state_dict.pop(prefix + "projected_entities", None)
-        super()._load_from_state_dict(state_dict, prefix, local_metadata, strict, missing_keys, unexpected_keys,
-                                      error_msgs)
-
-
-class TransDModel(TranslationModel):
+class TransDModel(ProjectedTranslationModel):
     """TransD (Ji et al. 2015) -- torchkge/models/translation.py:461-652: TransE-L2 between the projections
     P_r(e) = (e . e_p) r_p + e[:rel_emb_dim] of h and t, with an entity projection vector e_p
     (``ent_proj_vect``, ent_emb_dim) and a relation projection vector r_p (``rel_proj_vect``, rel_emb_dim).
@@ -349,6 +358,8 @@ class TransDModel(TranslationModel):
     ``LinkPredictionEvaluator``, ``RelationPredictionEvaluator``, ``EntityInference`` or
     ``RelationInference``.  Out of scope: the fused training step and ``shard=``.
     """
+
+    cand_width = "rel_emb_dim"
 
     def __init__(self, ent_emb_dim, rel_emb_dim, n_entities, n_relations):
         super().__init__(n_entities, n_relations, dissimilarity_type='L2')
@@ -384,24 +395,6 @@ class TransDModel(TranslationModel):
         self.normalize_parameters()
         return self.ent_emb.weight.data, self.rel_emb.weight.data, \
             self.ent_proj_vect.weight.data, self.rel_proj_vect.weight.data
-
-    def inference_prepare_candidates(self, h_idx, t_idx, r_idx, entities=True):
-        raise NotImplementedError(
-            "TransDModel has no inference_prepare_candidates: the reference's candidates are a per-row "
-            "(b, n_ent, rel_emb_dim) tensor of projected entities.  Use LinkPredictionEvaluator, "
-            "RelationPredictionEvaluator, EntityInference or RelationInference, which project on the GPU.")
-
-    def inference_scoring_function(self, h, t, r):
-        raise NotImplementedError(
-            "TransDModel has no inference_scoring_function: use LinkPredictionEvaluator, "
-            "RelationPredictionEvaluator, EntityInference or RelationInference.")
-
-    def _load_from_state_dict(self, state_dict, prefix, local_metadata, strict, missing_keys, unexpected_keys,
-                              error_msgs):
-        # a reference checkpoint carries its (n_rel, n_ent, rel_emb_dim) projection cache: not a parameter here
-        state_dict.pop(prefix + "projected_entities", None)
-        super()._load_from_state_dict(state_dict, prefix, local_metadata, strict, missing_keys, unexpected_keys,
-                                      error_msgs)
 
 
 class DistMultModel(BilinearModel):

@@ -10,8 +10,8 @@ import struct
 import torch
 
 from . import _lib
-from .engine import (EntityShard, ModelSpec, QueryShard, _check_table, _device_guard, _exchanged_rows, _plane_ptrs,
-                     _ptr, _stream, check_transd_widths, default_engine, projected_model)
+from .engine import (PROJECTED_SPECS, EntityShard, ModelSpec, QueryShard, _check_table, _device_guard,
+                     _exchanged_rows, _plane_ptrs, _ptr, _stream, check_transd_widths, default_engine)
 
 
 def _param_tensors(model, code):
@@ -125,12 +125,14 @@ def score_triples(model, h_idx, t_idx, r_idx):
     return _ScoreTriples.apply(code, _kernel_dim(model, code), h_idx, t_idx, r_idx, ent0, ent1, rel0, rel1)
 
 
-class _TransHScoreTriples(torch.autograd.Function):
-    """TransH's scoring_function on kge_transh_score_triples_fwd / _bwd (translation.py:183-202)."""
+class _ProjectedScoreTriples(torch.autograd.Function):
+    """TransH's or TransD's scoring_function on kge_<prefix>_score_triples_fwd / _bwd (translation.py:183-202,
+    538-568): ``prefix`` "transh" or "transd", ``dims`` the widths and ``tables`` the raw tables, in the order of
+    the C entry points."""
 
     @staticmethod
-    def forward(ctx, dim, h, t, r, ent, rel, norm_vect):
-        tables = [x.detach().contiguous() for x in (ent, rel, norm_vect)]
+    def forward(ctx, prefix, dims, h, t, r, *tables):
+        tables = [x.detach().contiguous() for x in tables]
         for x in tables:
             if x.dtype != torch.float32:
                 raise TypeError("embedding tables must be float32, got %s" % x.dtype)
@@ -138,10 +140,10 @@ class _TransHScoreTriples(torch.autograd.Function):
         dev = tables[0].device
         h, t, r = _idx(h, dev), _idx(t, dev), _idx(r, dev)
         out = torch.empty(h.shape[0], dtype=torch.float32, device=dev)
-        _lib.check(_lib.load().kge_transh_score_triples_fwd(*(_ptr(x) for x in tables), dim, _ptr(h), _ptr(t),
-                                                            _ptr(r), h.shape[0], _ptr(out), _stream(dev)),
-                   "kge_transh_score_triples_fwd")
-        ctx.dim = dim
+        name = "kge_%s_score_triples_fwd" % prefix
+        _lib.check(getattr(_lib.load(), name)(*(_ptr(x) for x in tables), *dims, _ptr(h), _ptr(t), _ptr(r),
+                                              h.shape[0], _ptr(out), _stream(dev)), name)
+        ctx.prefix, ctx.dims = prefix, dims
         ctx.save_for_backward(h, t, r, *tables)
         return out
 
@@ -150,58 +152,27 @@ class _TransHScoreTriples(torch.autograd.Function):
         h, t, r, *tables = ctx.saved_tensors
         grads = [torch.zeros_like(x) for x in tables]
         gout = gout.contiguous().float()
-        _lib.check(_lib.load().kge_transh_score_triples_bwd(*(_ptr(x) for x in tables), *(_ptr(g) for g in grads),
-                                                            ctx.dim, _ptr(h), _ptr(t), _ptr(r), h.shape[0],
-                                                            _ptr(gout), _stream(h.device)),
-                   "kge_transh_score_triples_bwd")
-        return (None, None, None, None, *grads)
+        name = "kge_%s_score_triples_bwd" % ctx.prefix
+        _lib.check(getattr(_lib.load(), name)(*(_ptr(x) for x in tables), *(_ptr(g) for g in grads), *ctx.dims,
+                                              _ptr(h), _ptr(t), _ptr(r), h.shape[0], _ptr(gout), _stream(h.device)),
+                   name)
+        return (None, None, None, None, None, *grads)
 
 
 def score_triples_transh(model, h_idx, t_idx, r_idx):
     """TransH's ``scoring_function(h_idx, t_idx, r_idx)`` -> (n,) float scores, differentiable with respect
     to ent_emb, rel_emb and norm_vect."""
-    return _TransHScoreTriples.apply(model.emb_dim, h_idx, t_idx, r_idx, model.ent_emb.weight,
-                                     model.rel_emb.weight, model.norm_vect.weight)
-
-
-class _TransDScoreTriples(torch.autograd.Function):
-    """TransD's scoring_function on kge_transd_score_triples_fwd / _bwd (translation.py:538-568)."""
-
-    @staticmethod
-    def forward(ctx, ent_dim, rel_dim, h, t, r, ent, rel, ent_proj, rel_proj):
-        tables = [x.detach().contiguous() for x in (ent, rel, ent_proj, rel_proj)]
-        for x in tables:
-            if x.dtype != torch.float32:
-                raise TypeError("embedding tables must be float32, got %s" % x.dtype)
-        _check_cuda(tables[0], h, t, r)
-        dev = tables[0].device
-        h, t, r = _idx(h, dev), _idx(t, dev), _idx(r, dev)
-        out = torch.empty(h.shape[0], dtype=torch.float32, device=dev)
-        _lib.check(_lib.load().kge_transd_score_triples_fwd(*(_ptr(x) for x in tables), ent_dim, rel_dim, _ptr(h),
-                                                            _ptr(t), _ptr(r), h.shape[0], _ptr(out), _stream(dev)),
-                   "kge_transd_score_triples_fwd")
-        ctx.dims = (ent_dim, rel_dim)
-        ctx.save_for_backward(h, t, r, *tables)
-        return out
-
-    @staticmethod
-    def backward(ctx, gout):
-        h, t, r, *tables = ctx.saved_tensors
-        grads = [torch.zeros_like(x) for x in tables]
-        gout = gout.contiguous().float()
-        _lib.check(_lib.load().kge_transd_score_triples_bwd(*(_ptr(x) for x in tables), *(_ptr(g) for g in grads),
-                                                            *ctx.dims, _ptr(h), _ptr(t), _ptr(r), h.shape[0],
-                                                            _ptr(gout), _stream(h.device)),
-                   "kge_transd_score_triples_bwd")
-        return (None, None, None, None, None, *grads)
+    return _ProjectedScoreTriples.apply("transh", (model.emb_dim,), h_idx, t_idx, r_idx, model.ent_emb.weight,
+                                        model.rel_emb.weight, model.norm_vect.weight)
 
 
 def score_triples_transd(model, h_idx, t_idx, r_idx):
     """TransD's ``scoring_function(h_idx, t_idx, r_idx)`` -> (n,) float scores, differentiable with respect
     to ent_emb, rel_emb, ent_proj_vect and rel_proj_vect."""
     check_transd_widths(model.ent_emb_dim, model.rel_emb_dim)
-    return _TransDScoreTriples.apply(model.ent_emb_dim, model.rel_emb_dim, h_idx, t_idx, r_idx, model.ent_emb.weight,
-                                     model.rel_emb.weight, model.ent_proj_vect.weight, model.rel_proj_vect.weight)
+    return _ProjectedScoreTriples.apply("transd", (model.ent_emb_dim, model.rel_emb_dim), h_idx, t_idx, r_idx,
+                                        model.ent_emb.weight, model.rel_emb.weight, model.ent_proj_vect.weight,
+                                        model.rel_proj_vect.weight)
 
 
 class _MarginLoss(torch.autograd.Function):
@@ -559,8 +530,8 @@ def _positional_csr(positional, n_rel, dev):
 
 def refuse_projected_fused_step(model):
     """TransH and TransD have per-triple kernels (score_triples_transh / _transd) but no fused training step."""
-    name = projected_model(model)
-    if name is not None:
+    name = type(model).__name__
+    if name in PROJECTED_SPECS:
         raise NotImplementedError("%s has no fused training step: train it with model(h, t, r, nh, nt), "
                                   "a loss and backward()" % name)
 
